@@ -378,6 +378,14 @@ namespace {
 const int TPB = 128;
 inline unsigned nblk(u64 n, int tpb = TPB) { return (unsigned)((n + tpb - 1) / tpb); }
 
+// one pass of the export encoder over NOB output blocks, in the build that is faster for that many (k_export.cuh)
+void launch_exp_encode(cudaStream_t st, DocInfo* docs, u64 NOB, const ExportTables& xt, XBlock* xb, u32* xscratch, u8* out,
+                       int pass) {
+    if (!NOB) return;
+    if (NOB >= LB_XENC_BOUNDED_MIN_BLOCKS) LB_LAUNCH(k_exp_encode<1>, nblk(NOB, 64), 64, 0, st, docs, NOB, xt, xb, xscratch, out, pass);
+    else LB_LAUNCH(k_exp_encode<0>, nblk(NOB, 64), 64, 0, st, docs, NOB, xt, xb, xscratch, out, pass);
+}
+
 // LB_PHASE_TRACE=1: host wall clock between named points (each one synchronises the stream: diagnosis only)
 void trace_point(lb_batch* b, const char* name);
 void mark(lb_batch* b) {
@@ -806,7 +814,7 @@ void pipeline(lb_batch* b) {
         u32* xscratch = dv.alloc<u32>(NSCR + 1);
         trace_point(b, "store+sizes");
         LB_LAUNCH(k_exp_list, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb);
-        if (NOB) { if (NOB >= LB_XENC_BOUNDED_MIN_BLOCKS) LB_LAUNCH(k_exp_encode<1>, nblk(NOB, 64), 64, 0, st, b->d_docs, NOB, xt, xb, xscratch, (u8*)nullptr, 0); else LB_LAUNCH(k_exp_encode<0>, nblk(NOB, 64), 64, 0, st, b->d_docs, NOB, xt, xb, xscratch, (u8*)nullptr, 0); }
+        launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, nullptr, 0);
         LB_LAUNCH(k_exp_layout, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb, d_tmp_a);
         tm.kernel_launches += 3;
         trace_point(b, "encode pass 0");
@@ -816,7 +824,7 @@ void pipeline(lb_batch* b) {
         trace_point(b, "layout scan + size d2h");
         b->d_export = dv.alloc<u8>(XT + 16, true);
         trace_point(b, "export buffer alloc+zero");
-        if (NOB) { if (NOB >= LB_XENC_BOUNDED_MIN_BLOCKS) LB_LAUNCH(k_exp_encode<1>, nblk(NOB, 64), 64, 0, st, b->d_docs, NOB, xt, xb, xscratch, b->d_export, 1); else LB_LAUNCH(k_exp_encode<0>, nblk(NOB, 64), 64, 0, st, b->d_docs, NOB, xt, xb, xscratch, b->d_export, 1); }
+        launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, b->d_export, 1);
         trace_point(b, "encode pass 1 kernel");
         LB_LAUNCH(k_exp_finish, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, xt, b->d_export);
         tm.kernel_launches += 2;
@@ -1032,12 +1040,12 @@ lb_status export_from(lb_batch* b, size_t doc, const lb_id_span* from, size_t n_
         XBlock* xb = dv.alloc<XBlock>(NOB + 1);
         u32* xscratch = dv.alloc<u32>(NSCR + 1);
         LB_LAUNCH(k_exp_list, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb);
-        if (NOB) { if (NOB >= LB_XENC_BOUNDED_MIN_BLOCKS) LB_LAUNCH(k_exp_encode<1>, nblk(NOB, 64), 64, 0, st, b->d_docs, NOB, xt, xb, xscratch, (u8*)nullptr, 0); else LB_LAUNCH(k_exp_encode<0>, nblk(NOB, 64), 64, 0, st, b->d_docs, NOB, xt, xb, xscratch, (u8*)nullptr, 0); }
+        launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, nullptr, 0);
         LB_LAUNCH(k_exp_layout, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb, tmp_a);
         run_scans(b, {ScanJob{(const u8*)tmp_a, (u8*)xdoc + offsetof(XDoc, exp_off), 4, sizeof(XDoc), D}});
         u64 XT = d2h_one(b, &xdoc[D].exp_off);
         u8* d_out = dv.alloc<u8>(XT + 16, true);
-        if (NOB) { if (NOB >= LB_XENC_BOUNDED_MIN_BLOCKS) LB_LAUNCH(k_exp_encode<1>, nblk(NOB, 64), 64, 0, st, b->d_docs, NOB, xt, xb, xscratch, d_out, 1); else LB_LAUNCH(k_exp_encode<0>, nblk(NOB, 64), 64, 0, st, b->d_docs, NOB, xt, xb, xscratch, d_out, 1); }
+        launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, d_out, 1);
         LB_LAUNCH(k_exp_finish, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, xt, d_out);
         XDoc x = d2h_one(b, xdoc + doc);
         lb_status rc = LB_OK;

@@ -712,12 +712,7 @@ __global__ void k_block_decode(const u8* __restrict__ bytes, BlockInfo* __restri
     if (err) decode_block_fail(bi, i, t, blocks, err);
 }
 // thread per block, one column at a time
-#ifdef LB_DCOLS_MINB
-__global__ void __launch_bounds__(64, LB_DCOLS_MINB) k_block_decode_cols(
-#else
-__global__ void k_block_decode_cols(
-#endif
-    const u8* __restrict__ bytes, BlockInfo* __restrict__ blocks, u64 n_blocks, Tables t) {
+__global__ void k_block_decode_cols(const u8* __restrict__ bytes, BlockInfo* __restrict__ blocks, u64 n_blocks, Tables t) {
     u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_blocks) return;
     BlockInfo bi = blocks[i];

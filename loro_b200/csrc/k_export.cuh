@@ -496,12 +496,7 @@ __device__ inline void segment_summaries(const ExportTables& t, const DocInfo& d
 
 // thread per change.  pass 0: per-row records, RleVec merge inside the change (XF_HEAD), segment count (XF_SEG marks
 // when no op has to be cut, a synthetic-row count otherwise).  pass 1 (split changes only): synthetic rows, summaries.
-#ifdef LB_XCHG_MINB
-__global__ void __launch_bounds__(64, LB_XCHG_MINB) k_exp_changes(
-#else
-__global__ void k_exp_changes(
-#endif
-    DocInfo* __restrict__ docs, u64 n_changes, ExportTables t, int pass) {
+__global__ void k_exp_changes(DocInfo* __restrict__ docs, u64 n_changes, ExportTables t, int pass) {
     u64 ch = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (ch >= n_changes) return;
     if (t.only_doc != 0xFFFFFFFFu && t.blocks[t.ch_block[ch]].doc != t.only_doc) return;
@@ -901,19 +896,14 @@ __global__ void k_exp_sizes(const DocInfo* __restrict__ docs, u32 n_docs, Export
 // are written (serde_columnar AnyRle state machine: maximal runs of >= 2 equal values become runs, the values
 // between them literal segments; a lone value is a literal of one).
 // The values come out of per-block scratch columns in global memory and every scan below is a chain of dependent
-// loads: with LB_XENC_LOOKAHEAD the scans
-// fetch four values at a time -- the loads are independent of each other and of the comparisons -- and consume them in
-// order.  Same segments, same bytes.
-#ifndef LB_XENC_LOOKAHEAD
-#define LB_XENC_LOOKAHEAD 1
-#endif
+// loads: the scans fetch four values at a time -- the loads are independent of each other and of the comparisons --
+// and consume them in order.
 template <class F, class W>
 __device__ inline void enc_anyrle(XSink& s, u32 n, F val, W wr) {
     u32 i = 0;
     while (i < n) {
         i64 v = val(i);
         u32 j = i;
-#if LB_XENC_LOOKAHEAD
         while (j + 1 < n) {
             const u32 base = j + 1, m = n - base < 4 ? n - base : 4;
             i64 w0 = val(base), w1 = m > 1 ? val(base + 1) : 0, w2 = m > 2 ? val(base + 2) : 0, w3 = m > 3 ? val(base + 3) : 0;
@@ -922,9 +912,6 @@ __device__ inline void enc_anyrle(XSink& s, u32 n, F val, W wr) {
             j += q;
             if (q < m) break;
         }
-#else
-        while (j + 1 < n && val(j + 1) == v) j++;
-#endif
         if (j > i) {
             s.zigzag((i64)(j - i + 1));
             wr(s, v);
@@ -933,7 +920,6 @@ __device__ inline void enc_anyrle(XSink& s, u32 n, F val, W wr) {
         }
         u32 k = i;
         i64 cur = v;
-#if LB_XENC_LOOKAHEAD
         while (k < n) {
             const u32 base = k + 1;
             if (base >= n) { k++; break; }
@@ -959,18 +945,6 @@ __device__ inline void enc_anyrle(XSink& s, u32 n, F val, W wr) {
             }
             for (; q < k; q++) wr(s, val(q));
         }
-#else
-        while (k < n) {
-            if (k + 1 < n) {
-                i64 nx = val(k + 1);
-                if (nx == cur) break;
-                cur = nx;
-            }
-            k++;
-        }
-        s.zigzag(-(i64)(k - i));
-        for (u32 q = i; q < k; q++) wr(s, val(q));
-#endif
         i = k;
     }
 }
@@ -1177,9 +1151,7 @@ __global__ void k_exp_posrank(const DocInfo* __restrict__ docs, u32 n_docs, Expo
 // against bounded: C3 at 4 k documents (~55 k blocks) 43.0 against 55.7 ms; C5 at 10 k documents (~160 k blocks) 145.9
 // against 130.8 ms; C3 at 40 k documents (~550 k blocks) 374.7 against 365.6 ms.  So batches of at least
 // LB_XENC_BOUNDED_MIN_BLOCKS output blocks take the bounded build.
-#ifndef LB_XENC_BOUNDED_MIN_BLOCKS
 #define LB_XENC_BOUNDED_MIN_BLOCKS 100000ull
-#endif
 __device__ __forceinline__ void exp_encode_body(
     const DocInfo* __restrict__ docs, u64 n_blocks, const ExportTables& t, XBlock* __restrict__ xb,
                              u32* __restrict__ scratch, u8* __restrict__ out, int pass) {

@@ -33,9 +33,7 @@
 #define LEAF_NONE 0xFFFFFFFFu
 #define ST_FUTURE 0x8000u
 #define SLOT_EMPTY ((u32)PEER_NONE | (1u << 16))   // no peer, never visible
-#ifndef LB_SEQ_NS
 #define LB_SEQ_NS 12          // internal nodes cached in shared memory per warp
-#endif
 #define LB_SEQ_WARPS 4        // warps (documents) per CTA
 
 // op record written by k_op_classify: x = kind | reversed << 3 | container << 4, y = counter, z = atoms,
@@ -782,8 +780,9 @@ __device__ __forceinline__ void seq_insert(const SeqPools& p, const Cx& c, u32 p
 // dependent 512-byte HBM read per op).  With LB_SEQ_PF, when 32 op records arrive, every lane
 // predicts the leaf ITS record will touch -- deletes from the atom -> leaf lookup they do anyway, inserts by walking the
 // shared-memory nodes on its own (lane-serial, the warp runs 32 descents at once) -- and asks L2 (or L1) for it.
-// It is off because the 32 resident warps per SM already overlap each other's leaf reads, and the predicted descents
-// add issue slots to every op.
+// The predicted descents add issue slots to every op.  On an H100, C3, prefetching delete targets only (=1) measured
+// about 0.2 % faster than off and inserts too (=2) about 6 % slower (DESIGN.md section 3); whether to turn =1 on is
+// left to an optimisation change.
 #ifndef LB_SEQ_PF
 #define LB_SEQ_PF 0           // 0: off, 1: delete targets only, 2: inserts too
 #endif
@@ -944,9 +943,7 @@ __device__ __noinline__ void emit_output(const SeqPools& p, const SeqTables& t, 
 // (single-peer documents do not skip the origin records, although nothing is ever concurrent in them: such a flag costs
 //  a register in every helper of a kernel that sits at its 64-register budget)
 // one warp per document, LB_SEQ_WARPS documents per CTA
-#ifndef LB_SEQ_MINB
 #define LB_SEQ_MINB 8         // 8 CTAs x 4 warps = 32 resident documents per SM (64 registers/thread)
-#endif
 __global__ void __launch_bounds__(32 * LB_SEQ_WARPS, LB_SEQ_MINB)
 k_seq_integrate(DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ SeqPools pools,
                 const __grid_constant__ SeqTables tables) {

@@ -76,15 +76,11 @@ struct Cur {
     __device__ __forceinline__ bool empty() const { return p >= end; }
     __device__ __forceinline__ u8 get() {
         if (p >= end) { err = 1; return 0; }
-#ifdef LB_CUR_UNBUFFERED
-        return *p++;
-#else
         const u8* a = (const u8*)((uintptr_t)p & ~(uintptr_t)7);
         if (a != bp) { buf = *(const u64*)a; bp = a; }
         u8 v = (u8)(buf >> (8 * (unsigned)((uintptr_t)p & 7)));
         p++;
         return v;
-#endif
     }
     __device__ __forceinline__ void skip(u64 n) {
         if (n > (u64)(end - p)) { err = 1; p = end; } else p += n;

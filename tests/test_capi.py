@@ -44,6 +44,28 @@ def test_sass_is_sm90a(lib):
     assert "sm_90a" in out and "sm_100" not in out, out
 
 
+def test_ctypes_structs_match_the_header(tmp_path):
+    """api.py's ctypes mirrors of lb_timings, lb_counters and lb_options have the size and field offsets the C compiler
+    gives the header's structs; a field api.py names that the header lacks fails the compile."""
+    import subprocess
+    from loro_b200 import api
+    structs = {"lb_timings": api._Timings, "lb_counters": api._Counters, "lb_options": api._Options}
+    want, lines = {}, ["#include <stddef.h>", "#include <stdio.h>", '#include "loro_b200.h"', "int main(void) {"]
+    for cname, py in structs.items():
+        want[cname] = ctypes.sizeof(py)
+        lines.append(f'    printf("{cname} %zu\\n", sizeof({cname}));')
+        for f, _ in py._fields_:
+            want[f"{cname}.{f}"] = getattr(py, f).offset
+            lines.append(f'    printf("{cname}.{f} %zu\\n", offsetof({cname}, {f}));')
+    src, exe = tmp_path / "layout.c", str(tmp_path / "layout")
+    src.write_text("\n".join(lines + ["    return 0;", "}"]) + "\n")
+    cc = subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-I" + os.path.join(ROOT, "include"), str(src), "-o", exe],
+                        capture_output=True, text=True)
+    assert cc.returncode == 0, cc.stderr
+    got = dict(line.split() for line in subprocess.check_output([exe], text=True).splitlines())
+    assert {k: int(v) for k, v in got.items()} == want
+
+
 def test_plain_c_caller_compiles_links_and_fails_loudly_without_a_device(lib, tmp_path):
     """include/loro_b200.h is plain C (no torch / C++ types in the signatures): examples/c/import_and_docset.c builds
     with -std=c99 -Wall -Wextra -Werror, links against the library and, without a CUDA device, gets LB_ERR_NO_DEVICE."""
