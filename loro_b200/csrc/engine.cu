@@ -378,7 +378,8 @@ namespace {
 const int TPB = 128;
 inline unsigned nblk(u64 n, int tpb = TPB) { return (unsigned)((n + tpb - 1) / tpb); }
 
-// one pass of the export encoder over NOB output blocks, in the build that is faster for that many (k_export.cuh)
+// one pass of the export encoder over NOB output blocks (pass 1 only touches the blocks that outgrew their staging
+// slot), in the build that is faster for that many (k_export.cuh)
 void launch_exp_encode(cudaStream_t st, DocInfo* docs, u64 NOB, const ExportTables& xt, XBlock* xb, u32* xscratch, u8* out,
                        int pass) {
     if (!NOB) return;
@@ -423,6 +424,55 @@ void run_scans(lb_batch* b, std::vector<ScanJob> jobs) {
 #define FIELD_JOB(base, type, in_field, out_field, count)                                              \
     ScanJob{(const u8*)(base) + offsetof(type, in_field), (u8*)(base) + offsetof(type, out_field), \
             sizeof(type), sizeof(type), (u64)(count)}
+
+// The encode end of phase 7, after the stores (k_exp_store) have cut every document's changes into output blocks;
+// shared by the batch's export and export_from.  Block list with scratch and staging slots, one encode pass into the
+// slots, layout (the lengths are exact, so are the offsets), the direct encode of the blocks that outgrew their slot
+// (only when there are any: their count comes back with the blob sizes), then the blobs assembled per document.
+// Returns the export buffer (*total bytes, document d's blob at xt.xdoc[d].exp_off).
+u8* export_encode(lb_batch* b, const ExportTables& xt, u64* total) {
+    Dev& dv = b->dev;
+    cudaStream_t st = dv.stream;
+    const u32 D = (u32)b->n_docs;
+    lb_timings& tm = b->timings;
+    u32* cnt = dv.alloc<u32>(3 * (u64)(D + 1));
+    u32 *n_a = cnt, *n_b = cnt + (D + 1), *n_c = cnt + 2 * (D + 1);
+    LB_LAUNCH(k_exp_sizes, nblk(D), TPB, 0, st, b->d_docs, D, xt, n_a, n_b, n_c);
+    tm.kernel_launches += 1;
+    run_scans(b, {ScanJob{(const u8*)n_a, (u8*)xt.xdoc + offsetof(XDoc, ob0), 4, sizeof(XDoc), D},
+                  ScanJob{(const u8*)n_b, (u8*)xt.xdoc + offsetof(XDoc, scratch0), 4, sizeof(XDoc), D},
+                  ScanJob{(const u8*)n_c, (u8*)xt.xdoc + offsetof(XDoc, stage0), 4, sizeof(XDoc), D}});
+    XDoc xtot = d2h_one(b, xt.xdoc + D);
+    const u64 NOB = xtot.ob0, NSCR = xtot.scratch0, NSTG = xtot.stage0;
+    XBlock* xb = dv.alloc<XBlock>(NOB + 1);
+    u32* xscratch = dv.alloc<u32>(NSCR + 1);
+    u8* xstage = dv.alloc<u8>(NSTG + 16);
+    const char* cap_env = getenv("LB_EXPORT_STAGE_CAP");   // testing hook: smaller slots send blocks to the direct encode
+    const u32 stage_max = cap_env ? (u32)strtoul(cap_env, nullptr, 10) : 0xFFFFFFFFu;
+    trace_point(b, "store+sizes");
+    LB_LAUNCH(k_exp_list, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb, stage_max);
+    launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, xstage, 0);
+    LB_LAUNCH(k_exp_layout, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb, n_a, n_b);
+    tm.kernel_launches += 3;
+    trace_point(b, "encode");
+    run_scans(b, {ScanJob{(const u8*)n_a, (u8*)xt.xdoc + offsetof(XDoc, exp_off), 4, sizeof(XDoc), D},
+                  ScanJob{(const u8*)n_b, (u8*)xt.xdoc + offsetof(XDoc, ovf0), 4, sizeof(XDoc), D}});
+    xtot = d2h_one(b, xt.xdoc + D);
+    const u64 XT = xtot.exp_off, NOVF = xtot.ovf0;
+    if (getenv("LB_PHASE_TRACE"))
+        fprintf(stderr, "[trace] export: %llu blocks, %llu outgrew their staging slot; %llu staging bytes for %llu exported\n",
+                (unsigned long long)NOB, (unsigned long long)NOVF, (unsigned long long)NSTG, (unsigned long long)XT);
+    trace_point(b, "layout scan + size d2h");
+    u8* out = dv.alloc<u8>(XT + 16, true);
+    trace_point(b, "export buffer alloc+zero");
+    if (NOVF) { launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, out, 1); tm.kernel_launches += 1; }
+    LB_LAUNCH(k_exp_finish, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, xt, xb, xstage, out);
+    tm.kernel_launches += 1;
+    trace_point(b, "assemble");
+    dv.release(cnt); dv.release(xb); dv.release(xscratch); dv.release(xstage);
+    *total = XT;
+    return out;
+}
 
 void pipeline(lb_batch* b) {
     Dev& dv = b->dev;
@@ -772,6 +822,7 @@ void pipeline(lb_batch* b) {
         xt.fc_src = dv.alloc<u32>(SEGCAP); xt.fc_pos = dv.alloc<u32>(SEGCAP); xt.fc_r0 = dv.alloc<u32>(SEGCAP);
         xt.fc_from = dv.alloc<u32>(SEGCAP); xt.fc_atoms = dv.alloc<u32>(SEGCAP); xt.fc_nrows = dv.alloc<u32>(SEGCAP);
         xt.fc_ndel = dv.alloc<u32>(SEGCAP); xt.fc_block = dv.alloc<u8>(SEGCAP); xt.fc_skip = dv.alloc<u32>(SEGCAP, true);
+        xt.fc_est = dv.alloc<u32>(SEGCAP);
         xt.only_doc = 0xFFFFFFFFu; xt.from_ctr = nullptr;
         trace_point(b, "export allocs");
         LB_LAUNCH(k_exp_init, nblk(D), TPB, 0, st, b->d_docs, D, xt);
@@ -797,38 +848,17 @@ void pipeline(lb_batch* b) {
                 dv.release(*pp);
                 *pp = nw;
             }
-            u32** fcs[8] = {&xt.fc_src, &xt.fc_pos, &xt.fc_r0, &xt.fc_from, &xt.fc_atoms, &xt.fc_nrows, &xt.fc_ndel, &xt.fc_skip};
+            u32** fcs[9] = {&xt.fc_src, &xt.fc_pos, &xt.fc_r0, &xt.fc_from, &xt.fc_atoms, &xt.fc_nrows, &xt.fc_ndel, &xt.fc_skip, &xt.fc_est};
             for (auto pp : fcs) { dv.release(*pp); *pp = dv.alloc<u32>(cap, true); }
             dv.release(xt.fc_block);
             xt.fc_block = dv.alloc<u8>(cap);
         }
         if (NOVF) { LB_LAUNCH(k_exp_changes, nblk(NCH, 64), 64, 0, st, b->d_docs, NCH, xt, 1); tm.kernel_launches += 1; }
         LB_LAUNCH(k_exp_store, nblk(D, 64), 64, 0, st, b->d_docs, D, xt);
-        LB_LAUNCH(k_exp_sizes, nblk(D), TPB, 0, st, b->d_docs, D, xt, d_tmp_a, d_tmp_b);
-        tm.kernel_launches += 2;
-        run_scans(b, {ScanJob{(const u8*)d_tmp_a, (u8*)xt.xdoc + offsetof(XDoc, ob0), 4, sizeof(XDoc), D},
-                      ScanJob{(const u8*)d_tmp_b, (u8*)xt.xdoc + offsetof(XDoc, scratch0), 4, sizeof(XDoc), D}});
-        XDoc xtot = d2h_one(b, xt.xdoc + D);
-        u64 NOB = xtot.ob0, NSCR = xtot.scratch0;
-        XBlock* xb = dv.alloc<XBlock>(NOB + 1);
-        u32* xscratch = dv.alloc<u32>(NSCR + 1);
-        trace_point(b, "store+sizes");
-        LB_LAUNCH(k_exp_list, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb);
-        launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, nullptr, 0);
-        LB_LAUNCH(k_exp_layout, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb, d_tmp_a);
-        tm.kernel_launches += 3;
-        trace_point(b, "encode pass 0");
-        run_scans(b, {ScanJob{(const u8*)d_tmp_a, (u8*)xt.xdoc + offsetof(XDoc, exp_off), 4, sizeof(XDoc), D}});
-        u64 XT = d2h_one(b, &xt.xdoc[D].exp_off);
+        tm.kernel_launches += 1;
+        u64 XT = 0;
+        b->d_export = export_encode(b, xt, &XT);
         b->export_total = XT;
-        trace_point(b, "layout scan + size d2h");
-        b->d_export = dv.alloc<u8>(XT + 16, true);
-        trace_point(b, "export buffer alloc+zero");
-        launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, b->d_export, 1);
-        trace_point(b, "encode pass 1 kernel");
-        LB_LAUNCH(k_exp_finish, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, xt, b->d_export);
-        tm.kernel_launches += 2;
-        trace_point(b, "encode pass 1");
         tm.export_bytes = XT;
         b->xt = xt;
         b->have_xt = true;
@@ -1024,29 +1054,14 @@ lb_status export_from(lb_batch* b, size_t doc, const lb_id_span* from, size_t n_
         xt.only_doc = (u32)doc;
         XDoc* xdoc = dv.alloc<XDoc>(D + 1, true);
         xt.xdoc = xdoc;
-        u32* tmp_a = dv.alloc<u32>(D + 1, true);
-        u32* tmp_b = dv.alloc<u32>(D + 1, true);
         LB_LAUNCH(k_exp_init, nblk(D), TPB, 0, st, b->d_docs, D, xt);
         if (NCH) {
             LB_LAUNCH(k_exp_changes, nblk(NCH, 64), 64, 0, st, b->d_docs, NCH, xt, 0);
             LB_LAUNCH(k_exp_changes, nblk(NCH, 64), 64, 0, st, b->d_docs, NCH, xt, 1);
         }
         LB_LAUNCH(k_exp_store, nblk(D, 64), 64, 0, st, b->d_docs, D, xt);
-        LB_LAUNCH(k_exp_sizes, nblk(D), TPB, 0, st, b->d_docs, D, xt, tmp_a, tmp_b);
-        run_scans(b, {ScanJob{(const u8*)tmp_a, (u8*)xdoc + offsetof(XDoc, ob0), 4, sizeof(XDoc), D},
-                      ScanJob{(const u8*)tmp_b, (u8*)xdoc + offsetof(XDoc, scratch0), 4, sizeof(XDoc), D}});
-        XDoc xtot = d2h_one(b, xdoc + D);
-        u64 NOB = xtot.ob0, NSCR = xtot.scratch0;
-        XBlock* xb = dv.alloc<XBlock>(NOB + 1);
-        u32* xscratch = dv.alloc<u32>(NSCR + 1);
-        LB_LAUNCH(k_exp_list, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb);
-        launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, nullptr, 0);
-        LB_LAUNCH(k_exp_layout, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb, tmp_a);
-        run_scans(b, {ScanJob{(const u8*)tmp_a, (u8*)xdoc + offsetof(XDoc, exp_off), 4, sizeof(XDoc), D}});
-        u64 XT = d2h_one(b, &xdoc[D].exp_off);
-        u8* d_out = dv.alloc<u8>(XT + 16, true);
-        launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, d_out, 1);
-        LB_LAUNCH(k_exp_finish, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, xt, d_out);
+        u64 XT = 0;
+        u8* d_out = export_encode(b, xt, &XT);
         XDoc x = d2h_one(b, xdoc + doc);
         lb_status rc = LB_OK;
         if ((x.flags & 1) || x.exp_len == 0) { g_last_error = "document uses features the export phase does not cover"; rc = LB_ERR_UNSUPPORTED; }
@@ -1055,7 +1070,7 @@ lb_status export_from(lb_batch* b, size_t doc, const lb_id_span* from, size_t n_
             CK(cudaMemcpyAsync(out.data(), d_out + x.exp_off, x.exp_len, cudaMemcpyDeviceToHost, st));
             CK(cudaStreamSynchronize(st));
         }
-        dv.release(d_from); dv.release(xdoc); dv.release(tmp_a); dv.release(tmp_b); dv.release(xb); dv.release(xscratch); dv.release(d_out);
+        dv.release(d_from); dv.release(xdoc); dv.release(d_out);
         return rc;
     } catch (lb_status s) {
         return s;

@@ -18,7 +18,9 @@
 //   C  into the fresh store export builds (export_blocks_from): same rules, freshly computed sizes.
 // Only per-row flag bits (op start, segment start) and per-segment summaries are written; the merge decisions
 // look at the boundary ops only.  A thread per output block then gathers its ops into scratch columns and
-// encodes them (two passes: sizes, bytes).
+// encodes them once, into a staging slot sized from the block's rows and store estimate; the lengths it records
+// place the block in its document's blob, and a warp per document assembles the blob from the staged pieces and the
+// length prefixes.  A block that outgrows its slot is encoded a second time, straight into the blob.
 // Whether two neighbouring inserts merge depends on where their payloads landed in the importing document's
 // arenas (arena.rs:237-263): values are adjacent when nothing else was allocated in between (decode order),
 // strings additionally need the append-only buffer not to have been reallocated (capacity doubles from 32;
@@ -45,6 +47,8 @@ struct XDoc {          // per document
     u64 exp_off;       // offset of the blob in the export buffer
     u32 exp_len;
     u32 scratch_words;
+    u64 stage0;        // first staging byte of this doc's blocks
+    u64 ovf0;          // blocks of the documents before this one that outgrew their staging slot (scan)
 };
 struct XBlock {        // one output block
     u32 doc;
@@ -56,6 +60,9 @@ struct XBlock {        // one output block
     u64 scratch;       // scratch words of this block
     u32 n_rows, n_dels;            // scratch capacities: rows, delete ops
     u32 n_ops, n_del_ops, n_cids, n_pos; // after the gather: merged ops, merged deletes, containers, positions
+    u64 stage;         // staging slot: first byte, capacity; the block's pieces without their length prefixes
+    u32 stage_cap;
+    u32 ovf;           // 1 = the pieces did not fit the slot: encoded straight into the blob instead
 };
 
 struct ExportTables {
@@ -96,6 +103,7 @@ struct ExportTables {
     // final changes (same index space: a document never ends up with more changes than segments)
     u32* fc_src; u32* fc_pos; u32* fc_r0; u32* fc_from; u32* fc_atoms; u32* fc_nrows; u32* fc_ndel; u8* fc_block;
     u32* fc_skip;      // atoms of the change's first row that lie before the `from` version (Op::slice)
+    u32* fc_est;       // the store's size estimate of the change's ops (sizes the staging slot of its block)
     // export(ExportMode::updates(from)) of ONE document on demand (lb_doc_export_updates): only_doc != ~0 restricts
     // every kernel to that document; from_ctr[doc peer slot] = first counter to export (encoding.rs:79-83,
     // change_store.rs:494-528 export_blocks_from, change.rs:203-258 Change::slice)
@@ -105,15 +113,16 @@ struct ExportTables {
 
 // ---------------------------------------------------------------------------------------------- byte sink
 struct XSink {
-    u8* dst;   // nullptr = counting
-    u64 n;
+    u8* dst;   // bytes [0, cap) are stored; what lies beyond is only counted (cap = 0: a counting sink)
+    u64 n, cap;
+    __device__ __forceinline__ XSink(u8* d, u64 c) : dst(d), n(0), cap(c) {}
     // (plain byte stores: collecting eight bytes per store or reading the scratch columns through a four-word window
     //  adds instructions and registers to every byte of an encoder bound by dependent-load latency at 25 % occupancy)
-    __device__ __forceinline__ void put(u8 c) { if (dst) dst[n] = c; n++; }
+    __device__ __forceinline__ void put(u8 c) { if (n < cap) dst[n] = c; n++; }
     __device__ __forceinline__ void varint(u64 v) { while (v >= 0x80) { put((u8)(v | 0x80)); v >>= 7; } put((u8)v); }
     __device__ __forceinline__ void zigzag(i64 v) { varint(((u64)v << 1) ^ (u64)(v >> 63)); }
     __device__ __forceinline__ void copy(const u8* s, u64 len) {
-        if (dst) {
+        if (n + len <= cap) {
             u8* d = dst + n;
             u64 i = 0;
             while (i < len && ((uintptr_t)(d + i) & 3)) { d[i] = s[i]; i++; }
@@ -802,6 +811,7 @@ __global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, Export
     auto emit = [&](const XEntry& e, bool starts_block) {
         t.fc_src[w] = e.src; t.fc_pos[w] = e.pos; t.fc_r0[w] = e.r0; t.fc_from[w] = e.from; t.fc_atoms[w] = e.atoms;
         t.fc_nrows[w] = e.nrows; t.fc_ndel[w] = e.ndel; t.fc_block[w] = starts_block ? 1 : 0; t.fc_skip[w] = e.skip;
+        t.fc_est[w] = e.est_ops;
         n_mb += starts_block;
         w++;
     };
@@ -848,8 +858,18 @@ __global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, Export
     t.xdoc[d] = x;
 }
 
-// thread per document: list the output blocks (after the scans of n_mb and scratch sizes)
-__global__ void k_exp_list(const DocInfo* __restrict__ docs, u32 n_docs, ExportTables t, XBlock* __restrict__ xb) {
+// Staging slot of an output block, in bytes: the store's size estimate of its changes (text bytes, 4 per list item,
+// 8 per delete span, 3 per map op) plus room for the op and delete columns, the per-change metadata and the
+// registers.  This is what the blocks usually need, not a bound (a bound is about 40 bytes per row against about 8
+// used): the few blocks that outgrow their slot are encoded again, straight into the export buffer.
+__device__ __forceinline__ u64 xstage_change(const ExportTables& t, u64 k) {
+    return t.fc_est[k] + 4ull * t.fc_nrows[k] + 4ull * t.fc_ndel[k] + 16;
+}
+__device__ __forceinline__ u64 xstage_block(const DocInfo& di) { return 64 + 8ull * (di.P + di.C); }
+
+// thread per document: list the output blocks (after the scans of n_mb, scratch and staging sizes).  stage_max caps
+// every slot's capacity (testing: forces the blocks that need more onto the direct encode)
+__global__ void k_exp_list(const DocInfo* __restrict__ docs, u32 n_docs, ExportTables t, XBlock* __restrict__ xb, u32 stage_max) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
     const DocInfo& di = docs[d];
@@ -857,38 +877,51 @@ __global__ void k_exp_list(const DocInfo* __restrict__ docs, u32 n_docs, ExportT
     if (di.code != DOC_OK || x.n_mb == 0) return;
     u64 f0 = di.ch0 + t.ch_seg0[di.ch0];
     u32 regs = 2 * (di.P + di.K + di.C);
-    u64 scr = x.scratch0;
+    u64 scr = x.scratch0, stg = x.stage0, slot = 0;
     int idx = -1;
     XBlock b;
     memset(&b, 0, sizeof(b));
+    auto close = [&]() {
+        b.stage_cap = (u32)(slot < stage_max ? slot : stage_max);
+        xb[x.ob0 + idx] = b;
+        scr += regs + (5 + ((x.flags >> 1) & 1u)) * b.n_rows + 3 * b.n_dels;
+        stg += slot;
+    };
     for (u64 k = f0; k < f0 + x.n_fc; k++) {
         if (t.fc_block[k]) {
-            if (idx >= 0) { b.fc1 = (u32)k; xb[x.ob0 + idx] = b; scr += regs + (5 + ((x.flags >> 1) & 1u)) * b.n_rows + 3 * b.n_dels; }
+            if (idx >= 0) { b.fc1 = (u32)k; close(); }
             idx++;
             memset(&b, 0, sizeof(b));
-            b.doc = d; b.fc0 = (u32)k; b.scratch = scr;
+            b.doc = d; b.fc0 = (u32)k; b.scratch = scr; b.stage = stg;
+            slot = xstage_block(di);
         }
         b.n_rows += t.fc_nrows[k];
         b.n_dels += t.fc_ndel[k];
+        slot += xstage_change(t, k);
     }
-    if (idx >= 0) { b.fc1 = (u32)(f0 + x.n_fc); xb[x.ob0 + idx] = b; }
+    if (idx >= 0) { b.fc1 = (u32)(f0 + x.n_fc); close(); }
 }
-// thread per document: scratch words of its blocks (registers + op columns + delete columns)
+// thread per document: scratch words (registers + op columns + delete columns) and staging bytes of its blocks
 __global__ void k_exp_sizes(const DocInfo* __restrict__ docs, u32 n_docs, ExportTables t, u32* __restrict__ n_blocks,
-                            u32* __restrict__ n_scratch) {
+                            u32* __restrict__ n_scratch, u32* __restrict__ n_stage) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
     const DocInfo& di = docs[d];
     const XDoc& x = t.xdoc[d];
     u32 nb = di.code == DOC_OK ? x.n_mb : 0;
-    u64 words = 0;
+    u64 words = 0, bytes = 0;
     if (nb) {
         u64 f0 = di.ch0 + t.ch_seg0[di.ch0];
         words = (u64)nb * 2 * (di.P + di.K + di.C);
-        for (u64 k = f0; k < f0 + x.n_fc; k++) words += (5ull + ((x.flags >> 1) & 1u)) * t.fc_nrows[k] + 3ull * t.fc_ndel[k];
+        bytes = (u64)nb * xstage_block(di);
+        for (u64 k = f0; k < f0 + x.n_fc; k++) {
+            words += (5ull + ((x.flags >> 1) & 1u)) * t.fc_nrows[k] + 3ull * t.fc_ndel[k];
+            bytes += xstage_change(t, k);
+        }
     }
     n_blocks[d] = nb;
     n_scratch[d] = (u32)words;
+    n_stage[d] = (u32)bytes;
 }
 
 // ---------------------------------------------------------------------------------------------- column encoders
@@ -1144,12 +1177,17 @@ __global__ void k_exp_posrank(const DocInfo* __restrict__ docs, u32 n_docs, Expo
     if (lane == 0) t.xdoc[d].n_prank = carry;
 }
 
-// thread per output block.  pass 0: gather ops into scratch columns, registers, section sizes ; pass 1: bytes.
+// thread per output block.  pass 0: gather ops into scratch columns and registers while writing the values section
+// into the block's staging slot (`out` = the staging buffer), then every other section (column) writer stores its body
+// after it and its length into the XBlock;
+// a block whose pieces outgrow the slot only counts from there on and is flagged (XBlock::ovf).  pass 1, flagged
+// blocks only: the same writers once more, with the length prefixes, straight into the blob (`out` = the export
+// buffer, after k_exp_layout).
 // Two builds of the same code: <1> is compiled with __launch_bounds__(64, 5) (the compiler then schedules for 64-thread
-// CTAs: 132 registers against 124 without bounds, other load / store placement), <0> without bounds.
+// CTAs: 136 registers against 124 without bounds, other load / store placement), <0> without bounds.
 // The host picks by the number of output blocks.  Re-export phase on one H100 80GB HBM3 (400 W power limit), unbounded
-// against bounded: C3 at 4 k documents (~55 k blocks) 43.0 against 55.7 ms; C5 at 10 k documents (~160 k blocks) 145.9
-// against 130.8 ms; C3 at 40 k documents (~550 k blocks) 374.7 against 365.6 ms.  So batches of at least
+// against bounded: C3 at 4 k documents (~55 k blocks) 39.1 against 46.6 ms; C5 at 10 k documents (160 k blocks) 128.5
+// against 106.4 ms; C3 at 40 k documents (~550 k blocks) 346.4 against 325.3 / 323.4 ms.  So batches of at least
 // LB_XENC_BOUNDED_MIN_BLOCKS output blocks take the bounded build.
 #define LB_XENC_BOUNDED_MIN_BLOCKS 100000ull
 __device__ __forceinline__ void exp_encode_body(
@@ -1158,6 +1196,7 @@ __device__ __forceinline__ void exp_encode_body(
     u64 bi_ = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (bi_ >= n_blocks) return;
     XBlock B = xb[bi_];
+    if (pass == 1 && !B.ovf) return;
     const DocInfo& di = docs[B.doc];
     const u32 P = di.P, K = di.K, C = di.C;
     u32* sc = scratch + B.scratch;
@@ -1236,8 +1275,11 @@ __device__ __forceinline__ void exp_encode_body(
             for (u32 i = 0; i < m; i++) if (i == 0 || p_rank[i] != p_rank[w - 1]) p_rank[w++] = p_rank[i];
             B.n_pos = w;
         }
-        // ops in order: containers, map keys, delete targets (block_encode.rs:180-236)
-        u32 n_ops = 0, n_del = 0, vbytes = 0;
+        // ops in order: containers, map keys, delete targets (block_encode.rs:180-236).  The values section is written
+        // on the way, at the start of the staging slot: the op's value prefix once its rows are merged, then the
+        // payloads of those rows, which were just loaded (w_values is the same walk, for the direct encode)
+        XSink vs(out + B.stage, B.stage_cap);
+        u32 n_ops = 0, n_del = 0;
         u32 prev_cidx = 0, prev_prop = 0, prev_dp = 0, prev_dc = 0, prev_dl = 0;   // 32-bit wrap-around deltas
         for (u32 j = 0; j < N; j++) {
             XRows it(t, t.fc_pos[fc0 + j], t.fc_r0[fc0 + j]);
@@ -1248,25 +1290,22 @@ __device__ __forceinline__ void exp_encode_body(
                 XRows it0 = it;
                 const u32 left0 = left;
                 const u32 skip0 = skip;
-                XOp o = xop_gather(t, di, it, left, has_maps ? nullptr : &vbytes, skip);
+                XOp o = xop_gather(t, di, it, left, nullptr, skip);
                 skip = left ? it.skip : 0u;   // (the next op may start on the first kept row of a trimmed change)
-                if (o.xk == XK_LIST) vbytes += 1 + varint_len(o.atoms);
-                else if (o.xk == XK_TEXT) vbytes += varint_len(o.f1 - o.f0);
+                if (o.xk == XK_LIST) { vs.put(7); vs.varint(o.atoms); }
+                else if (o.xk == XK_TEXT) vs.varint(o.f1 - o.f0);
                 // DeltaRle columns are stored as deltas right away (the encoders then read every value once)
                 u32 lc = cids.reg(o.cidx);
                 u32 lp = (o.xk == XK_MAPSET || o.xk == XK_MAPDEL) ? keys.reg((u32)o.prop) : (u32)o.prop;
-                if (has_maps) {   // payload sizes after the op's own registrations: nested keys register in value order
+                if (o.xk == XK_LIST || o.xk == XK_TEXT || o.xk == XK_MAPSET) {
+                    // payloads after the op's own registrations: nested keys register in value order
                     u32 k = left0 - left;
                     while (k) {
                         const u8* pp;
                         u32 pn;
                         xr_payload_skip(t, it0.row(), o.xk, k == left0 - left ? skip0 : it0.skip, &pp, &pn);
-                        if (o.xk == XK_LIST || o.xk == XK_MAPSET) {
-                            XSink cs;
-                            cs.dst = nullptr; cs.n = 0;
-                            xvalue_copy(cs, pp, pn, t, t.blocks[t.ch_block[it0.ch]].key0, keys, true);
-                            vbytes += (u32)cs.n;
-                        } else vbytes += pn;
+                        if (has_maps && o.xk != XK_TEXT) xvalue_copy(vs, pp, pn, t, t.blocks[t.ch_block[it0.ch]].key0, keys, true);
+                        else vs.copy(pp, pn);
                         k--;
                         if (k) it0.next();
                     }
@@ -1280,10 +1319,7 @@ __device__ __forceinline__ void exp_encode_body(
                     uint4 ids = t.tr_ids[o.f0];
                     peers.reg(ids.x);
                     if ((ids.z & 3u) != TRP_ROOT) peers.reg(ids.z >> 2);
-                    XSink cs;
-                    cs.dst = nullptr; cs.n = 0;
-                    w_tree_value(cs, o.f0);
-                    vbytes += (u32)cs.n;
+                    w_tree_value(vs, o.f0);
                 }
                 if (o.xk == XK_DEL) {
                     u32 dp = peers.reg(o.f0);
@@ -1297,7 +1333,7 @@ __device__ __forceinline__ void exp_encode_body(
         }
         B.n_ops = n_ops;
         B.n_del_ops = n_del;
-        B.sec_len[7] = vbytes;   // values section: sizes come with the gather, no second walk
+        B.sec_len[7] = (u32)vs.n;   // values section: written with the gather, no second walk
         // ContainerArena::from_containers (arena.rs:103-147): roots register their name, normals their peer
         for (u32 i = 0; i < cids.n; i++) {
             const DocContainer& dc = t.dcont[di.cid0 + cids.ord[i]];
@@ -1440,37 +1476,44 @@ __device__ __forceinline__ void exp_encode_body(
     u32 lam0 = (u32)lamport(0);
     u32 lam_len = (u32)lamport(N - 1) + t.fc_atoms[B.fc1 - 1] - lam0;
     if (pass == 0) {
-        XSink s;
-        s.dst = nullptr;
-        s.n = 0; w_header(s); B.sec_len[0] = (u32)s.n;
-        s.n = 0; w_meta(s); B.sec_len[1] = (u32)s.n;
-        s.n = 0; w_cids(s); B.sec_len[2] = (u32)s.n;
-        s.n = 0; w_keys(s); B.sec_len[3] = (u32)s.n;
+        // staged pieces: the values (written by the gather), then in blob order the five header varints, the bodies of
+        // sections 0-3, the position columns, the op columns, the delete columns (k_exp_finish adds the prefixes)
+        XSink s(out + B.stage, B.stage_cap);
+        s.n = B.sec_len[7];
+        s.varint(counter0);
+        s.varint(counter_len);
+        s.varint(lam0);
+        s.varint(lam_len);
+        s.varint(N);
+        u64 m = s.n;
+        w_header(s); B.sec_len[0] = (u32)(s.n - m); m = s.n;
+        w_meta(s); B.sec_len[1] = (u32)(s.n - m); m = s.n;
+        w_cids(s); B.sec_len[2] = (u32)(s.n - m); m = s.n;
+        w_keys(s); B.sec_len[3] = (u32)(s.n - m); m = s.n;
         u32 tot = 0;
         if (B.n_pos) {
             tot = 2;   // varint(1) varint(2)
-            for (int c = 0; c < 2; c++) { s.n = 0; w_poscol(s, c); B.col_len[8 + c] = (u32)s.n; tot += varint_len(s.n) + (u32)s.n; }
+            for (int c = 0; c < 2; c++) { w_poscol(s, c); B.col_len[8 + c] = (u32)(s.n - m); m = s.n; tot += varint_len(B.col_len[8 + c]) + B.col_len[8 + c]; }
         }
         B.sec_len[4] = tot;
         tot = 2;   // varint(1) varint(4)
-        for (int c = 0; c < 4; c++) { s.n = 0; w_opcol(s, c); B.col_len[c] = (u32)s.n; tot += varint_len(s.n) + (u32)s.n; }
+        for (int c = 0; c < 4; c++) { w_opcol(s, c); B.col_len[c] = (u32)(s.n - m); m = s.n; tot += varint_len(B.col_len[c]) + B.col_len[c]; }
         B.sec_len[5] = tot;
         if (n_del) {
             tot = 2;
-            for (int c = 0; c < 3; c++) { s.n = 0; w_delcol(s, c); B.col_len[4 + c] = (u32)s.n; tot += varint_len(s.n) + (u32)s.n; }
+            for (int c = 0; c < 3; c++) { w_delcol(s, c); B.col_len[4 + c] = (u32)(s.n - m); m = s.n; tot += varint_len(B.col_len[4 + c]) + B.col_len[4 + c]; }
             B.sec_len[6] = tot;
         } else B.sec_len[6] = 0;
+        B.ovf = s.n > s.cap;
         u32 len = varint_len(counter0) + varint_len(counter_len) + varint_len(lam0) + varint_len(lam_len) + varint_len(N);
         for (int i = 0; i < 8; i++) len += varint_len(B.sec_len[i]) + B.sec_len[i];
         B.len = len;
         xb[bi_] = B;
         return;
     }
-    // ---- pass 1: ULEB length prefix + block bytes at the document's slot
+    // ---- pass 1 (blocks that outgrew their slot): ULEB length prefix + block bytes at the document's slot
     u64 base = t.xdoc[B.doc].exp_off + B.off;
-    XSink s;
-    s.dst = out + base - varint_len(B.len);
-    s.n = 0;
+    XSink s(out + base - varint_len(B.len), ~0ull);
     s.varint(B.len);
     s.varint(counter0);
     s.varint(counter_len);
@@ -1509,13 +1552,13 @@ template <> __global__ void __launch_bounds__(64, 5) k_exp_encode<1>(const DocIn
     exp_encode_body(docs, n_blocks, t, xb, scratch, out, pass);
 }
 
-// thread per document: block offsets inside the blob, blob length (after encode pass 0)
+// thread per document: block offsets inside the blob, blob length, blocks that outgrew their slot (after encode pass 0)
 __global__ void k_exp_layout(const DocInfo* __restrict__ docs, u32 n_docs, ExportTables t, XBlock* __restrict__ xb,
-                             u32* __restrict__ padded_len) {
+                             u32* __restrict__ padded_len, u32* __restrict__ n_ovf) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
     XDoc& x = t.xdoc[d];
-    u32 len = 0;
+    u32 len = 0, ovf = 0;
     if (docs[d].code == DOC_OK && !(x.flags & 1)) {
         len = 22;
         for (u32 i = 0; i < x.n_mb; i++) {
@@ -1523,20 +1566,69 @@ __global__ void k_exp_layout(const DocInfo* __restrict__ docs, u32 n_docs, Expor
             len += varint_len(b.len);
             b.off = len;
             len += b.len;
+            ovf += b.ovf;
         }
     }
     x.exp_len = len;
     padded_len[d] = (len + 15u) & ~15u;
+    n_ovf[d] = ovf;
 }
 
-// thread per document: header, mode, checksum (encoding.rs:397-416)
-__global__ void k_exp_finish(const DocInfo* __restrict__ docs, u32 n_docs, ExportTables t, u8* __restrict__ out) {
+// warp per document: the blob from the staged pieces of its blocks and their length prefixes (the blocks that
+// outgrew their slot are in place already), then header, mode, checksum (encoding.rs:397-416)
+__global__ void k_exp_finish(const DocInfo* __restrict__ docs, u32 n_docs, ExportTables t, const XBlock* __restrict__ xb,
+                             const u8* __restrict__ stage, u8* __restrict__ out) {
     u32 d = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // warp per document: the checksum walks the whole blob
     int lane = threadIdx.x & 31;
     if (d >= n_docs) return;
     const XDoc& x = t.xdoc[d];
     if (x.exp_len == 0) return;
     u8* b = out + x.exp_off;
+    for (u32 i = 0; i < x.n_mb; i++) {
+        const XBlock& B = xb[x.ob0 + i];
+        if (B.ovf) continue;
+        u8* dst = b + B.off - varint_len(B.len);
+        const u8* src = stage + B.stage;
+        u64 o = 0, so = B.sec_len[7];   // the values come first in the slot and last in the block
+        auto prefix = [&](u32 v) {
+            if (lane == 0) { XSink s(dst + o, ~0ull); s.varint(v); }
+            o += varint_len(v);
+        };
+        auto piece = [&](u32 n) {   // four independent byte loads per lane in flight, then the stores
+            u8* dd = dst + o;
+            const u8* ss = src + so;
+            u32 k = (u32)lane;
+            for (; k + 96 < n; k += 128) {
+                u8 a = ss[k], c = ss[k + 32], e = ss[k + 64], g = ss[k + 96];
+                dd[k] = a; dd[k + 32] = c; dd[k + 64] = e; dd[k + 96] = g;
+            }
+            for (; k < n; k += 32) dd[k] = ss[k];
+            o += n;
+            so += n;
+        };
+        u32 head = B.len;   // the five header varints
+        for (int k = 0; k < 8; k++) head -= varint_len(B.sec_len[k]) + B.sec_len[k];
+        prefix(B.len);
+        piece(head);
+        for (int k = 0; k < 4; k++) { prefix(B.sec_len[k]); piece(B.sec_len[k]); }
+        prefix(B.sec_len[4]);
+        if (B.n_pos) {
+            prefix(1); prefix(2);
+            for (int c = 0; c < 2; c++) { prefix(B.col_len[8 + c]); piece(B.col_len[8 + c]); }
+        }
+        prefix(B.sec_len[5]);
+        prefix(1); prefix(4);
+        for (int c = 0; c < 4; c++) { prefix(B.col_len[c]); piece(B.col_len[c]); }
+        prefix(B.sec_len[6]);
+        if (B.n_del_ops) {
+            prefix(1); prefix(3);
+            for (int c = 0; c < 3; c++) { prefix(B.col_len[4 + c]); piece(B.col_len[4 + c]); }
+        }
+        prefix(B.sec_len[7]);
+        so = 0;
+        piece(B.sec_len[7]);
+    }
+    __syncwarp();
     if (lane == 0) {
         b[0] = 'l'; b[1] = 'o'; b[2] = 'r'; b[3] = 'o';
         for (int i = 4; i < 20; i++) b[i] = 0;
