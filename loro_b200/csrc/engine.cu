@@ -22,7 +22,6 @@
 #include "k_frame.cuh"
 #include "k_decode.cuh"
 #include "k_decode_warp.cuh"
-#include "k_decode_group.cuh"
 #include "k_resolve.cuh"
 #include "k_classify.cuh"
 #include "k_seq.cuh"
@@ -130,10 +129,6 @@ __global__ void k_copy_segments(const CopySeg* __restrict__ segs, u32 n) {
     for (u64 i = lane; i < n16; i += 32) d4[i] = s4[i];
     for (u64 i = (n16 << 4) + lane; i < sg.len; i += 32) sg.dst[i] = sg.src[i];
 }
-
-#ifndef LB_DECODE_DEFAULT
-#define LB_DECODE_DEFAULT 1   // 0 rows, 1 cols, 2 warp, 3 group (k_decode*.cuh)
-#endif
 
 namespace {
 
@@ -554,22 +549,12 @@ void pipeline(lb_batch* b) {
     t.tr_parent_peer = dv.alloc<u32>(NTR); t.tr_parent_ctr = dv.alloc<i32>(NTR); t.tr_pos = dv.alloc<u32>(NTR);
     t.dw_stats = dv.alloc<unsigned long long>(4, true);
     if (B) {
-        // decoder variants (A/B switch LB_DECODE = rows | cols | warp | group): thread per block with all cursors at once,
-        // thread per block one column at a time, warp per block on TMA-staged shared memory (lane-parallel run
-        // expansion), warp per four TMA-staged blocks with a lane per column stream
+        // block decoder (DESIGN.md section 4): LB_DECODE=warp selects a warp per block on TMA-staged shared memory
+        // (k_decode_warp.cuh); anything else, or nothing, a thread per block one column at a time (k_decode.cuh)
         static const char* mode_env = getenv("LB_DECODE");
-        static const int mode = !mode_env ? LB_DECODE_DEFAULT
-                                : (!strcmp(mode_env, "rows") ? 0 : (!strcmp(mode_env, "warp") ? 2 : (!strcmp(mode_env, "group") ? 3 : 1)));
-        if (mode == 0) LB_LAUNCH(k_block_decode, nblk(B, 64), 64, 0, st, b->d_bytes, blk, B, t);
-        else if (mode == 1) LB_LAUNCH(k_block_decode_cols, nblk(B, 64), 64, 0, st, b->d_bytes, blk, B, t);
-        else if (mode == 3) {
-            const size_t smem = sizeof(DgWarp) * DG_WARPS;
-#ifndef LB_SIMT_EMU
-            static bool attr_set_g = false;
-            if (!attr_set_g) { CK(cudaFuncSetAttribute(k_block_decode_group, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr_set_g = true; }
-#endif
-            LB_LAUNCH(k_block_decode_group, nblk(B, DG_G * DG_WARPS), 32 * DG_WARPS, smem, st, b->d_bytes, blk, B, t);
-        } else {
+        static const bool warp = mode_env && !strcmp(mode_env, "warp");
+        if (!warp) LB_LAUNCH(k_block_decode_cols, nblk(B, 64), 64, 0, st, b->d_bytes, blk, B, t);
+        else {
             const size_t smem = sizeof(DwWarp) * DW_WARPS;
 #ifndef LB_SIMT_EMU
             static bool attr_set = false;

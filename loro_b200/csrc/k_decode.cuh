@@ -277,12 +277,12 @@ enum { TRP_ROOT = 0, TRP_NODE = 1, TRP_DELETED = 2 };
 
 // ---------------------------------------------------------------- pass 2: fill
 // The block decoder in three single-thread pieces (`b` = the block's bytes, in global or in shared memory):
-//   decode_block_small  header, change meta, keys, cids, positions   (tens of bytes per block)
-//   decode_block_rows   delete-start ids, the four ops columns, the values walk   (the bulk)
-//   decode_block_fail   a failed block still leaves its rows pointing at its own changes
-// k_block_decode runs them one thread per block (blocks larger than the staging buffer, and the emulated build's
-// reference path); k_block_decode_warp (k_decode_warp.cuh) stages the block in shared memory and replaces
-// decode_block_rows by lane-parallel column expansion and value-chain resolution.
+//   decode_block_small      header, change meta, keys, cids, positions   (tens of bytes per block)
+//   decode_block_rows_cols  delete-start ids, the four ops columns, the values walk   (the bulk)
+//   decode_block_fail       a failed block still leaves its rows pointing at its own changes
+// k_block_decode_cols (the default) runs them one thread per block.  k_block_decode_warp (k_decode_warp.cuh) stages the
+// block in shared memory and replaces decode_block_rows_cols by lane-parallel column expansion and value-chain
+// resolution; the blocks its fast path does not cover still go through decode_block_rows_cols, on one lane.
 __device__ inline u32 decode_block_small(const u8* b, const BlockInfo& bi, u64 i, const Tables& t) {
     u32 N = bi.n_changes;
     u32 err = 0;
@@ -465,119 +465,11 @@ __device__ inline u32 decode_block_small(const u8* b, const BlockInfo& bi, u64 i
     return err;
 }
 
-__device__ inline u32 decode_block_rows(const u8* b, const BlockInfo& bi, const Tables& t, u32 err, u32* n_maps_out) {
-    u32 N = bi.n_changes;
-    // ---- delete start ids (3 DeltaRle columns)
-    if (bi.sec_len[6]) {
-        const u8* col[3];
-        u32 cl[3];
-        if (!columnar_open(b + bi.sec_off[6], bi.sec_len[6], 3, col, cl)) err = err ? err : LB_ERR(DOC_ERR_DECODE);
-        else {
-            RleCur a(col[0], cl[0], 2), bb(col[1], cl[1], 2), cc(col[2], cl[2], 2);
-            i64 pa = 0, pb = 0, pc = 0;
-            for (u32 q = 0; q < bi.n_dels; q++) {
-                i64 x, y, z;
-                if (!a.next(&x) || !bb.next(&y) || !cc.next(&z)) { err = err ? err : LB_ERR(DOC_ERR_DECODE); break; }
-                pa += x; pb += y; pc += z;
-                if (pa < 0 || (u64)pa >= bi.n_peers || pc == 0) err = err ? err : LB_ERR(DOC_ERR_CORRUPT);
-                t.del_peer_idx[bi.del0 + q] = (u32)pa;
-                t.del_counter[bi.del0 + q] = (i32)pb;
-                t.del_len[bi.del0 + q] = (i32)pc;
-            }
-            if (a.c.err || bb.c.err || cc.c.err) err = err ? err : LB_ERR(DOC_ERR_DECODE);
-        }
-    } else if (bi.n_dels) err = err ? err : LB_ERR(DOC_ERR_DECODE);
-    // ---- ops: 4 columns + values walk
-    {
-        const u8* col[4];
-        u32 cl[4];
-        columnar_open(b + bi.sec_off[5], bi.sec_len[5], 4, col, cl);
-        RleCur c0(col[0], cl[0], 2), c1(col[1], cl[1], 2), c2(col[2], cl[2], 0), c3(col[3], cl[3], 1);
-        Cur v(b + bi.sec_off[7], bi.sec_len[7]);
-        i64 acc_c = 0, acc_p = 0;
-        i32 counter = (i32)bi.counter_start;
-        u32 change = 0;
-        u32 ch_first_row = 0;
-        u32 ndel = 0, ntree = 0;
-        u32 n_maps = 0;
-        i32 next_boundary = (i32)bi.counter_start + (i32)t.ch_len[bi.ch0];
-        t.ch_op0[bi.ch0] = bi.op0;
-        for (u32 r = 0; r < bi.n_ops; r++) {
-            i64 dc, dp, vt, ln;
-            if (!c0.next(&dc) || !c1.next(&dp) || !c2.next(&vt) || !c3.next(&ln)) { err = err ? err : LB_ERR(DOC_ERR_DECODE); break; }
-            acc_c += dc;
-            acc_p += dp;
-            if (acc_c < 0 || (u64)acc_c >= bi.n_cids || ln <= 0 || change >= N) { err = err ? err : LB_ERR(DOC_ERR_CORRUPT); break; }
-            u64 row = bi.op0 + r;
-            t.op_cid[row] = (u32)acc_c;
-            t.op_prop[row] = (i32)acc_p;
-            t.op_vtype[row] = (u8)vt;
-            t.op_len[row] = (u32)ln;
-            t.op_counter[row] = counter;
-            t.op_change[row] = (u32)(bi.ch0 + change);
-            if ((u8)vt == VK_LORO_VALUE && t.cid_type[bi.cid0 + (u32)acc_c] == CT_LIST) {
-                // a List insert carries LoroValue::List with exactly `len` items (outdated_encode_reordered.rs:246-262,
-                // the reference fails the import otherwise): later phases address the items through `len`
-                Cur pk = v;
-                u8 k = pk.get();
-                u64 n_items = pk.varint();
-                if (k != 7 || n_items != (u64)ln) { err = err ? err : LB_ERR(DOC_ERR_CORRUPT); break; }
-            }
-            const u8* v0 = v.p;
-            u32 aux_idx = 0xFFFFFFFFu;
-            if ((u8)vt == VK_RAW_TREE_MOVE) {
-                // read_raw_tree_move (value.rs:969-989): subject peer idx / counter, position idx, parent (null = root)
-                u64 sp = v.varint(), sc = v.varint(), pi = v.varint();
-                u8 pn = v.get();
-                u64 pp = 0, pcn = 0;
-                if (!pn) { pp = v.varint(); pcn = v.varint(); }
-                if (ntree >= bi.n_tree || sp >= bi.n_peers || (!pn && pp >= bi.n_peers) || sc > 0x7FFFFFFFull || pcn > 0x7FFFFFFFull) {
-                    err = err ? err : LB_ERR(DOC_ERR_CORRUPT);
-                    break;
-                }
-                u8 pk = pn ? TRP_ROOT : TRP_NODE;
-                if (!pn && t.peer_id[bi.peer0 + (u32)pp] == DELETED_ROOT_PEER && (i32)pcn == DELETED_ROOT_CTR) pk = TRP_DELETED;
-                if (pk != TRP_DELETED && pi >= bi.n_pos) { err = err ? err : LB_ERR(DOC_ERR_CORRUPT); break; }
-                u64 ti = bi.tr0 + ntree++;
-                t.tr_target_peer[ti] = (u32)sp;
-                t.tr_target_ctr[ti] = (i32)sc;
-                t.tr_parent_kind[ti] = pk;
-                t.tr_parent_peer[ti] = (u32)pp;
-                t.tr_parent_ctr[ti] = (i32)pcn;
-                t.tr_pos[ti] = pk == TRP_DELETED ? 0xFFFFFFFFu : (u32)(bi.pos0 + pi);
-                aux_idx = (u32)ti;
-            } else
-                skip_value(v, (u8)vt, &n_maps);
-            t.op_val_off[row] = bi.off + (u64)(v0 - b);
-            t.op_val_len[row] = (u32)(v.p - v0);
-            if ((u8)vt == VK_DELETE_SEQ) aux_idx = (u32)(bi.del0 + ndel++);
-            t.op_del[row] = aux_idx;
-            counter += (i32)ln;
-            // a row never straddles a change boundary: the reference's encoder cuts ops at changes, and everything
-            // downstream (atom tables, pending ranges) trusts ch_len -- a blob that disagrees is corrupt
-            if (counter > next_boundary) { err = err ? err : LB_ERR(DOC_ERR_CORRUPT); break; }
-            if (counter == next_boundary) {
-                t.ch_nops[bi.ch0 + change] = r + 1 - ch_first_row;
-                change++;
-                ch_first_row = r + 1;
-                if (change < N) {
-                    t.ch_op0[bi.ch0 + change] = bi.op0 + r + 1;
-                    next_boundary += (i32)t.ch_len[bi.ch0 + change];
-                }
-            }
-        }
-        if (v.err || !v.empty() || c0.c.err || c1.c.err || c2.c.err || c3.c.err) err = err ? err : LB_ERR(DOC_ERR_DECODE);
-        if (!err && (change != N || counter != (i32)(bi.counter_start + bi.counter_len) || ndel != bi.n_dels || ntree != bi.n_tree))
-            err = LB_ERR(DOC_ERR_CORRUPT);
-        *n_maps_out = n_maps;
-    }
-    return err;
-}
-
-// ---- the rows again, one COLUMN at a time: a thread has a single byte cursor alive at any moment, so its cache
-// lines stay resident in L1 between windows (seven cursors 4 KB apart thrash it), the loop bodies need a fraction of the registers, and consecutive stores of a thread
-// fall into the same 32-byte sector back to back.  The values walk reads the kind / length / container of a row back
-// from the tables the column passes just wrote (sequential per thread).  Same results, same error codes.
+// ---- the rows, one COLUMN at a time: a thread has a single byte cursor alive at any moment, so its cache lines stay
+// resident in L1 between windows (seven cursors 4 KB apart, all columns at once, thrash it), the loop bodies need a
+// fraction of the registers, and consecutive stores of a thread fall into the same 32-byte sector back to back.  The
+// values walk reads the kind / length / container of a row back from the tables the column passes just wrote
+// (sequential per thread).
 template <int MODE, class Emit>
 __device__ __forceinline__ u32 column_pass(const u8* col, u32 len, u32 n, Emit emit) {   // returns rows emitted, ~0u on malformed input
     RleCur c(col, len, MODE);
@@ -697,20 +589,6 @@ __device__ inline void decode_block_fail(const BlockInfo& bi, u64 i, const Table
     }
 }
 
-// (no register cap: capping the registers makes this kernel spill)
-__global__ void k_block_decode(const u8* __restrict__ bytes, BlockInfo* __restrict__ blocks, u64 n_blocks,
-                               Tables t) {
-    u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_blocks) return;
-    BlockInfo bi = blocks[i];
-    if (bi.err) return;
-    const u8* b = bytes + bi.off;
-    u32 n_maps = 0;
-    u32 err = decode_block_small(b, bi, i, t);
-    err = decode_block_rows(b, bi, t, err, &n_maps);
-    blocks[i].n_value_maps = n_maps;
-    if (err) decode_block_fail(bi, i, t, blocks, err);
-}
 // thread per block, one column at a time
 __global__ void k_block_decode_cols(const u8* __restrict__ bytes, BlockInfo* __restrict__ blocks, u64 n_blocks, Tables t) {
     u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;

@@ -15,8 +15,10 @@
 //     together, and each lane then walks its own chunk from its true entry.  Rows pick their value by rank;
 //   * every SoA table is written with consecutive lanes on consecutive rows.
 // Anything the fast path does not cover (a block larger than the staging buffer, two kinds of payload in one block,
-// nested values, a values section beyond the table, malformed input) is handed to decode_block_rows on one lane --
-// it rewrites the same rows and produces the precise error code -- so the fast path never has to explain a failure.
+// nested values, a values section beyond the table, malformed input) is handed to decode_block_rows_cols on one lane --
+// the default decoder's row code: it rewrites the same rows and produces the precise error code, so the fast path never
+// has to explain a failure.  Like the default decoder, it leaves the check that a List insert carries exactly `len`
+// items to k_op_classify, which runs after every decoder; a block that fails it fails its document there.
 #pragma once
 #include "k_decode.cuh"
 
@@ -383,51 +385,47 @@ k_block_decode_warp(const u8* __restrict__ bytes, BlockInfo* __restrict__ blocks
     DwWarp& S = smem[w];
     const u32 shift = (u32)(bi.off & 15);
     const u32 span = (shift + bi.len + 15u) & ~15u;
+    const bool staged = span <= DW_BYTES;   // (uniform) a larger block is decoded from global memory by one lane
+    const u8* b = bytes + bi.off;
     u32 err = 0, n_maps = 0;
-    if (span > DW_BYTES) {
-        // larger than the staging buffer: one lane decodes from global memory
-        if (lane == 0) {
-            const u8* g = bytes + bi.off;
-            err = decode_block_small(g, bi, i, t);
-            err = decode_block_rows(g, bi, t, err, &n_maps);
-            blocks[i].n_value_maps = n_maps;
-            if (err) decode_block_fail(bi, i, t, blocks, err);
-            atomicAdd(&t.dw_stats[2], 1ull);
-        }
-        return;
-    }
-    // ---- stage the block: one bulk asynchronous copy, completion on the warp's mbarrier
+    bool fast = false;
+    if (staged) {
+        // ---- stage the block: one bulk asynchronous copy, completion on the warp's mbarrier
 #ifdef LB_SIMT_EMU
-    for (u32 k = (u32)lane; k < span; k += 32) S.bytes[k] = bytes[bi.off - shift + k];
-    __syncwarp();
-#else
-    {
-        const u32 bar = (u32)__cvta_generic_to_shared(&S.bar);
-        const u32 dst = (u32)__cvta_generic_to_shared(S.bytes);
-        if (lane == 0) {
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(span) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(dst), "l"(bytes + (bi.off - shift)), "r"(span), "r"(bar) : "memory");
-        }
+        for (u32 k = (u32)lane; k < span; k += 32) S.bytes[k] = bytes[bi.off - shift + k];
         __syncwarp();
-        u32 done = 0;
-        while (!done) {
-            asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                         : "=r"(done) : "r"(bar), "r"(0u) : "memory");
+#else
+        {
+            const u32 bar = (u32)__cvta_generic_to_shared(&S.bar);
+            const u32 dst = (u32)__cvta_generic_to_shared(S.bytes);
+            if (lane == 0) {
+                asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(span) : "memory");
+                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                             ::"r"(dst), "l"(bytes + (bi.off - shift)), "r"(span), "r"(bar) : "memory");
+            }
+            __syncwarp();
+            u32 done = 0;
+            while (!done) {
+                asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                             : "=r"(done) : "r"(bar), "r"(0u) : "memory");
+            }
         }
-    }
 #endif
-    const u8* b = S.bytes + shift;
-    if (lane == 0) err = decode_block_small(b, bi, i, t);
-    err = (u32)__shfl_sync(LB_FULL, (int)err, 0);
-    __syncwarp();
-    bool fast = !err && dw_rows_fast(b, bi, t, S.tab, lane);
-    __syncwarp();
+        b = S.bytes + shift;
+        if (lane == 0) err = decode_block_small(b, bi, i, t);
+        err = (u32)__shfl_sync(LB_FULL, (int)err, 0);
+        __syncwarp();
+        fast = !err && dw_rows_fast(b, bi, t, S.tab, lane);
+        __syncwarp();
+    }
+    // one call site for the one-lane rows: with a second call of decode_block_rows_cols ptxas keeps one of them as a
+    // real call, and the kernel drops to 80 registers and spills
     if (lane == 0) {
-        if (!fast) err = decode_block_rows(b, bi, t, err, &n_maps);
-        atomicAdd(&t.dw_stats[fast ? 0 : 1], 1ull);
+        if (!staged) err = decode_block_small(b, bi, i, t);
+        if (!fast) err = decode_block_rows_cols(b, bi, t, err, &n_maps);
+        atomicAdd(&t.dw_stats[fast ? 0 : staged ? 1 : 2], 1ull);
         blocks[i].n_value_maps = n_maps;
         if (err) decode_block_fail(bi, i, t, blocks, err);
     }

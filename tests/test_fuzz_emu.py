@@ -10,10 +10,17 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 EMU = os.path.join(HERE, "emu", "libloro_b200_emu.so")
 
 
-@pytest.mark.parametrize("seed,wide", [(21, False), (23, False), (61, True)])
-def test_mutated_blobs_stay_inside_their_tables(seed, wide):
+@pytest.mark.parametrize("seed,wide,decode", [
+    pytest.param(21, False, None, id="21-False"),
+    pytest.param(23, False, None, id="23-False"),
+    pytest.param(61, True, None, id="61-True"),
+    pytest.param(61, True, "warp", id="61-True-warp"),   # the warp decoder: fast path, one-lane fallback, unstaged blocks
+])
+def test_mutated_blobs_stay_inside_their_tables(seed, wide, decode):
     subprocess.check_call([os.path.join(HERE, "emu", "build_emu.sh")])
     env = dict(os.environ, LB_EMU_GUARD="1", LB_EMU_THREADS="1")
+    if decode:
+        env["LB_DECODE"] = decode
     if wide:
         env["LB_FUZZ_WIDE"] = "1"   # more document shapes (seed 61 used to find a list insert whose item count lied)
     out = subprocess.run([sys.executable, os.path.join(HERE, "tools", "fuzz_emu.py"), EMU, str(seed), "150"],
