@@ -306,27 +306,21 @@ struct lb_batch {
     uint32_t flags = 0;
     bool owns_bytes = false;
     // device state
-    const u8* d_bytes = nullptr;
+    BatchTables tb{};             // every batch-wide table (the input bytes at tb.bytes), kept for export(updates(from))
     u64* d_offs = nullptr;
     u32* d_lens = nullptr;
     size_t n_blobs = 0;                       // blobs in the byte buffer (>= n_docs: import_batch groups)
     std::vector<u32> blob_doc, doc_blob0;     // blob -> document ; document -> first blob (n_docs + 1)
     std::vector<u32> doc_nprior;              // lb_docset_import: leading blobs of each document that restate its earlier state
     DocInfo* d_docs = nullptr;
-    BlockInfo* d_blocks = nullptr;
-    DocPeer* d_dpeer = nullptr;
     u8* d_json = nullptr;
     u8* d_export = nullptr;      // phase 7 output: one FastUpdates blob per document
-    XDoc* d_xdoc = nullptr;
     u64 export_total = 0;
     std::vector<XDoc> xdocs;
-    ExportTables xt{};            // phase-7 tables kept for export(updates(from)) on demand
-    bool have_xt = false;
     std::unordered_map<size_t, std::vector<uint8_t>> from_exports;   // last on-demand export per document
     uint8_t* exported = nullptr;  // malloc'ed host copy (lbstage::download)
     bool export_fetched = false;
     u64 n_blocks = 0, n_changes = 0, n_rows = 0, n_peers_tot = 0, json_total = 0, n_deps = 0;
-    Tables tb{};
     // host results
     std::vector<DocInfo> docs;
     std::vector<DocPeer> dpeer;          // packed: document d owns [peer_base[d], peer_base[d] + P)
@@ -375,7 +369,7 @@ inline unsigned nblk(u64 n, int tpb = TPB) { return (unsigned)((n + tpb - 1) / t
 
 // one pass of the export encoder over NOB output blocks (pass 1 only touches the blocks that outgrew their staging
 // slot), in the build that is faster for that many (k_export.cuh)
-void launch_exp_encode(cudaStream_t st, DocInfo* docs, u64 NOB, const ExportTables& xt, XBlock* xb, u32* xscratch, u8* out,
+void launch_exp_encode(cudaStream_t st, DocInfo* docs, u64 NOB, const BatchTables& xt, XBlock* xb, u32* xscratch, u8* out,
                        int pass) {
     if (!NOB) return;
     if (NOB >= LB_XENC_BOUNDED_MIN_BLOCKS) LB_LAUNCH(k_exp_encode<1>, nblk(NOB, 64), 64, 0, st, docs, NOB, xt, xb, xscratch, out, pass);
@@ -425,7 +419,7 @@ void run_scans(lb_batch* b, std::vector<ScanJob> jobs) {
 // slots, layout (the lengths are exact, so are the offsets), the direct encode of the blocks that outgrew their slot
 // (only when there are any: their count comes back with the blob sizes), then the blobs assembled per document.
 // Returns the export buffer (*total bytes, document d's blob at xt.xdoc[d].exp_off).
-u8* export_encode(lb_batch* b, const ExportTables& xt, u64* total) {
+u8* export_encode(lb_batch* b, const BatchTables& xt, u64* total) {
     Dev& dv = b->dev;
     cudaStream_t st = dv.stream;
     const u32 D = (u32)b->n_docs;
@@ -479,6 +473,7 @@ void pipeline(lb_batch* b) {
         b->docs.resize(1);
         return;
     }
+    BatchTables& t = b->tb;
     // ------------------------------------------------------------ phase 1: frame
     u32 Q = (u32)b->n_blobs;
     b->d_docs = dv.alloc<DocInfo>(D + 1, true);
@@ -489,7 +484,7 @@ void pipeline(lb_batch* b) {
     u32* d_doc_blob0 = dv.alloc<u32>(D + 2);
     CK(cudaMemcpyAsync(d_blob_doc, b->blob_doc.data(), sizeof(u32) * Q, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_doc_blob0, b->doc_blob0.data(), sizeof(u32) * (D + 1), cudaMemcpyHostToDevice, st));
-    LB_LAUNCH(k_frame_count, nblk((u64)Q * 32, 128), 128, 0, st, b->d_bytes, b->d_offs, b->d_lens, Q, d_blob_code, d_blob_nblocks);
+    LB_LAUNCH(k_frame_count, nblk((u64)Q * 32, 128), 128, 0, st, t.bytes, b->d_offs, b->d_lens, Q, d_blob_code, d_blob_nblocks);
     run_scans(b, {ScanJob{(const u8*)d_blob_nblocks, (u8*)d_blob_block0, 4, 8, Q}});
     u32* d_doc_nprior = nullptr;
     if (!b->doc_nprior.empty()) {
@@ -500,14 +495,14 @@ void pipeline(lb_batch* b) {
     tm.kernel_launches += 2;
     u64 B = d2h_one(b, d_blob_block0 + Q);
     b->n_blocks = B;
-    b->d_blocks = dv.alloc<BlockInfo>(B + 1, true);
-    LB_LAUNCH(k_frame_fill, nblk(Q), TPB, 0, st, b->d_bytes, b->d_offs, b->d_lens, Q, d_blob_doc, d_blob_code, d_blob_block0, d_doc_blob0, b->d_blocks);
+    t.blocks = dv.alloc<BlockInfo>(B + 1, true);
+    LB_LAUNCH(k_frame_fill, nblk(Q), TPB, 0, st, t.bytes, b->d_offs, b->d_lens, Q, d_blob_doc, d_blob_code, d_blob_block0, d_doc_blob0, t.blocks);
     tm.kernel_launches += 1;
     mark(b);  // [1] frame done
     // ------------------------------------------------------------ phase 2: decode
-    BlockInfo* blk = b->d_blocks;
+    BlockInfo* blk = t.blocks;
     if (B) {
-        LB_LAUNCH(k_block_count, nblk(B, 64), 64, 0, st, b->d_bytes, blk, B);
+        LB_LAUNCH(k_block_count, nblk(B, 64), 64, 0, st, t.bytes, blk, B);
         tm.kernel_launches += 1;
     }
     run_scans(b, {FIELD_JOB(blk, BlockInfo, n_peers, peer0, B), FIELD_JOB(blk, BlockInfo, n_keys, key0, B),
@@ -530,12 +525,11 @@ void pipeline(lb_batch* b) {
     b->n_rows = NR;
     b->n_peers_tot = NP;
     b->n_deps = ND;
-    Tables& t = b->tb;
     t.peer_id = dv.alloc<u64>(NP);
     t.key_off = dv.alloc<u64>(NK); t.key_len = dv.alloc<u32>(NK);
     t.cid_root = dv.alloc<u8>(NC); t.cid_type = dv.alloc<u8>(NC); t.cid_peer_idx = dv.alloc<u32>(NC); t.cid_koc = dv.alloc<i32>(NC);
     t.ch_block = dv.alloc<u32>(NCH); t.ch_counter = dv.alloc<i32>(NCH); t.ch_len = dv.alloc<u32>(NCH);
-    t.ch_lamport = dv.alloc<u32>(NCH); t.ch_ts = dv.alloc<i64>(NCH); t.ch_dep0 = dv.alloc<u64>(NCH);
+    t.ch_lamport_wire = dv.alloc<u32>(NCH); t.ch_ts = dv.alloc<i64>(NCH); t.ch_dep0 = dv.alloc<u64>(NCH);
     t.ch_msg_off = dv.alloc<u64>(NCH); t.ch_msg_len = dv.alloc<u32>(NCH, true);
     t.ch_ndeps = dv.alloc<u32>(NCH); t.ch_dep_self = dv.alloc<u8>(NCH); t.ch_op0 = dv.alloc<u64>(NCH);
     t.ch_nops = dv.alloc<u32>(NCH, true);
@@ -553,14 +547,14 @@ void pipeline(lb_batch* b) {
         // (k_decode_warp.cuh); anything else, or nothing, a thread per block one column at a time (k_decode.cuh)
         static const char* mode_env = getenv("LB_DECODE");
         static const bool warp = mode_env && !strcmp(mode_env, "warp");
-        if (!warp) LB_LAUNCH(k_block_decode_cols, nblk(B, 64), 64, 0, st, b->d_bytes, blk, B, t);
+        if (!warp) LB_LAUNCH(k_block_decode_cols, nblk(B, 64), 64, 0, st, t.bytes, blk, B, t);
         else {
             const size_t smem = sizeof(DwWarp) * DW_WARPS;
 #ifndef LB_SIMT_EMU
             static bool attr_set = false;
             if (!attr_set) { CK(cudaFuncSetAttribute(k_block_decode_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr_set = true; }
 #endif
-            LB_LAUNCH(k_block_decode_warp, nblk(B, DW_WARPS), 32 * DW_WARPS, smem, st, b->d_bytes, blk, B, t);
+            LB_LAUNCH(k_block_decode_warp, nblk(B, DW_WARPS), 32 * DW_WARPS, smem, st, t.bytes, blk, B, t);
         }
         tm.kernel_launches += 1;
     }
@@ -568,36 +562,27 @@ void pipeline(lb_batch* b) {
     // SURVEY 8d algorithmic bytes of decode: blob bytes read + SoA written
     tm.decode_bytes_written = NR * 13 + NCH * (4 + 4 + 8 + 4) + ND * 12;
     // ------------------------------------------------------------ phase 3: resolve
-    ResolveTables rt;
-    memset(&rt, 0, sizeof(rt));
-    rt.peer_id = t.peer_id; rt.key_off = t.key_off; rt.key_len = t.key_len;
-    rt.cid_root = t.cid_root; rt.cid_type = t.cid_type; rt.cid_peer_idx = t.cid_peer_idx; rt.cid_koc = t.cid_koc;
-    rt.ch_block = t.ch_block; rt.ch_counter = t.ch_counter; rt.ch_len = t.ch_len; rt.ch_lamport_wire = t.ch_lamport;
-    rt.ch_dep0 = t.ch_dep0; rt.ch_ndeps = t.ch_ndeps; rt.ch_dep_self = t.ch_dep_self;
-    rt.dep_peer_idx = t.dep_peer_idx; rt.dep_counter = t.dep_counter;
-    b->d_dpeer = dv.alloc<DocPeer>(NP, true);
-    rt.dpeer = b->d_dpeer; rt.peer_map = dv.alloc<u32>(NP);
-    DocContainer* dcont = dv.alloc<DocContainer>(NC + 1, true);
-    rt.dcont = dcont; rt.cid_map = dv.alloc<u32>(NC);
-    rt.dkey_off = dv.alloc<u64>(NK); rt.dkey_len = dv.alloc<u32>(NK); rt.key_map = dv.alloc<u32>(NK);
-    rt.blk_order = dv.alloc<u32>(B);
-    rt.ch_order = dv.alloc<u32>(NCH);
-    rt.ch_aorder = dv.alloc<u32>(NCH);
-    rt.ch_peer = dv.alloc<u16>(NCH);
-    rt.ch_applied = dv.alloc<u8>(NCH, true);
-    rt.ch_lamport = dv.alloc<u32>(NCH, true);
-    rt.ch_walk = dv.alloc<u32>(NCH);
-    rt.ch_pos = dv.alloc<u32>(NCH, true);
-    rt.ch_trim = dv.alloc<u32>(NCH, true);
+    t.dpeer = dv.alloc<DocPeer>(NP, true); t.peer_map = dv.alloc<u32>(NP);
+    t.dcont = dv.alloc<DocContainer>(NC + 1, true); t.cid_map = dv.alloc<u32>(NC);
+    t.dkey_off = dv.alloc<u64>(NK); t.dkey_len = dv.alloc<u32>(NK); t.key_map = dv.alloc<u32>(NK);
+    t.blk_order = dv.alloc<u32>(B);
+    t.ch_order = dv.alloc<u32>(NCH);
+    t.ch_aorder = dv.alloc<u32>(NCH);
+    t.ch_peer = dv.alloc<u16>(NCH);
+    t.ch_applied = dv.alloc<u8>(NCH, true);
+    t.ch_lamport = dv.alloc<u32>(NCH, true);
+    t.ch_walk = dv.alloc<u32>(NCH);
+    t.ch_pos = dv.alloc<u32>(NCH, true);
+    t.ch_trim = dv.alloc<u32>(NCH, true);
     // status of multi-blob documents (import_batch groups, lb_docset_import): per-copy epochs, per-blob pending hulls
     i32* d_pend_scratch = nullptr;
     if (Q > D) {
-        rt.ch_epoch = dv.alloc<u32>(NCH);
-        rt.ch_maxend = dv.alloc<i32>(NCH);
-        rt.head_lamport = dv.alloc<u32>(NP);
+        t.ch_epoch = dv.alloc<u32>(NCH);
+        t.ch_maxend = dv.alloc<i32>(NCH);
+        t.head_lamport = dv.alloc<u32>(NP);
         d_pend_scratch = dv.alloc<i32>(2 * (u64)Q + 2);
     }
-    LB_LAUNCH(k_doc_tables, nblk(D, 64), 64, 0, st, b->d_bytes, b->d_docs, D, blk, rt);
+    LB_LAUNCH(k_doc_tables, nblk(D, 64), 64, 0, st, t.bytes, b->d_docs, D, blk, t);
     u32* d_tmp_a = dv.alloc<u32>(D + 1, true);
     u32* d_tmp_b = dv.alloc<u32>(D + 1, true);
     u32* d_tmp_c = dv.alloc<u32>(D + 1, true);
@@ -605,10 +590,10 @@ void pipeline(lb_batch* b) {
     tm.kernel_launches += 2;
     run_scans(b, {ScanJob{(const u8*)d_tmp_a, (u8*)b->d_docs + offsetof(DocInfo, vv0), 4, sizeof(DocInfo), D}});
     u64 VV = d2h_one(b, &b->d_docs[D].vv0);
-    rt.ch_vv = dv.alloc<i32>(VV);
+    t.ch_vv = dv.alloc<i32>(VV);
     u32* d_cursor = dv.alloc<u32>(NP);
-    LB_LAUNCH(k_doc_causal, nblk(D, 64), 64, 0, st, b->d_docs, D, blk, rt, d_cursor, d_doc_blob0, d_pend_scratch);
-    LB_LAUNCH(k_doc_frontiers, nblk(D, 64), 64, 0, st, b->d_docs, D, rt);
+    LB_LAUNCH(k_doc_causal, nblk(D, 64), 64, 0, st, b->d_docs, D, blk, t, d_cursor, d_doc_blob0, d_pend_scratch);
+    LB_LAUNCH(k_doc_frontiers, nblk(D, 64), 64, 0, st, b->d_docs, D, t);
     LB_LAUNCH(k_doc_sizes, nblk(D), TPB, 0, st, b->d_docs, D, d_tmp_a, d_tmp_b, d_tmp_c, 1);
     tm.kernel_launches += 3;
     run_scans(b, {ScanJob{(const u8*)d_tmp_b, (u8*)b->d_docs + offsetof(DocInfo, atom0), 4, sizeof(DocInfo), D},
@@ -617,27 +602,15 @@ void pipeline(lb_batch* b) {
     u64 NATOM = dtot.atom0, NSLOT = dtot.mapslot0;
     mark(b);  // [3] resolve done
     // ------------------------------------------------------------ phase 4: classify + map LWW
-    ClassifyTables ct;
-    memset(&ct, 0, sizeof(ct));
-    ct.blocks = blk; ct.ch_block = t.ch_block; ct.ch_applied = rt.ch_applied; ct.ch_lamport = rt.ch_lamport;
-    ct.ch_counter = t.ch_counter; ct.ch_peer = rt.ch_peer; ct.ch_trim = rt.ch_trim;
-    ct.bytes = b->d_bytes; ct.op_val_off = t.op_val_off; ct.op_val_len = t.op_val_len;
-    ct.op_cid = t.op_cid; ct.op_prop = t.op_prop; ct.op_vtype = t.op_vtype; ct.op_len = t.op_len;
-    ct.op_counter = t.op_counter; ct.op_change = t.op_change;
-    ct.op_del = t.op_del; ct.del_peer_idx = t.del_peer_idx; ct.del_counter = t.del_counter; ct.del_len = t.del_len;
-    ct.peer_map = rt.peer_map;
-    ct.tr_target_peer = t.tr_target_peer; ct.tr_target_ctr = t.tr_target_ctr; ct.tr_parent_kind = t.tr_parent_kind;
-    ct.tr_parent_peer = t.tr_parent_peer; ct.tr_parent_ctr = t.tr_parent_ctr; ct.tr_pos = t.tr_pos;
-    ct.tr_rec = dv.alloc<uint4>(NTR); ct.tr_key = dv.alloc<u64>(NTR); ct.tr_ids = dv.alloc<uint4>(NTR);
-    ct.cid_map = rt.cid_map; ct.key_map = rt.key_map; ct.dcont = dcont; ct.dpeer = b->d_dpeer;
-    ct.op_kind = dv.alloc<u8>(NR); ct.op_cidx = dv.alloc<u32>(NR); ct.op_lamport = dv.alloc<u32>(NR);
-    ct.atom_row = dv.alloc<u32>(NATOM);
-    ct.op_rec = dv.alloc<uint4>(NR); ct.op_aux = dv.alloc<u32>(NR);
-    ct.map_best = dv.alloc<unsigned long long>(NSLOT, true);
-    ct.map_row = dv.alloc<u32>(NSLOT);
+    t.tr_rec = dv.alloc<uint4>(NTR); t.tr_key = dv.alloc<u64>(NTR); t.tr_ids = dv.alloc<uint4>(NTR);
+    t.op_kind = dv.alloc<u8>(NR); t.op_cidx = dv.alloc<u32>(NR); t.op_lamport = dv.alloc<u32>(NR);
+    t.atom_row = dv.alloc<u32>(NATOM);
+    t.op_rec = dv.alloc<uint4>(NR); t.op_aux = dv.alloc<u32>(NR);
+    t.map_best = dv.alloc<unsigned long long>(NSLOT, true);
+    t.map_row = dv.alloc<u32>(NSLOT);
     if (NR) {
-        LB_LAUNCH(k_op_classify, nblk(NR, 256), 256, 0, st, b->d_docs, NR, ct);
-        LB_LAUNCH(k_map_winner, nblk(NR, 256), 256, 0, st, b->d_docs, NR, ct);
+        LB_LAUNCH(k_op_classify, nblk(NR, 256), 256, 0, st, b->d_docs, NR, t);
+        LB_LAUNCH(k_map_winner, nblk(NR, 256), 256, 0, st, b->d_docs, NR, t);
         tm.kernel_launches += 2;
     }
     // capacities -> pools
@@ -647,17 +620,15 @@ void pipeline(lb_batch* b) {
     u32* cap_cvv = dv.alloc<u32>(NC + 1, true);
     u32* span_cap = dv.alloc<u32>(D + 1, true);
     const u32 leaf_w = 32;   // slots per leaf = lanes per warp (k_seq.cuh)
-    LB_LAUNCH(k_container_caps, nblk(D), TPB, 0, st, b->d_docs, D, dcont, cap_leaf, cap_node, cap_out, cap_cvv, span_cap, leaf_w);
+    LB_LAUNCH(k_container_caps, nblk(D), TPB, 0, st, b->d_docs, D, t.dcont, cap_leaf, cap_node, cap_out, cap_cvv, span_cap, leaf_w);
     tm.kernel_launches += 1;
-    run_scans(b, {ScanJob{(const u8*)cap_leaf, (u8*)dcont + offsetof(DocContainer, leaf0), 4, sizeof(DocContainer), NC},
-                  ScanJob{(const u8*)cap_node, (u8*)dcont + offsetof(DocContainer, node0), 4, sizeof(DocContainer), NC},
-                  ScanJob{(const u8*)cap_out, (u8*)dcont + offsetof(DocContainer, out0), 4, sizeof(DocContainer), NC},
-                  ScanJob{(const u8*)cap_cvv, (u8*)dcont + offsetof(DocContainer, cvv0), 4, sizeof(DocContainer), NC},
+    run_scans(b, {ScanJob{(const u8*)cap_leaf, (u8*)t.dcont + offsetof(DocContainer, leaf0), 4, sizeof(DocContainer), NC},
+                  ScanJob{(const u8*)cap_node, (u8*)t.dcont + offsetof(DocContainer, node0), 4, sizeof(DocContainer), NC},
+                  ScanJob{(const u8*)cap_out, (u8*)t.dcont + offsetof(DocContainer, out0), 4, sizeof(DocContainer), NC},
+                  ScanJob{(const u8*)cap_cvv, (u8*)t.dcont + offsetof(DocContainer, cvv0), 4, sizeof(DocContainer), NC},
                   ScanJob{(const u8*)span_cap, (u8*)b->d_docs + offsetof(DocInfo, span0), 4, sizeof(DocInfo), D}});
-    DocContainer ctot = d2h_one(b, dcont + NC);
-    DocInfo dtot2 = d2h_one(b, &b->d_docs[D]);
+    DocContainer ctot = d2h_one(b, t.dcont + NC);
     u64 NLEAF = ctot.leaf0, NNODE = ctot.node0, NOUT = ctot.out0, NCVV = ctot.cvv0;
-    (void)dtot2;
     mark(b);  // [4] classify done
     // ------------------------------------------------------------ phase 5: sequence integration
     SeqPools sp;
@@ -670,40 +641,26 @@ void pipeline(lb_batch* b) {
     sp.a_org = dv.alloc<uint4>(NATOM);
     sp.cvv = dv.alloc<i32>(NCVV, true);
     sp.cont_epoch = dv.alloc<u32>(NC + 1);
-    sp.out_row = dv.alloc<u32>(NOUT); sp.out_off = dv.alloc<u32>(NOUT); sp.out_len = dv.alloc<u32>(NOUT);
-    SeqTables sq;
-    memset(&sq, 0, sizeof(sq));
-    sq.dpeer = b->d_dpeer; sq.dcont = dcont;
-    sq.ch_walk = rt.ch_walk; sq.ch_op0 = t.ch_op0; sq.ch_nops = t.ch_nops; sq.ch_peer = rt.ch_peer; sq.ch_vv = rt.ch_vv;
-    sq.ch_order = rt.ch_aorder; sq.ch_counter = t.ch_counter; sq.ch_ndeps = t.ch_ndeps; sq.ch_dep_self = t.ch_dep_self;
-    sq.ch_pos = rt.ch_pos;
-    sq.op_rec = ct.op_rec; sq.op_aux = ct.op_aux; sq.op_change = t.op_change; sq.op_counter = t.op_counter;
-    sq.atom_row = ct.atom_row;
-    LB_LAUNCH(k_seq_integrate, nblk(D, LB_SEQ_WARPS), 32 * LB_SEQ_WARPS, 0, st, b->d_docs, D, sp, sq);
+    t.out_row = dv.alloc<u32>(NOUT); t.out_off = dv.alloc<u32>(NOUT); t.out_len = dv.alloc<u32>(NOUT);
+    LB_LAUNCH(k_seq_integrate, nblk(D, LB_SEQ_WARPS), 32 * LB_SEQ_WARPS, 0, st, b->d_docs, D, sp, t);
     tm.kernel_launches += 1;
     if (!(b->flags & LB_FLAG_KEEP_DEVICE)) {   // the tracker pools are the largest tables of the batch: free them early
         dv.release(sp.leaf); dv.release(sp.node); dv.release(sp.node_parent); dv.release(sp.atom_leaf); dv.release(sp.a_org);
-        dv.release(sp.cvv); dv.release(sp.cont_epoch); dv.release(ct.atom_row); dv.release(ct.op_rec);
+        dv.release(sp.cvv); dv.release(sp.cont_epoch); dv.release(t.atom_row); dv.release(t.op_rec);
     }
     mark(b);  // [5] list/text integration done
     // ------------------------------------------------------------ phase 5b: movable trees
-    TreeTables tt;
-    memset(&tt, 0, sizeof(tt));
     if (NTR) {
         CK(cudaMemsetAsync(d_tmp_b + D, 0, sizeof(u32), st));
         LB_LAUNCH(k_doc_sizes, nblk(D), TPB, 0, st, b->d_docs, D, d_tmp_a, d_tmp_b, d_tmp_c, 2);
         run_scans(b, {ScanJob{(const u8*)d_tmp_a, (u8*)b->d_docs + offsetof(DocInfo, tree0), 4, sizeof(DocInfo), D}});
         u64 NTS = d2h_one(b, &b->d_docs[D].tree0);
         const u32 max_atoms = d2h_one(b, d_tmp_b + D);
-        tt.dpeer = b->d_dpeer; tt.blocks = blk; tt.op_cidx = ct.op_cidx; tt.op_lamport = ct.op_lamport;
-        tt.tr_rec = ct.tr_rec; tt.tr_key = ct.tr_key;
-        tt.ts_key = dv.alloc<u64>(NTR); tt.ts_val = dv.alloc<u32>(NTR); tt.ts_rec = dv.alloc<uint4>(NTR);
-        tt.pos_off = t.pos_off; tt.pos_len = t.pos_len; tt.pos_pool = t.pos_pool;
-        tt.tn_parent = dv.alloc<u32>(NTS); tt.tn_move = dv.alloc<u32>(NTS); tt.tn_base = dv.alloc<u32>(NTS);
-        tt.tn_cnt = dv.alloc<u32>(NTS); tt.tn_sib = dv.alloc<u32>(NTS); tt.ns_key = dv.alloc<u64>(NTS);
-        tt.tn_child = dv.alloc<u32>(NTS);
-        tt.tn_root = dv.alloc<u32>(NTS); tt.tn_aopen = dv.alloc<u32>(NTS); tt.tn_aclose = dv.alloc<u32>(NTS);
-        tt.dcont = dcont;
+        t.ts_key = dv.alloc<u64>(NTR); t.ts_val = dv.alloc<u32>(NTR); t.ts_rec = dv.alloc<uint4>(NTR);
+        t.tn_parent = dv.alloc<u32>(NTS); t.tn_move = dv.alloc<u32>(NTS); t.tn_base = dv.alloc<u32>(NTS);
+        t.tn_cnt = dv.alloc<u32>(NTS); t.tn_sib = dv.alloc<u32>(NTS); t.ns_key = dv.alloc<u64>(NTS);
+        t.tn_child = dv.alloc<u32>(NTS);
+        t.tn_root = dv.alloc<u32>(NTS); t.tn_aopen = dv.alloc<u32>(NTS); t.tn_aclose = dv.alloc<u32>(NTS);
         // 16-bit parent links of one document in shared memory, sized for the largest tree document of the batch:
         // the number of resident documents (one sequential chain each) is what the apply kernel's speed depends on
         u32 s_nodes = max_atoms < TREE_S_NODES_MAX ? max_atoms : (u32)TREE_S_NODES_MAX;
@@ -718,36 +675,24 @@ void pipeline(lb_batch* b) {
             fprintf(stderr, "[trace] k_tree_apply: %zu bytes of shared memory per document, %d documents resident per SM\n", tree_smem, nb);
         }
 #endif
-        LB_LAUNCH(k_tree_sort, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, tt);
-        LB_LAUNCH(k_tree_apply, nblk((u64)D * 32, 32 * TREE_WARPS), 32 * TREE_WARPS, tree_smem, st, b->d_docs, D, tt, s_nodes);
-        LB_LAUNCH(k_tree_layout, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, tt);
+        LB_LAUNCH(k_tree_sort, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, t);
+        LB_LAUNCH(k_tree_apply, nblk((u64)D * 32, 32 * TREE_WARPS), 32 * TREE_WARPS, tree_smem, st, b->d_docs, D, t, s_nodes);
+        LB_LAUNCH(k_tree_layout, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, t);
         tm.kernel_launches += 4;
     }
     mark(b);  // [5b] trees done
     tm.tree_ops = NTR;
     // ------------------------------------------------------------ phase 6: JSON
-    StateTables stt;
-    memset(&stt, 0, sizeof(stt));
-    stt.bytes = b->d_bytes; stt.dpeer = b->d_dpeer; stt.dcont = dcont;
-    stt.dkey_off = rt.dkey_off; stt.dkey_len = rt.dkey_len; stt.map_row = ct.map_row; stt.map_best = ct.map_best;
-    stt.op_kind = ct.op_kind; stt.op_vtype = t.op_vtype; stt.op_len = t.op_len; stt.op_counter = t.op_counter;
-    stt.op_change = t.op_change; stt.op_val_off = t.op_val_off; stt.op_val_len = t.op_val_len; stt.ch_peer = rt.ch_peer;
-    stt.ch_block = t.ch_block; stt.bkey_off = t.key_off; stt.bkey_len = t.key_len;
-    stt.out_row = sp.out_row; stt.out_off = sp.out_off; stt.out_len = sp.out_len;
-    stt.blocks = blk; stt.tn_parent = tt.tn_parent; stt.tn_move = tt.tn_move; stt.tn_base = tt.tn_base; stt.tn_cnt = tt.tn_cnt;
-    stt.tn_sib = tt.tn_sib; stt.tn_child = tt.tn_child; stt.tr_rec = ct.tr_rec;
-    stt.tn_root = tt.tn_root; stt.tn_aopen = tt.tn_aopen; stt.tn_aclose = tt.tn_aclose; stt.ns_key = tt.ns_key;
-    stt.pos_off = t.pos_off; stt.pos_len = t.pos_len; stt.pos_pool = t.pos_pool;
     unsigned long long* d_acc = dv.alloc<unsigned long long>(4, true);
     if (!(b->flags & LB_FLAG_NO_JSON)) {
-        LB_LAUNCH(k_json, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, stt, (u8*)nullptr, 0);
+        LB_LAUNCH(k_json, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, t, (u8*)nullptr, 0);
         LB_LAUNCH(k_json_padlen, nblk(D), TPB, 0, st, b->d_docs, D, d_tmp_a);
         tm.kernel_launches += 2;
         run_scans(b, {ScanJob{(const u8*)d_tmp_a, (u8*)b->d_docs + offsetof(DocInfo, json_off), 4, sizeof(DocInfo), D}});
         u64 JT = d2h_one(b, &b->d_docs[D].json_off);
         b->json_total = JT;
         b->d_json = dv.alloc<u8>(JT + 16, true);
-        LB_LAUNCH(k_json, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, stt, b->d_json, 1);
+        LB_LAUNCH(k_json, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, t, b->d_json, 1);
         tm.kernel_launches += 1;
     }
     LB_LAUNCH(k_doc_hash, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, (const u8*)b->d_json, d_acc);
@@ -769,84 +714,68 @@ void pipeline(lb_batch* b) {
     // ------------------------------------------------------------ phase 7: re-export (all_updates per document)
     if (b->flags & LB_FLAG_EXPORT) {
         trace_point(b, "before export");
-        ExportTables xt;
-        memset(&xt, 0, sizeof(xt));
-        xt.bytes = b->d_bytes; xt.blocks = blk; xt.dpeer = b->d_dpeer; xt.dcont = dcont;
-        xt.dkey_off = rt.dkey_off; xt.dkey_len = rt.dkey_len; xt.key_map = rt.key_map; xt.peer_map = rt.peer_map;
-        xt.ch_order = rt.ch_aorder; xt.ch_applied = rt.ch_applied; xt.ch_block = t.ch_block; xt.ch_counter = t.ch_counter;
-        xt.ch_len = t.ch_len; xt.ch_lamport = rt.ch_lamport; xt.ch_ts = t.ch_ts; xt.ch_op0 = t.ch_op0; xt.ch_nops = t.ch_nops;
-        xt.ch_dep0 = t.ch_dep0; xt.ch_ndeps = t.ch_ndeps; xt.ch_dep_self = t.ch_dep_self;
-        xt.dep_peer_idx = t.dep_peer_idx; xt.dep_counter = t.dep_counter;
-        xt.ch_msg_off = t.ch_msg_off; xt.ch_msg_len = t.ch_msg_len;
-        xt.op_kind = ct.op_kind; xt.op_vtype = t.op_vtype; xt.op_cidx = ct.op_cidx; xt.op_prop = t.op_prop; xt.op_len = t.op_len;
-        xt.op_counter = t.op_counter; xt.op_val_off = t.op_val_off; xt.op_val_len = t.op_val_len; xt.op_del = t.op_del;
-        xt.op_aux = ct.op_aux; xt.del_counter = t.del_counter; xt.del_len = t.del_len;
-        xt.tr_ids = ct.tr_ids; xt.tr_pos = t.tr_pos; xt.pos_off = t.pos_off; xt.pos_len = t.pos_len; xt.pos_pool = t.pos_pool;
         if (NTR) {
-            xt.pos_rank = dv.alloc<u32>(NPOS); xt.pos_rep = dv.alloc<u32>(NPOS);
-            xt.ps_key = dv.alloc<u64>(NPOS); xt.ps_val = dv.alloc<u32>(NPOS);
+            t.pos_rank = dv.alloc<u32>(NPOS); t.pos_rep = dv.alloc<u32>(NPOS);
+            t.ps_key = dv.alloc<u64>(NPOS); t.ps_val = dv.alloc<u32>(NPOS);
         }
-        xt.x_rec = dv.alloc<uint4>(NR); xt.r_bytes = dv.alloc<u32>(NR); xt.r_flag = dv.alloc<u8>(NR);
-        xt.ch_nseg = dv.alloc<u32>(NCH + 1, true); xt.ch_novf = dv.alloc<u32>(NCH + 1, true);
-        xt.ch_seg0 = dv.alloc<u64>(NCH + 2, true);
-        xt.n_changes = NCH;
-        xt.n_rows = NR;
-        xt.ch_syn = dv.alloc<u32>(NCH + 1, true); xt.ch_syn0 = dv.alloc<u64>(NCH + 2, true);
-        xt.xdoc = dv.alloc<XDoc>(D + 1, true);
-        b->d_xdoc = xt.xdoc;
-        xt.ch_aval = dv.alloc<u32>(NCH + 1, true); xt.ch_astr = dv.alloc<u32>(NCH + 1, true);
-        xt.ch_aval0 = dv.alloc<u64>(NCH + 2, true); xt.ch_astr0 = dv.alloc<u64>(NCH + 2, true);
+        t.x_rec = dv.alloc<uint4>(NR); t.r_bytes = dv.alloc<u32>(NR); t.r_flag = dv.alloc<u8>(NR);
+        t.ch_nseg = dv.alloc<u32>(NCH + 1, true); t.ch_novf = dv.alloc<u32>(NCH + 1, true);
+        t.ch_seg0 = dv.alloc<u64>(NCH + 2, true);
+        t.n_changes = NCH;
+        t.n_rows = NR;
+        t.ch_syn = dv.alloc<u32>(NCH + 1, true); t.ch_syn0 = dv.alloc<u64>(NCH + 2, true);
+        t.xdoc = dv.alloc<XDoc>(D + 1, true);
+        t.ch_aval = dv.alloc<u32>(NCH + 1, true); t.ch_astr = dv.alloc<u32>(NCH + 1, true);
+        t.ch_aval0 = dv.alloc<u64>(NCH + 2, true); t.ch_astr0 = dv.alloc<u64>(NCH + 2, true);
         // segment / final-change records: one slot per change + one per extra segment of a split change; the
         // extras are counted by pass 0, so the arrays are sized with a bound first and checked after the scan
         u64 SEGCAP = NCH + NCH / 4 + 1024;
         if (getenv("LB_EXPORT_TIGHT_SEGCAP")) SEGCAP = NCH;   // testing hook: force the growth path
-        xt.sg_src = dv.alloc<u32>(SEGCAP); xt.sg_r0 = dv.alloc<u32>(SEGCAP); xt.sg_from = dv.alloc<u32>(SEGCAP);
-        xt.sg_atoms = dv.alloc<u32>(SEGCAP); xt.sg_est = dv.alloc<u32>(SEGCAP); xt.sg_nmops = dv.alloc<u32>(SEGCAP);
-        xt.sg_ndel = dv.alloc<u32>(SEGCAP); xt.sg_nrows = dv.alloc<u32>(SEGCAP); xt.sg_last_head = dv.alloc<u32>(SEGCAP);
-        xt.sg_skip = dv.alloc<u32>(SEGCAP, true); xt.ch_trim = rt.ch_trim;
-        xt.fc_src = dv.alloc<u32>(SEGCAP); xt.fc_pos = dv.alloc<u32>(SEGCAP); xt.fc_r0 = dv.alloc<u32>(SEGCAP);
-        xt.fc_from = dv.alloc<u32>(SEGCAP); xt.fc_atoms = dv.alloc<u32>(SEGCAP); xt.fc_nrows = dv.alloc<u32>(SEGCAP);
-        xt.fc_ndel = dv.alloc<u32>(SEGCAP); xt.fc_block = dv.alloc<u8>(SEGCAP); xt.fc_skip = dv.alloc<u32>(SEGCAP, true);
-        xt.fc_est = dv.alloc<u32>(SEGCAP);
-        xt.only_doc = 0xFFFFFFFFu; xt.from_ctr = nullptr;
+        t.sg_src = dv.alloc<u32>(SEGCAP); t.sg_r0 = dv.alloc<u32>(SEGCAP); t.sg_from = dv.alloc<u32>(SEGCAP);
+        t.sg_atoms = dv.alloc<u32>(SEGCAP); t.sg_est = dv.alloc<u32>(SEGCAP); t.sg_nmops = dv.alloc<u32>(SEGCAP);
+        t.sg_ndel = dv.alloc<u32>(SEGCAP); t.sg_nrows = dv.alloc<u32>(SEGCAP); t.sg_last_head = dv.alloc<u32>(SEGCAP);
+        t.sg_skip = dv.alloc<u32>(SEGCAP, true);
+        t.fc_src = dv.alloc<u32>(SEGCAP); t.fc_pos = dv.alloc<u32>(SEGCAP); t.fc_r0 = dv.alloc<u32>(SEGCAP);
+        t.fc_from = dv.alloc<u32>(SEGCAP); t.fc_atoms = dv.alloc<u32>(SEGCAP); t.fc_nrows = dv.alloc<u32>(SEGCAP);
+        t.fc_ndel = dv.alloc<u32>(SEGCAP); t.fc_block = dv.alloc<u8>(SEGCAP); t.fc_skip = dv.alloc<u32>(SEGCAP, true);
+        t.fc_est = dv.alloc<u32>(SEGCAP);
+        t.only_doc = 0xFFFFFFFFu; t.from_ctr = nullptr;
         trace_point(b, "export allocs");
-        LB_LAUNCH(k_exp_init, nblk(D), TPB, 0, st, b->d_docs, D, xt);
-        if (NTR) { LB_LAUNCH(k_exp_posrank, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, xt); tm.kernel_launches += 1; }
-        if (NCH) LB_LAUNCH(k_exp_arena, nblk(NCH, 64), 64, 0, st, NCH, xt, b->d_docs);
-        run_scans(b, {ScanJob{(const u8*)xt.ch_aval, (u8*)xt.ch_aval0, 4, 8, NCH}, ScanJob{(const u8*)xt.ch_astr, (u8*)xt.ch_astr0, 4, 8, NCH}});
+        LB_LAUNCH(k_exp_init, nblk(D), TPB, 0, st, b->d_docs, D, t);
+        if (NTR) { LB_LAUNCH(k_exp_posrank, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, t); tm.kernel_launches += 1; }
+        if (NCH) LB_LAUNCH(k_exp_arena, nblk(NCH, 64), 64, 0, st, NCH, t, b->d_docs);
+        run_scans(b, {ScanJob{(const u8*)t.ch_aval, (u8*)t.ch_aval0, 4, 8, NCH}, ScanJob{(const u8*)t.ch_astr, (u8*)t.ch_astr0, 4, 8, NCH}});
         trace_point(b, "posrank+arena");
-        if (NCH) LB_LAUNCH(k_exp_changes, nblk(NCH, 64), 64, 0, st, b->d_docs, NCH, xt, 0);
+        if (NCH) LB_LAUNCH(k_exp_changes, nblk(NCH, 64), 64, 0, st, b->d_docs, NCH, t, 0);
         tm.kernel_launches += 3;
         trace_point(b, "changes pass 0");
-        run_scans(b, {ScanJob{(const u8*)xt.ch_novf, (u8*)xt.ch_seg0, 4, 8, NCH}, ScanJob{(const u8*)xt.ch_syn, (u8*)xt.ch_syn0, 4, 8, NCH}});
-        u64 NOVF = d2h_one(b, xt.ch_seg0 + NCH);
-        u64 NSYN = d2h_one(b, xt.ch_syn0 + NCH);
-        xt.has_syn = NSYN ? 1 : 0;
-        xt.s_rec = dv.alloc<uint4>(NSYN); xt.s_len = dv.alloc<u32>(NSYN); xt.s_bytes = dv.alloc<u32>(NSYN);
-        xt.s_flag = dv.alloc<u8>(NSYN); xt.s_voff = dv.alloc<u64>(NSYN); xt.s_vlen = dv.alloc<u32>(NSYN); xt.s_aux = dv.alloc<u32>(NSYN);
+        run_scans(b, {ScanJob{(const u8*)t.ch_novf, (u8*)t.ch_seg0, 4, 8, NCH}, ScanJob{(const u8*)t.ch_syn, (u8*)t.ch_syn0, 4, 8, NCH}});
+        u64 NOVF = d2h_one(b, t.ch_seg0 + NCH);
+        u64 NSYN = d2h_one(b, t.ch_syn0 + NCH);
+        t.has_syn = NSYN ? 1 : 0;
+        t.s_rec = dv.alloc<uint4>(NSYN); t.s_len = dv.alloc<u32>(NSYN); t.s_bytes = dv.alloc<u32>(NSYN);
+        t.s_flag = dv.alloc<u8>(NSYN); t.s_voff = dv.alloc<u64>(NSYN); t.s_vlen = dv.alloc<u32>(NSYN); t.s_aux = dv.alloc<u32>(NSYN);
         if (NCH + NOVF > SEGCAP) {   // unusually many split changes: grow the tables, keep what pass 0 wrote
             u64 cap = NCH + NOVF;
-            u32** sgs[10] = {&xt.sg_src, &xt.sg_r0, &xt.sg_from, &xt.sg_atoms, &xt.sg_est, &xt.sg_nmops, &xt.sg_ndel, &xt.sg_nrows, &xt.sg_last_head, &xt.sg_skip};
+            u32** sgs[10] = {&t.sg_src, &t.sg_r0, &t.sg_from, &t.sg_atoms, &t.sg_est, &t.sg_nmops, &t.sg_ndel, &t.sg_nrows, &t.sg_last_head, &t.sg_skip};
             for (auto pp : sgs) {
                 u32* nw = dv.alloc<u32>(cap);
                 CK(cudaMemcpyAsync(nw, *pp, sizeof(u32) * NCH, cudaMemcpyDeviceToDevice, st));
                 dv.release(*pp);
                 *pp = nw;
             }
-            u32** fcs[9] = {&xt.fc_src, &xt.fc_pos, &xt.fc_r0, &xt.fc_from, &xt.fc_atoms, &xt.fc_nrows, &xt.fc_ndel, &xt.fc_skip, &xt.fc_est};
+            u32** fcs[9] = {&t.fc_src, &t.fc_pos, &t.fc_r0, &t.fc_from, &t.fc_atoms, &t.fc_nrows, &t.fc_ndel, &t.fc_skip, &t.fc_est};
             for (auto pp : fcs) { dv.release(*pp); *pp = dv.alloc<u32>(cap, true); }
-            dv.release(xt.fc_block);
-            xt.fc_block = dv.alloc<u8>(cap);
+            dv.release(t.fc_block);
+            t.fc_block = dv.alloc<u8>(cap);
         }
-        if (NOVF) { LB_LAUNCH(k_exp_changes, nblk(NCH, 64), 64, 0, st, b->d_docs, NCH, xt, 1); tm.kernel_launches += 1; }
-        LB_LAUNCH(k_exp_store, nblk(D, 64), 64, 0, st, b->d_docs, D, xt);
+        if (NOVF) { LB_LAUNCH(k_exp_changes, nblk(NCH, 64), 64, 0, st, b->d_docs, NCH, t, 1); tm.kernel_launches += 1; }
+        LB_LAUNCH(k_exp_store, nblk(D, 64), 64, 0, st, b->d_docs, D, t);
         tm.kernel_launches += 1;
         u64 XT = 0;
-        b->d_export = export_encode(b, xt, &XT);
+        b->d_export = export_encode(b, t, &XT);
         b->export_total = XT;
         tm.export_bytes = XT;
-        b->xt = xt;
-        b->have_xt = true;
     }
     mark(b);  // [7] export done
     // ------------------------------------------------------------ results to host
@@ -857,9 +786,9 @@ void pipeline(lb_batch* b) {
     CK(cudaMemcpyAsync(acc, d_acc, sizeof(acc), cudaMemcpyDeviceToHost, st));
     unsigned long long dws[4] = {0, 0, 0, 0};
     CK(cudaMemcpyAsync(dws, t.dw_stats, sizeof(dws), cudaMemcpyDeviceToHost, st));
-    if (b->d_xdoc) {
+    if (t.xdoc) {
         b->xdocs.resize(D);
-        CK(cudaMemcpyAsync(b->xdocs.data(), b->d_xdoc, sizeof(XDoc) * D, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(b->xdocs.data(), t.xdoc, sizeof(XDoc) * D, cudaMemcpyDeviceToHost, st));
     }
     CK(cudaStreamSynchronize(st));
     // the peer table is sized by the blocks' peer registers (a few entries per BLOCK: hundreds of MB for 10^6 blocks) but a
@@ -873,7 +802,7 @@ void pipeline(lb_batch* b) {
             u64* d_pbase = dv.alloc<u64>(D + 1);
             DocPeer* d_packed = dv.alloc<DocPeer>(total);
             CK(cudaMemcpyAsync(d_pbase, b->peer_base.data(), sizeof(u64) * (D + 1), cudaMemcpyHostToDevice, st));
-            LB_LAUNCH(k_pack_peers, nblk(D), TPB, 0, st, b->d_docs, D, b->d_dpeer, d_pbase, d_packed);
+            LB_LAUNCH(k_pack_peers, nblk(D), TPB, 0, st, b->d_docs, D, t.dpeer, d_pbase, d_packed);
             tm.kernel_launches += 1;
             CK(cudaMemcpyAsync(b->dpeer.data(), d_packed, sizeof(DocPeer) * total, cudaMemcpyDeviceToHost, st));
         }
@@ -892,7 +821,6 @@ void pipeline(lb_batch* b) {
     tm.decode_fast_blocks = dws[0]; tm.decode_lane_blocks = dws[1]; tm.decode_unstaged_blocks = dws[2];
     c.json_bytes = 0;
     for (u32 d = 0; d < D; d++) c.json_bytes += b->docs[d].json_len;
-    (void)NDEL;
 }
 
 // ImportStatus / vv / frontiers spans of every document, flat: [off[d], off[d + 1]) of one array per kind (a vector per
@@ -1026,7 +954,7 @@ lb_status export_from(lb_batch* b, size_t doc, const lb_id_span* from, size_t n_
         const u32 D = (u32)b->n_docs;
         const u64 NCH = b->n_changes;
         const DocInfo& di = b->docs[doc];
-        ExportTables xt = b->xt;
+        BatchTables xt = b->tb;
         // only the document's own peer slots are read (every kernel is restricted to `only_doc`)
         std::vector<i32> h_from(di.P + 1, 0);
         for (size_t k = 0; k < n_from; k++)
@@ -1106,7 +1034,7 @@ void docset_store(lb_docset* set, lb_batch* b, const std::vector<u64>& offs, con
             w += ((u64)len + 15) & ~(u64)15;
         };
         if (pk.exported) push(b->d_export + b->xdocs[pk.doc].exp_off, b->xdocs[pk.doc].exp_len);
-        else for (u32 q = b->doc_blob0[pk.doc]; q < b->doc_blob0[pk.doc + 1]; q++) push(b->d_bytes + offs[q], lens[q]);
+        else for (u32 q = b->doc_blob0[pk.doc]; q < b->doc_blob0[pk.doc + 1]; q++) push(b->tb.bytes + offs[q], lens[q]);
         fresh.push_back({b->doc_ids[pk.doc], std::move(nd_)});
     }
     CopySeg* d_segs = b->dev.alloc<CopySeg>(segs.size());
@@ -1263,7 +1191,7 @@ static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_opti
         }
         CK(cudaMemcpyAsync(b->d_offs, offs.data(), sizeof(u64) * (Q + 1), cudaMemcpyHostToDevice, b->dev.stream));
         CK(cudaMemcpyAsync(b->d_lens, lens.data(), sizeof(u32) * (Q + 1), cudaMemcpyHostToDevice, b->dev.stream));
-        b->d_bytes = d_bytes;
+        b->tb.bytes = d_bytes;
         b->timings.decode_bytes_read = b->counters.blob_bytes;
         mark(b);  // [1] h2d done (index 0 = start)
         // event indices: 0 start,1 h2d,2 frame,3 decode,4 resolve,5 classify,6 integrate,7 materialise,8 d2h
@@ -1336,7 +1264,7 @@ lb_status lb_import_batch_device(const uint8_t* d_bytes, const uint64_t* offsets
         b->d_lens = b->dev.alloc<u32>(n_docs + 1);
         CK(cudaMemcpyAsync(b->d_offs, offs.data(), sizeof(u64) * (n_docs + 1), cudaMemcpyHostToDevice, b->dev.stream));
         CK(cudaMemcpyAsync(b->d_lens, lens.data(), sizeof(u32) * (n_docs + 1), cudaMemcpyHostToDevice, b->dev.stream));
-        b->d_bytes = d_bytes;
+        b->tb.bytes = d_bytes;
         b->timings.decode_bytes_read = b->counters.blob_bytes;
         mark(b);  // [1]
         s = run_batch(b);
@@ -1407,7 +1335,7 @@ lb_status lb_doc_export_updates(const lb_batch* cb, size_t doc, const lb_id_span
     if (!(b->flags & LB_FLAG_EXPORT)) { g_last_error = "batch was imported without LB_FLAG_EXPORT"; return LB_ERR_INVALID_ARG; }
     if (b->docs[doc].code != DOC_OK) { g_last_error = "document failed to import"; return LB_ERR_INVALID_ARG; }
     if (from && n_from) {   // export(ExportMode::updates(from)): computed on demand for this document
-        if (!b->have_xt) { g_last_error = "batch holds no export tables"; return LB_ERR_INVALID_ARG; }
+        if (!b->tb.xdoc) { g_last_error = "batch holds no export tables"; return LB_ERR_INVALID_ARG; }
         std::vector<uint8_t>& buf = b->from_exports[doc];
         lb_status rc = export_from(b, doc, from, n_from, buf);
         if (rc != LB_OK) return rc;
@@ -1451,12 +1379,12 @@ lb_status lb_debug_table(const lb_batch* b, const char* name, void* dst, size_t 
     std::string nm(name);
     const void* src = nullptr;
     size_t n = 0, es = 0;
-    const Tables& t = b->tb;
+    const BatchTables& t = b->tb;
 #define TAB(str, ptr, cnt) if (nm == str) { src = ptr; n = cnt; es = sizeof(*ptr); }
     TAB("op_cid", t.op_cid, b->n_rows) TAB("op_prop", t.op_prop, b->n_rows) TAB("op_vtype", t.op_vtype, b->n_rows)
     TAB("op_len", t.op_len, b->n_rows) TAB("op_counter", t.op_counter, b->n_rows)
     TAB("ch_counter", t.ch_counter, b->n_changes) TAB("ch_len", t.ch_len, b->n_changes)
-    TAB("ch_lamport", t.ch_lamport, b->n_changes) TAB("ch_ts", t.ch_ts, b->n_changes)
+    TAB("ch_lamport", t.ch_lamport_wire, b->n_changes) TAB("ch_ts", t.ch_ts, b->n_changes)
     TAB("dep_peer", t.dep_peer_idx, b->n_deps) TAB("dep_counter", t.dep_counter, b->n_deps)
 #undef TAB
     if (nm == "blk_doc" || nm == "blk_nchanges") {   // fields of the block descriptors
@@ -1465,7 +1393,7 @@ lb_status lb_debug_table(const lb_batch* b, const char* name, void* dst, size_t 
         if (dst) {
             if (dst_bytes < b->n_blocks * 4) { g_last_error = "buffer too small"; return LB_ERR_INVALID_ARG; }
             std::vector<BlockInfo> hb(b->n_blocks);
-            if (b->n_blocks && cudaMemcpy(hb.data(), b->d_blocks, sizeof(BlockInfo) * b->n_blocks, cudaMemcpyDeviceToHost) != cudaSuccess) return LB_ERR_CUDA;
+            if (b->n_blocks && cudaMemcpy(hb.data(), b->tb.blocks, sizeof(BlockInfo) * b->n_blocks, cudaMemcpyDeviceToHost) != cudaSuccess) return LB_ERR_CUDA;
             for (size_t i = 0; i < hb.size(); i++) ((u32*)dst)[i] = nm == "blk_doc" ? hb[i].doc : hb[i].n_changes;
         }
         return LB_OK;

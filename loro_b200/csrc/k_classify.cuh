@@ -6,31 +6,7 @@
 // Fully data-parallel: one thread per op row; the LWW reduce is an atomicMax over a packed
 // (lamport, peer rank) key followed by a pass that elects the matching row.
 #pragma once
-#include "lb_defs.h"
-
-struct ClassifyTables {
-    const BlockInfo* blocks;
-    const u32* ch_block; const u8* ch_applied; const u32* ch_lamport; const i32* ch_counter; const u16* ch_peer;
-    const u32* ch_trim;     // atoms at the head of the change the document already had (k_doc_causal)
-    const u8* bytes; const u64* op_val_off; const u32* op_val_len;   // value payloads (List insert: item count check)
-    const u32* op_cid; const i32* op_prop; const u8* op_vtype; const u32* op_len; const i32* op_counter;
-    const u32* op_change;
-    const u32* op_del; const u32* del_peer_idx; const i32* del_counter; const i32* del_len; const u32* peer_map;
-    // movable tree: decoded RawTreeMove fields in, resolved records out (k_tree.cuh)
-    const u32* tr_target_peer; const i32* tr_target_ctr; const u8* tr_parent_kind; const u32* tr_parent_peer;
-    const i32* tr_parent_ctr; const u32* tr_pos;
-    u64* tr_key;            // (lamport << 32 | peer rank << 16): the total order of a tree's ops (diff_calc/tree.rs:445-452)
-    uint4* tr_ids;          // x = target peer (document level), y = target counter, z = parent kind | parent peer << 2, w = parent counter
-    uint4* tr_rec;          // x = target atom (document-relative), y = parent atom | TREE_ROOT | TREE_DELETED, z = position, w = row
-    const u32* cid_map; const u32* key_map;
-    DocContainer* dcont; const DocPeer* dpeer;
-    // outputs
-    u8* op_kind; u32* op_cidx; u32* op_lamport;
-    uint4* op_rec; u32* op_aux;   // compact records for the tracker (layout: k_seq.cuh REC_*)
-    u32* atom_row;          // per doc: atom -> op row (batch-wide row index, 32-bit)
-    unsigned long long* map_best;  // per (doc, container, key): max packed (lamport<<32 | rank<<16 | 1)
-    u32* map_row;           // winner row per slot
-};
+#include "lb_tables.cuh"
 
 __device__ __forceinline__ u8 classify_op(u8 ctype, u8 vt) {
     switch (ctype) {
@@ -53,7 +29,7 @@ __device__ __forceinline__ u8 classify_op(u8 ctype, u8 vt) {
     }
 }
 
-__global__ void k_op_classify(DocInfo* __restrict__ docs, u64 n_rows, ClassifyTables t) {
+__global__ void k_op_classify(DocInfo* __restrict__ docs, u64 n_rows, const __grid_constant__ BatchTables t) {
     u64 row = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (row >= n_rows) return;
     u32 ch = t.op_change[row];
@@ -178,7 +154,7 @@ __global__ void k_op_classify(DocInfo* __restrict__ docs, u64 n_rows, ClassifyTa
     }
 }
 
-__global__ void k_map_winner(const DocInfo* __restrict__ docs, u64 n_rows, ClassifyTables t) {
+__global__ void k_map_winner(const DocInfo* __restrict__ docs, u64 n_rows, const __grid_constant__ BatchTables t) {
     u64 row = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (row >= n_rows) return;
     u8 kind = t.op_kind[row];

@@ -9,7 +9,7 @@
 // Round-1 shape: one thread per block, two passes (count -> host allocates -> fill).  Blocks are ~4 KB and a
 // batch holds 10^5..10^6 of them, so the parallelism is across blocks.
 #pragma once
-#include "lb_defs.h"
+#include "lb_tables.cuh"
 
 // ---- skip one LoroValue (kind byte already consumed) ; iterative, bounded depth
 // reference: value.rs:620-700 read_value_content
@@ -250,29 +250,6 @@ __global__ void k_block_count(const u8* __restrict__ bytes, BlockInfo* __restric
     blocks[i] = bi;
 }
 
-// ---------------------------------------------------------------- batch-wide SoA tables (device pointers)
-struct Tables {
-    // block-local peer tables
-    u64* peer_id;
-    // keys (block-local arena)
-    u64* key_off; u32* key_len;
-    // cids (block-local arena)
-    u8* cid_root; u8* cid_type; u32* cid_peer_idx; i32* cid_koc;  // key idx or counter
-    // changes
-    u32* ch_block; i32* ch_counter; u32* ch_len; u32* ch_lamport; i64* ch_ts; u64* ch_msg_off; u32* ch_msg_len;
-    u64* ch_dep0; u32* ch_ndeps; u8* ch_dep_self; u64* ch_op0; u32* ch_nops;
-    // deps (other peers)
-    u32* dep_peer_idx; i32* dep_counter;
-    // op rows
-    u32* op_cid; i32* op_prop; u8* op_vtype; u32* op_len; i32* op_counter; u32* op_change;
-    u64* op_val_off; u32* op_val_len; u32* op_del;  // op_del: index into del tables for DeleteSeq rows
-    // delete start ids
-    u32* del_peer_idx; i32* del_counter; i32* del_len;
-    // fractional indexes (expanded) + movable-tree ops (op_del of a RawTreeMove row indexes tr_*)
-    u64* pos_off; u32* pos_len; u8* pos_pool;
-    u32* tr_target_peer; i32* tr_target_ctr; u8* tr_parent_kind; u32* tr_parent_peer; i32* tr_parent_ctr; u32* tr_pos;
-    unsigned long long* dw_stats;   // [0] blocks decoded lane-parallel, [1] staged but rows on one lane, [2] not staged
-};
 enum { TRP_ROOT = 0, TRP_NODE = 1, TRP_DELETED = 2 };
 
 // ---------------------------------------------------------------- pass 2: fill
@@ -283,7 +260,7 @@ enum { TRP_ROOT = 0, TRP_NODE = 1, TRP_DELETED = 2 };
 // k_block_decode_cols (the default) runs them one thread per block.  k_block_decode_warp (k_decode_warp.cuh) stages the
 // block in shared memory and replaces decode_block_rows_cols by lane-parallel column expansion and value-chain
 // resolution; the blocks its fast path does not cover still go through decode_block_rows_cols, on one lane.
-__device__ inline u32 decode_block_small(const u8* b, const BlockInfo& bi, u64 i, const Tables& t) {
+__device__ inline u32 decode_block_small(const u8* b, const BlockInfo& bi, u64 i, const BatchTables& t) {
     u32 N = bi.n_changes;
     u32 err = 0;
     // ---- header
@@ -373,9 +350,9 @@ __device__ inline u32 decode_block_small(const u8* b, const BlockInfo& bi, u64 i
     {
         DodCur d;
         d.begin(&h);
-        for (u32 k = 0; k + 1 < N; k++) t.ch_lamport[bi.ch0 + k] = (u32)d.next(k == 0);
+        for (u32 k = 0; k + 1 < N; k++) t.ch_lamport_wire[bi.ch0 + k] = (u32)d.next(k == 0);
         d.finish();
-        t.ch_lamport[bi.ch0 + N - 1] = bi.lamport_start + bi.lamport_len - t.ch_len[bi.ch0 + N - 1];
+        t.ch_lamport_wire[bi.ch0 + N - 1] = bi.lamport_start + bi.lamport_len - t.ch_len[bi.ch0 + N - 1];
     }
     if (h.err || !h.empty()) err = err ? err : LB_ERR(DOC_ERR_DECODE);
     // ---- change meta: timestamps DoD (N), commit-message lengths AnyRle<u32> (N), message bytes
@@ -486,7 +463,7 @@ __device__ __forceinline__ u32 column_pass(const u8* col, u32 len, u32 n, Emit e
     if (r == n && c.next(&extra)) return 0xFFFFFFFFu;   // more rows than announced
     return r;
 }
-__device__ inline u32 decode_block_rows_cols(const u8* b, const BlockInfo& bi, const Tables& t, u32 err, u32* n_maps_out) {
+__device__ inline u32 decode_block_rows_cols(const u8* b, const BlockInfo& bi, const BatchTables& t, u32 err, u32* n_maps_out) {
     const u32 N = bi.n_changes, R = bi.n_ops;
     // ---- delete start ids
     if (bi.sec_len[6]) {
@@ -579,7 +556,7 @@ __device__ inline u32 decode_block_rows_cols(const u8* b, const BlockInfo& bi, c
     return err;
 }
 
-__device__ inline void decode_block_fail(const BlockInfo& bi, u64 i, const Tables& t, BlockInfo* blocks, u32 err) {
+__device__ inline void decode_block_fail(const BlockInfo& bi, u64 i, const BatchTables& t, BlockInfo* blocks, u32 err) {
     {
         // row-parallel kernels find their document through op_change: every row of a failed block must point
         // at one of the block's own changes, whatever the walk above managed to write
@@ -590,7 +567,7 @@ __device__ inline void decode_block_fail(const BlockInfo& bi, u64 i, const Table
 }
 
 // thread per block, one column at a time
-__global__ void k_block_decode_cols(const u8* __restrict__ bytes, BlockInfo* __restrict__ blocks, u64 n_blocks, Tables t) {
+__global__ void k_block_decode_cols(const u8* __restrict__ bytes, BlockInfo* __restrict__ blocks, u64 n_blocks, const __grid_constant__ BatchTables t) {
     u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_blocks) return;
     BlockInfo bi = blocks[i];

@@ -190,7 +190,7 @@ __device__ __forceinline__ bool dw_zero_len_kind(u8 vt) {
 
 // ---- the rows of a staged block, lane-parallel.  false = not covered (or malformed): the caller runs the
 // single-lane decoder, which rewrites every row.
-__device__ inline bool dw_rows_fast(const u8* b, const BlockInfo& bi, const Tables& t, u16* tab, int lane) {
+__device__ inline bool dw_rows_fast(const u8* b, const BlockInfo& bi, const BatchTables& t, u16* tab, int lane) {
     bool bad = false;
     const u32 R = bi.n_ops;
     // ---- delete start ids: three DeltaRle columns
@@ -369,7 +369,7 @@ __device__ inline bool dw_rows_fast(const u8* b, const BlockInfo& bi, const Tabl
 }
 
 __global__ void __launch_bounds__(32 * DW_WARPS)
-k_block_decode_warp(const u8* __restrict__ bytes, BlockInfo* __restrict__ blocks, u64 n_blocks, Tables t) {
+k_block_decode_warp(const u8* __restrict__ bytes, BlockInfo* __restrict__ blocks, u64 n_blocks, const __grid_constant__ BatchTables t) {
 #ifdef LB_SIMT_EMU
     LB_DYN_SMEM(DwWarp, smem);
 #else

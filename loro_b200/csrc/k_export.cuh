@@ -30,7 +30,7 @@
 // export but their payloads still count for the arena positions; a document built from several blobs sees them
 // in import_batch's order (the host lays them out that way).
 #pragma once
-#include "lb_defs.h"
+#include "lb_tables.cuh"
 
 enum { XK_NONE = 0, XK_LIST = 1, XK_TEXT = 2, XK_DEL = 3, XK_MAPSET = 4, XK_MAPDEL = 5, XK_TREE = 6 };
 #define LB_MAX_BLOCK_SIZE 4096   // change_store.rs:37
@@ -63,52 +63,6 @@ struct XBlock {        // one output block
     u64 stage;         // staging slot: first byte, capacity; the block's pieces without their length prefixes
     u32 stage_cap;
     u32 ovf;           // 1 = the pieces did not fit the slot: encoded straight into the blob instead
-};
-
-struct ExportTables {
-    const u8* bytes; const BlockInfo* blocks; const DocPeer* dpeer; const DocContainer* dcont;
-    const u64* dkey_off; const u32* dkey_len; const u32* key_map; const u32* peer_map;
-    const u32* ch_order; const u8* ch_applied; const u32* ch_block; const i32* ch_counter; const u32* ch_len;
-    const u32* ch_lamport; const i64* ch_ts; const u64* ch_op0; const u32* ch_nops;
-    const u64* ch_dep0; const u32* ch_ndeps; const u8* ch_dep_self; const u32* dep_peer_idx; const i32* dep_counter;
-    const u64* ch_msg_off; const u32* ch_msg_len;
-    const u8* op_kind; const u8* op_vtype; const u32* op_cidx; const i32* op_prop; const u32* op_len; const i32* op_counter;
-    const u64* op_val_off; const u32* op_val_len; const u32* op_del; const u32* op_aux;
-    const i32* del_counter; const i32* del_len;
-    // movable tree: decoded RawTreeMove fields (k_decode.cuh) + the document-wide order of the fractional indexes
-    const uint4* tr_ids; const u32* tr_pos;   // (k_classify.cuh) subject / parent at document level ; position entry
-    const u64* pos_off; const u32* pos_len; const u8* pos_pool;
-    u32* pos_rank;     // per position entry: dense rank of its bytes among the document's positions
-    u32* pos_rep;      // per (document position base + rank): one entry holding those bytes
-    u64* ps_key; u32* ps_val;   // sort space of k_exp_posrank
-    // per row
-    uint4* x_rec;      // resolved op record per row (xop_pack): kind | reversed | container, counter, prop, arena start / target counter
-    u32* r_bytes;      // text rows: payload bytes
-    u8* r_flag;        // XF_*
-    // per change
-    u32* ch_nseg;      // segments the change enters the store as (0 = not applied)
-    u32* ch_novf;      // nseg - 1 (scan input): only split changes need slots beyond their own
-    // changes whose split cuts an op (Op::slice, list_op.rs:603-658) get SYNTHETIC rows: one per source row or slice,
-    // addressed as row = n_rows + ch_syn0[ch] + i; every row accessor below understands both spaces
-    u32* ch_syn; u64* ch_syn0; u64 n_rows;
-    u32 has_syn;       // any synthetic row in the batch (uniform: the common batch never leaves the decoded rows)
-    uint4* s_rec; u32* s_len; u32* s_bytes; u8* s_flag; u64* s_voff; u32* s_vlen; u32* s_aux;
-    u64 n_changes;     // segment q of change ch lives at q == 0 ? ch : n_changes + ch_seg0[ch] + q - 1
-    u32* ch_aval; u32* ch_astr; u64* ch_aval0; u64* ch_astr0;   // arena sums per change + their scans
-    u64* ch_seg0;      // scan of ch_novf
-    // per segment
-    u32* sg_src; u32* sg_r0; u32* sg_from; u32* sg_atoms; u32* sg_est; u32* sg_nmops; u32* sg_ndel; u32* sg_nrows; u32* sg_last_head;
-    u32* sg_skip;      // atoms of the segment's first row the document already had (import-side trim, k_doc_causal)
-    const u32* ch_trim;
-    // final changes (same index space: a document never ends up with more changes than segments)
-    u32* fc_src; u32* fc_pos; u32* fc_r0; u32* fc_from; u32* fc_atoms; u32* fc_nrows; u32* fc_ndel; u8* fc_block;
-    u32* fc_skip;      // atoms of the change's first row that lie before the `from` version (Op::slice)
-    u32* fc_est;       // the store's size estimate of the change's ops (sizes the staging slot of its block)
-    // export(ExportMode::updates(from)) of ONE document on demand (lb_doc_export_updates): only_doc != ~0 restricts
-    // every kernel to that document; from_ctr[doc peer slot] = first counter to export (encoding.rs:79-83,
-    // change_store.rs:494-528 export_blocks_from, change.rs:203-258 Change::slice)
-    u32 only_doc; const i32* from_ctr;
-    XDoc* xdoc;
 };
 
 // ---------------------------------------------------------------------------------------------- byte sink
@@ -214,7 +168,7 @@ __device__ inline void xop_merge(XOp& a, const XOp& b) {
 // one decoded row as an op (map keys and delete targets at document level): the resolving form walks the decode
 // tables (container type, block key arena, delete table); k_exp_changes runs it once per row and leaves a 16-byte
 // record, which is what every later pass loads (three independent loads per row instead of a chain)
-__device__ inline XOp xop_resolve(const ExportTables& t, const DocInfo& di, u32 ch, u64 row, u32 astart) {
+__device__ inline XOp xop_resolve(const BatchTables& t, const DocInfo& di, u32 ch, u64 row, u32 astart) {
     XOp o;
     u8 kind = t.op_kind[row];
     o.cidx = t.op_cidx[row];
@@ -251,20 +205,20 @@ __device__ __forceinline__ uint4 xop_pack(const XOp& o) {
     return r;
 }
 // ---- row accessors: decoded rows [0, n_rows) and synthetic rows [n_rows, ...)
-__device__ __forceinline__ uint4 xr_rec(const ExportTables& t, u64 row) { return (!t.has_syn || row < t.n_rows) ? t.x_rec[row] : t.s_rec[row - t.n_rows]; }
-__device__ __forceinline__ u32 xr_len(const ExportTables& t, u64 row) { return (!t.has_syn || row < t.n_rows) ? t.op_len[row] : t.s_len[row - t.n_rows]; }
-__device__ __forceinline__ u32 xr_bytes(const ExportTables& t, u64 row) { return (!t.has_syn || row < t.n_rows) ? t.r_bytes[row] : t.s_bytes[row - t.n_rows]; }
-__device__ __forceinline__ u32 xr_aux(const ExportTables& t, u64 row) { return (!t.has_syn || row < t.n_rows) ? t.op_aux[row] : t.s_aux[row - t.n_rows]; }
-__device__ __forceinline__ u8* xr_flagp(const ExportTables& t, u64 row) { return (!t.has_syn || row < t.n_rows) ? &t.r_flag[row] : &t.s_flag[row - t.n_rows]; }
-__device__ __forceinline__ u8 xr_flag(const ExportTables& t, u64 row) { return *xr_flagp(t, row); }
+__device__ __forceinline__ uint4 xr_rec(const BatchTables& t, u64 row) { return (!t.has_syn || row < t.n_rows) ? t.x_rec[row] : t.s_rec[row - t.n_rows]; }
+__device__ __forceinline__ u32 xr_len(const BatchTables& t, u64 row) { return (!t.has_syn || row < t.n_rows) ? t.op_len[row] : t.s_len[row - t.n_rows]; }
+__device__ __forceinline__ u32 xr_bytes(const BatchTables& t, u64 row) { return (!t.has_syn || row < t.n_rows) ? t.r_bytes[row] : t.s_bytes[row - t.n_rows]; }
+__device__ __forceinline__ u32 xr_aux(const BatchTables& t, u64 row) { return (!t.has_syn || row < t.n_rows) ? t.op_aux[row] : t.s_aux[row - t.n_rows]; }
+__device__ __forceinline__ u8* xr_flagp(const BatchTables& t, u64 row) { return (!t.has_syn || row < t.n_rows) ? &t.r_flag[row] : &t.s_flag[row - t.n_rows]; }
+__device__ __forceinline__ u8 xr_flag(const BatchTables& t, u64 row) { return *xr_flagp(t, row); }
 // the rows of a change as the export sees them
-__device__ __forceinline__ void change_rows(const ExportTables& t, u32 ch, u64* row0, u32* nr) {
+__device__ __forceinline__ void change_rows(const BatchTables& t, u32 ch, u64* row0, u32* nr) {
     u32 ns = t.has_syn ? t.ch_syn[ch] : 0;
     if (ns) { *row0 = t.n_rows + t.ch_syn0[ch]; *nr = ns; }
     else { *row0 = t.ch_op0[ch]; *nr = t.ch_nops[ch]; }
 }
 // payload bytes a row contributes to the values section (items of a list insert, text bytes, a whole map value)
-__device__ __forceinline__ void xr_payload(const ExportTables& t, u64 row, u32 xk, const u8** p, u32* n) {
+__device__ __forceinline__ void xr_payload(const BatchTables& t, u64 row, u32 xk, const u8** p, u32* n) {
     if (t.has_syn && row >= t.n_rows) { *p = t.bytes + t.s_voff[row - t.n_rows]; *n = t.s_vlen[row - t.n_rows]; return; }
     const u8* v = t.bytes + t.op_val_off[row];
     u32 vl = t.op_val_len[row];
@@ -283,7 +237,7 @@ __device__ __forceinline__ void xr_payload(const ExportTables& t, u64 row, u32 x
     else if (xk == XK_MAPSET) { *p = v; *n = vl; }
     else { *p = v; *n = 0; }
 }
-__device__ __forceinline__ XOp xop_from_row(const ExportTables& t, const DocInfo&, u32, u64 row) {
+__device__ __forceinline__ XOp xop_from_row(const BatchTables& t, const DocInfo&, u32, u64 row) {
     uint4 r = xr_rec(t, row);
     XOp o;
     o.xk = (u8)(r.x & 7u);
@@ -310,7 +264,7 @@ __device__ inline u32 text_byte_index(const u8* p, u32 nb, u32 n, u32 k) {
     return i;
 }
 // payload of a row without its first `skip` atoms (list items / unicode scalar values)
-__device__ inline void xr_payload_skip(const ExportTables& t, u64 row, u32 xk, u32 skip, const u8** p, u32* n) {
+__device__ inline void xr_payload_skip(const BatchTables& t, u64 row, u32 xk, u32 skip, const u8** p, u32* n) {
     xr_payload(t, row, xk, p, n);
     if (!skip) return;
     u32 off = 0;
@@ -324,7 +278,7 @@ __device__ inline void xr_payload_skip(const ExportTables& t, u64 row, u32 xk, u
     *n -= off;
 }
 // Op::slice(skip, len) of the op made from `row` (op.rs:161-172, list_op.rs:603-658, 251-278, 436-444)
-__device__ inline void xop_slice_front(const ExportTables& t, XOp& o, u64 row, u32 skip) {
+__device__ inline void xop_slice_front(const BatchTables& t, XOp& o, u64 row, u32 skip) {
     if (!skip) return;
     switch (o.xk) {
         case XK_LIST: o.prop += (i32)skip; o.f0 += skip; break;
@@ -349,7 +303,7 @@ __device__ inline void xop_slice_front(const ExportTables& t, XOp& o, u64 row, u
 // The importing document allocates arena space while it decodes (block_encode.rs:619-657): the position of a row's
 // payload is the sum over the rows decoded before it.  Changes are numbered in decode order, so: per-change sums
 // (thread per change), one scan over the changes, and k_exp_changes hands out the row positions.
-__global__ void k_exp_init(const DocInfo* __restrict__ docs, u32 n_docs, ExportTables t) {
+__global__ void k_exp_init(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
     const DocInfo& di = docs[d];
@@ -363,7 +317,7 @@ __global__ void k_exp_init(const DocInfo* __restrict__ docs, u32 n_docs, ExportT
     }
     t.xdoc[d] = x;
 }
-__global__ void k_exp_arena(u64 n_changes, ExportTables t, const DocInfo* __restrict__ docs) {
+__global__ void k_exp_arena(u64 n_changes, const __grid_constant__ BatchTables t, const DocInfo* __restrict__ docs) {
     u64 ch = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (ch >= n_changes) return;
     const BlockInfo& sb = t.blocks[t.ch_block[ch]];
@@ -398,7 +352,7 @@ __global__ void k_exp_arena(u64 n_changes, ExportTables t, const DocInfo* __rest
 // row `row`, whether it starts an op and whether it starts a segment -- to `emit`.
 struct XSplit { u32 nseg, nsyn; bool sliced; };
 template <class Emit>
-__device__ inline XSplit split_change(const ExportTables& t, const DocInfo& di, u32 ch, u64 r0, u32 nr, u32 est0, Emit emit) {
+__device__ inline XSplit split_change(const BatchTables& t, const DocInfo& di, u32 ch, u64 r0, u32 nr, u32 est0, Emit emit) {
     XSplit out;
     out.nseg = 0; out.nsyn = 0; out.sliced = false;
     u64 est = est0;
@@ -476,7 +430,7 @@ __device__ inline XSplit split_change(const ExportTables& t, const DocInfo& di, 
 }
 
 // one summary record per segment of a change whose rows (decoded or synthetic) carry XF_HEAD / XF_SEG
-__device__ inline void segment_summaries(const ExportTables& t, const DocInfo& di, u32 ch) {
+__device__ inline void segment_summaries(const BatchTables& t, const DocInfo& di, u32 ch) {
     u64 row0;
     u32 nr;
     change_rows(t, ch, &row0, &nr);
@@ -505,7 +459,7 @@ __device__ inline void segment_summaries(const ExportTables& t, const DocInfo& d
 
 // thread per change.  pass 0: per-row records, RleVec merge inside the change (XF_HEAD), segment count (XF_SEG marks
 // when no op has to be cut, a synthetic-row count otherwise).  pass 1 (split changes only): synthetic rows, summaries.
-__global__ void k_exp_changes(DocInfo* __restrict__ docs, u64 n_changes, ExportTables t, int pass) {
+__global__ void k_exp_changes(DocInfo* __restrict__ docs, u64 n_changes, const __grid_constant__ BatchTables t, int pass) {
     u64 ch = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (ch >= n_changes) return;
     if (t.only_doc != 0xFFFFFFFFu && t.blocks[t.ch_block[ch]].doc != t.only_doc) return;
@@ -617,7 +571,7 @@ __global__ void k_exp_changes(DocInfo* __restrict__ docs, u64 n_changes, ExportT
 // ---------------------------------------------------------------------------------------------- B + C: the stores
 struct XEntry {        // a change on its way through a store: one segment, or a run of merged ones
     u32 src, from;     // metadata of its first segment: source change + atom offset (deps, lamport, timestamp, message)
-    u32 pos, r0;       // where its rows start: position in ch_order (absolute) + row inside that change
+    u32 pos, r0;       // where its rows start: position in ch_aorder (absolute) + row inside that change
     u32 atoms, est_ops, nmops, ndel, nrows;
     u32 skip;          // atoms of the first row already known to the importer of this export (from-version cut)
     u32 lh_ch, lh_row; // last op: source change + row (inside that change) of its first row ...
@@ -630,7 +584,7 @@ struct XStore {
     XEntry open;       // the store's last change (still able to absorb the next one)
     XOp back;          // last op of `open`, accumulated
 };
-__device__ __forceinline__ bool xmsg_same(const ExportTables& t, u32 a, u32 b) {
+__device__ __forceinline__ bool xmsg_same(const BatchTables& t, u32 a, u32 b) {
     u32 la = t.ch_msg_len[a], lb = t.ch_msg_len[b];
     if (la != lb) return false;
     const u8* pa = t.bytes + t.ch_msg_off[a];
@@ -639,22 +593,22 @@ __device__ __forceinline__ bool xmsg_same(const ExportTables& t, u32 a, u32 b) {
         if (pa[i] != pb[i]) return false;
     return true;
 }
-__device__ __forceinline__ u32 xentry_ndeps(const ExportTables& t, const XEntry& e) {
+__device__ __forceinline__ u32 xentry_ndeps(const BatchTables& t, const XEntry& e) {
     return e.from ? 1u : t.ch_ndeps[e.src] + (t.ch_dep_self[e.src] ? 1u : 0u);
 }
 // cursor over the rows of an entry in store order (rows of consecutive applied changes of the peer)
 struct XRows {
-    const ExportTables& t; u32 pos; u32 r; u32 ch; u32 nr; u64 row0;
+    const BatchTables& t; u32 pos; u32 r; u32 ch; u32 nr; u64 row0;
     u32 skip;   // atoms of the CURRENT row that are not part of the store (first kept row of a trimmed change); the
                 // creator of the cursor knows the skip of the row it starts on (entry / final-change records)
-    __device__ XRows(const ExportTables& t_, u32 pos_, u32 r_) : t(t_), pos(pos_), r(r_), skip(0) { load(); }
-    __device__ void load() { ch = t.ch_order[pos]; change_rows(t, ch, &row0, &nr); }
+    __device__ XRows(const BatchTables& t_, u32 pos_, u32 r_) : t(t_), pos(pos_), r(r_), skip(0) { load(); }
+    __device__ void load() { ch = t.ch_aorder[pos]; change_rows(t, ch, &row0, &nr); }
     __device__ u64 row() const { return row0 + r; }
     __device__ void next() {
         r++;
         skip = 0;
         while (r >= nr) {
-            pos++; r = 0; ch = t.ch_order[pos];
+            pos++; r = 0; ch = t.ch_aorder[pos];
             if (!t.ch_applied[ch]) { nr = 0; continue; }
             change_rows(t, ch, &row0, &nr);
             if (t.ch_trim[ch]) { r = t.sg_r0[ch]; skip = t.sg_skip[ch]; }   // a trimmed change starts at its first kept row
@@ -663,13 +617,13 @@ struct XRows {
 };
 // accumulate the merged op that starts at the cursor (consumes its rows, at most `left` of them)
 // bytes one row contributes to the values section of a (merged) op, without the op's own prefix
-__device__ __forceinline__ u32 row_value_bytes(const ExportTables& t, const XOp& o, u64 row) {
+__device__ __forceinline__ u32 row_value_bytes(const BatchTables& t, const XOp& o, u64 row) {
     const u8* p;
     u32 n;
     xr_payload(t, row, o.xk, &p, &n);
     return n;
 }
-__device__ inline XOp xop_gather(const ExportTables& t, const DocInfo& di, XRows& it, u32& left, u32* vbytes = nullptr, u32 skip = 0) {
+__device__ inline XOp xop_gather(const BatchTables& t, const DocInfo& di, XRows& it, u32& left, u32* vbytes = nullptr, u32 skip = 0) {
     XOp o = xop_from_row(t, di, it.ch, it.row());
     if (skip) xop_slice_front(t, o, it.row(), skip);
     if (vbytes) { const u8* pp; u32 pn; xr_payload_skip(t, it.row(), o.xk, skip, &pp, &pn); *vbytes += pn; }
@@ -686,20 +640,20 @@ __device__ inline XOp xop_gather(const ExportTables& t, const DocInfo& di, XRows
     return o;
 }
 // last op of an entry that came straight from stage A: from its head row to the end of its segment
-__device__ inline XOp xentry_last_op(const ExportTables& t, const DocInfo& di, const XEntry& E) {
+__device__ inline XOp xentry_last_op(const BatchTables& t, const DocInfo& di, const XEntry& E) {
     if (E.last_valid) return E.last;
     u64 row0;
     u32 nr;
     change_rows(t, E.lh_ch, &row0, &nr);
     XOp o = xop_from_row(t, di, E.lh_ch, row0 + E.lh_row);
-    if (E.skip && E.lh_row == E.r0 && E.lh_ch == t.ch_order[E.pos]) xop_slice_front(t, o, row0 + E.lh_row, E.skip);
+    if (E.skip && E.lh_row == E.r0 && E.lh_ch == t.ch_aorder[E.pos]) xop_slice_front(t, o, row0 + E.lh_row, E.skip);
     u32 r = E.lh_row + 1;
     while (r < nr && !(xr_flag(t, row0 + r) & (XF_HEAD | XF_SEG))) { xop_merge(o, xop_from_row(t, di, E.lh_ch, row0 + r)); r++; }
     return o;
 }
 // ChangeStore::insert_change + ChangesBlock::push_change (change_store.rs:711-764, 1244-1291): E is the next change
 // of the peer.  Returns true when the store's previous last change is complete (copied to `done`).
-__device__ inline bool xstore_push(const ExportTables& t, const DocInfo& di, XStore& s, const XEntry& E, XEntry& done,
+__device__ inline bool xstore_push(const BatchTables& t, const DocInfo& di, XStore& s, const XEntry& E, XEntry& done,
                                    bool& done_starts_block) {
     u32 nd = xentry_ndeps(t, E);
     u32 est = 4 + E.est_ops + (nd > 1 ? (nd - 1) * 4 : 0);
@@ -754,7 +708,7 @@ __device__ inline bool xstore_push(const ExportTables& t, const DocInfo& di, XSt
 
 // Change::slice at the `from` version (change_store.rs:505-521, change.rs:203-258): entry E covers counters
 // [c0, c0 + atoms) of its peer; what lies before `start` is dropped.  false = nothing left.
-__device__ inline bool xentry_cut(const ExportTables& t, const DocInfo& di, XEntry& E, i32 start) {
+__device__ inline bool xentry_cut(const BatchTables& t, const DocInfo& di, XEntry& E, i32 start) {
     i32 c0 = t.ch_counter[E.src] + (i32)E.from;
     if (start <= c0) return true;
     if (start >= c0 + (i32)E.atoms) return false;
@@ -797,7 +751,7 @@ __device__ inline bool xentry_cut(const ExportTables& t, const DocInfo& di, XEnt
 }
 
 // thread per document
-__global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, ExportTables t) {
+__global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
     const DocInfo& di = docs[d];
@@ -829,7 +783,7 @@ __global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, Export
         bool done_blk = false;
         for (u32 k = 0; k < dp.ch_count; k++) {
             u32 pos = (u32)di.ch0 + dp.ch_first + k;
-            u32 ch = t.ch_order[pos];
+            u32 ch = t.ch_aorder[pos];
             u32 nseg = t.ch_nseg[ch];
             for (u32 q = 0; q < nseg; q++) {
                 u64 sg = q == 0 ? (u64)ch : t.n_changes + t.ch_seg0[ch] + q - 1;
@@ -862,14 +816,14 @@ __global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, Export
 // 8 per delete span, 3 per map op) plus room for the op and delete columns, the per-change metadata and the
 // registers.  This is what the blocks usually need, not a bound (a bound is about 40 bytes per row against about 8
 // used): the few blocks that outgrow their slot are encoded again, straight into the export buffer.
-__device__ __forceinline__ u64 xstage_change(const ExportTables& t, u64 k) {
+__device__ __forceinline__ u64 xstage_change(const BatchTables& t, u64 k) {
     return t.fc_est[k] + 4ull * t.fc_nrows[k] + 4ull * t.fc_ndel[k] + 16;
 }
 __device__ __forceinline__ u64 xstage_block(const DocInfo& di) { return 64 + 8ull * (di.P + di.C); }
 
 // thread per document: list the output blocks (after the scans of n_mb, scratch and staging sizes).  stage_max caps
 // every slot's capacity (testing: forces the blocks that need more onto the direct encode)
-__global__ void k_exp_list(const DocInfo* __restrict__ docs, u32 n_docs, ExportTables t, XBlock* __restrict__ xb, u32 stage_max) {
+__global__ void k_exp_list(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t, XBlock* __restrict__ xb, u32 stage_max) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
     const DocInfo& di = docs[d];
@@ -902,7 +856,7 @@ __global__ void k_exp_list(const DocInfo* __restrict__ docs, u32 n_docs, ExportT
     if (idx >= 0) { b.fc1 = (u32)(f0 + x.n_fc); close(); }
 }
 // thread per document: scratch words (registers + op columns + delete columns) and staging bytes of its blocks
-__global__ void k_exp_sizes(const DocInfo* __restrict__ docs, u32 n_docs, ExportTables t, u32* __restrict__ n_blocks,
+__global__ void k_exp_sizes(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t, u32* __restrict__ n_blocks,
                             u32* __restrict__ n_scratch, u32* __restrict__ n_stage) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
@@ -1066,7 +1020,7 @@ struct XReg {
 // LoroValues [p, p + n) copied into `s` with the key indices of nested maps translated from the source block's key
 // arena (doc-level key = key_map[src_key0 + idx]) to the output block's register (write_loro_value registers a map's
 // keys as it meets them: encoding/value.rs:1027-1036).  reg = true: first use registers (the sizing pass).
-__device__ inline void xvalue_copy(XSink& s, const u8* p, u32 n, const ExportTables& t, u64 src_key0, XReg& keys, bool reg) {
+__device__ inline void xvalue_copy(XSink& s, const u8* p, u32 n, const BatchTables& t, u64 src_key0, XReg& keys, bool reg) {
     Cur c(p, n);
     u32 stack[24];
     int sp = 0;
@@ -1101,8 +1055,8 @@ __device__ inline void xvalue_copy(XSink& s, const u8* p, u32 n, const ExportTab
 }
 // cross-peer deps of the block's changes as one flat sequence (cursor: accesses are almost monotonic)
 struct XDeps {
-    const ExportTables& t; u32 fc0, N; u32 j; u32 base;
-    __device__ XDeps(const ExportTables& t_, u32 fc0_, u32 N_) : t(t_), fc0(fc0_), N(N_), j(0), base(0) {}
+    const BatchTables& t; u32 fc0, N; u32 j; u32 base;
+    __device__ XDeps(const BatchTables& t_, u32 fc0_, u32 N_) : t(t_), fc0(fc0_), N(N_), j(0), base(0) {}
     __device__ u32 nd(u32 jj) const { return t.fc_from[fc0 + jj] ? 0u : t.ch_ndeps[t.fc_src[fc0 + jj]]; }
     __device__ u64 at(u32 i) {   // index of flat dep i in the dep tables
         if (i < base) { j = 0; base = 0; }
@@ -1129,7 +1083,7 @@ __device__ __forceinline__ u8 xk_value_type(u8 xk) {
 // encode_block pre-fills its position register with the block's positions in sorted order (block_encode.rs:156-178).
 // The byte-string sort happens once per document: a warp sorts the document's position entries (first eight bytes as
 // the key, full comparison on ties) and hands every entry the dense rank of its bytes; a block then only sorts ranks.
-__device__ inline int xpos_cmp(const ExportTables& t, u32 a, u32 b) {
+__device__ inline int xpos_cmp(const BatchTables& t, u32 a, u32 b) {
     if (a == b) return 0;
     const u8* pa = t.pos_pool + t.pos_off[a];
     const u8* pb = t.pos_pool + t.pos_off[b];
@@ -1139,7 +1093,7 @@ __device__ inline int xpos_cmp(const ExportTables& t, u32 a, u32 b) {
         if (pa[i] != pb[i]) return pa[i] < pb[i] ? -1 : 1;
     return la < lb ? -1 : (la > lb ? 1 : 0);
 }
-__global__ void k_exp_posrank(const DocInfo* __restrict__ docs, u32 n_docs, ExportTables t) {
+__global__ void k_exp_posrank(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t) {
     u32 d = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     int lane = threadIdx.x & 31;
     if (d >= n_docs) return;
@@ -1191,7 +1145,7 @@ __global__ void k_exp_posrank(const DocInfo* __restrict__ docs, u32 n_docs, Expo
 // LB_XENC_BOUNDED_MIN_BLOCKS output blocks take the bounded build.
 #define LB_XENC_BOUNDED_MIN_BLOCKS 100000ull
 __device__ __forceinline__ void exp_encode_body(
-    const DocInfo* __restrict__ docs, u64 n_blocks, const ExportTables& t, XBlock* __restrict__ xb,
+    const DocInfo* __restrict__ docs, u64 n_blocks, const BatchTables& t, XBlock* __restrict__ xb,
                              u32* __restrict__ scratch, u8* __restrict__ out, int pass) {
     u64 bi_ = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (bi_ >= n_blocks) return;
@@ -1540,20 +1494,20 @@ __device__ __forceinline__ void exp_encode_body(
     s.varint(B.sec_len[7]); w_values(s);
 }
 
-template <int CAPPED> __global__ void k_exp_encode(const DocInfo* __restrict__ docs, u64 n_blocks, ExportTables t, XBlock* __restrict__ xb,
+template <int CAPPED> __global__ void k_exp_encode(const DocInfo* __restrict__ docs, u64 n_blocks, const __grid_constant__ BatchTables t, XBlock* __restrict__ xb,
                                                  u32* __restrict__ scratch, u8* __restrict__ out, int pass);
-template <> __global__ void k_exp_encode<0>(const DocInfo* __restrict__ docs, u64 n_blocks, ExportTables t, XBlock* __restrict__ xb,
+template <> __global__ void k_exp_encode<0>(const DocInfo* __restrict__ docs, u64 n_blocks, const __grid_constant__ BatchTables t, XBlock* __restrict__ xb,
                                             u32* __restrict__ scratch, u8* __restrict__ out, int pass) {
     exp_encode_body(docs, n_blocks, t, xb, scratch, out, pass);
 }
-template <> __global__ void __launch_bounds__(64, 5) k_exp_encode<1>(const DocInfo* __restrict__ docs, u64 n_blocks, ExportTables t,
+template <> __global__ void __launch_bounds__(64, 5) k_exp_encode<1>(const DocInfo* __restrict__ docs, u64 n_blocks, const __grid_constant__ BatchTables t,
                                                                      XBlock* __restrict__ xb, u32* __restrict__ scratch,
                                                                      u8* __restrict__ out, int pass) {
     exp_encode_body(docs, n_blocks, t, xb, scratch, out, pass);
 }
 
 // thread per document: block offsets inside the blob, blob length, blocks that outgrew their slot (after encode pass 0)
-__global__ void k_exp_layout(const DocInfo* __restrict__ docs, u32 n_docs, ExportTables t, XBlock* __restrict__ xb,
+__global__ void k_exp_layout(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t, XBlock* __restrict__ xb,
                              u32* __restrict__ padded_len, u32* __restrict__ n_ovf) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
@@ -1576,7 +1530,7 @@ __global__ void k_exp_layout(const DocInfo* __restrict__ docs, u32 n_docs, Expor
 
 // warp per document: the blob from the staged pieces of its blocks and their length prefixes (the blocks that
 // outgrew their slot are in place already), then header, mode, checksum (encoding.rs:397-416)
-__global__ void k_exp_finish(const DocInfo* __restrict__ docs, u32 n_docs, ExportTables t, const XBlock* __restrict__ xb,
+__global__ void k_exp_finish(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t, const XBlock* __restrict__ xb,
                              const u8* __restrict__ stage, u8* __restrict__ out) {
     u32 d = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // warp per document: the checksum walks the whole blob
     int lane = threadIdx.x & 31;

@@ -10,42 +10,8 @@
 //   diff_calc.rs:175-236 (the version vector handed to each calculator before a change)
 // Round-1 shape: one thread per document (documents are independent; a batch has 10^3..10^5 of them).
 #pragma once
-#include "lb_defs.h"
+#include "lb_tables.cuh"
 
-struct ResolveTables {
-    // block-level inputs
-    const u64* peer_id;
-    const u64* key_off; const u32* key_len;
-    const u8* cid_root; const u8* cid_type; const u32* cid_peer_idx; const i32* cid_koc;
-    const u32* ch_block; const i32* ch_counter; const u32* ch_len; const u32* ch_lamport_wire;
-    const u64* ch_dep0; const u32* ch_ndeps; const u8* ch_dep_self;
-    const u32* dep_peer_idx; const i32* dep_counter;
-    // doc-level outputs (index spaces: peers <-> block peer entries, containers <-> block cid entries,
-    // keys <-> block key entries, changes <-> batch-wide change index)
-    DocPeer* dpeer; u32* peer_map;
-    DocContainer* dcont; u32* cid_map;
-    u64* dkey_off; u32* dkey_len; u32* key_map;
-    u32* blk_order;      // per doc: its blocks sorted by (peer, counter_start)
-    u32* ch_order;       // per doc: changes grouped by peer, counter order (batch-wide change ids): every COPY
-    u32* ch_aorder;      // same grouping: the peer's APPLIED copies in the order they were applied (their applied ranges
-                         // [counter + trim, counter + len) are disjoint and ascending), then the copies that were not;
-                         // this is the order every later phase walks (tracker version switches, change store)
-    u16* ch_peer;        // doc peer idx of each change
-    u8* ch_applied;
-    u32* ch_lamport;     // recomputed lamport
-    u32* ch_walk;        // per doc: applied changes in replay order
-    i32* ch_vv;          // per doc: n_changes * P
-    u32* ch_pos;         // per change: its position in the doc's ch_order (= row of ch_vv)
-    u32* ch_trim;        // per change: leading atoms the document already had when the change arrived
-                         // (OpLog::trim_the_known_part_of_change, oplog.rs:181-196: the rest is applied as a slice)
-    u32* ch_epoch;       // per change COPY of a multi-blob document: the rank of the blob during whose import the reference
-                         // can first apply it (its own blob, or the later one that brings its last missing dependency:
-                         // blobs of a document are imported one after the other, loro.rs:1183-1290, and parked changes wait
-                         // in the pending store, pending_changes.rs); bit 31: in that blob's FIRST pass
-                         // (import_changes_to_oplog) rather than by its try_apply_pending
-    i32* ch_maxend;      // per position of the per-peer change lists: highest counter end among the entries up to there
-    u32* head_lamport;   // per doc peer: lamport of the first atom of the copy at the status pass's cursor
-};
 #define EPOCH_FP 0x80000000u
 #define EPOCH_NEVER 0x7FFFFFFFu
 
@@ -57,7 +23,7 @@ __device__ inline bool bytes_eq(const u8* a, const u8* b, u32 n) {
 
 // thread per doc: intern peers / containers / keys, order the changes per peer.
 __global__ void k_doc_tables(const u8* __restrict__ bytes, DocInfo* __restrict__ docs, u32 n_docs,
-                             const BlockInfo* __restrict__ blocks, ResolveTables t) {
+                             const BlockInfo* __restrict__ blocks, const __grid_constant__ BatchTables t) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
     DocInfo di = docs[d];
@@ -226,7 +192,7 @@ __global__ void k_doc_tables(const u8* __restrict__ bytes, DocInfo* __restrict__
 
 // lamport of atom (peer p, counter c) if applied; returns false when unknown.  The applied copies of a peer are kept in
 // application order (ch_aorder): their applied ranges ascend, so the one holding c is found by bisection on the start.
-__device__ inline bool lamport_of(const DocInfo& di, const ResolveTables& t, u32 p, i32 c, u32* out,
+__device__ inline bool lamport_of(const DocInfo& di, const BatchTables& t, u32 p, i32 c, u32* out,
                                   u32* ch_out) {
     const DocPeer& dp = t.dpeer[di.peer0 + p];
     if (c < 0 || c >= dp.end_counter || dp.n_app == 0) return false;
@@ -250,7 +216,7 @@ __device__ inline bool lamport_of(const DocInfo& di, const ResolveTables& t, u32
 // lamport of their first atom (a merge of the per-peer lists), so every copy covering a dependency has its T by then.
 #define EPOCH_SCAN_CAP 512   // covering copies looked at per atom: a document with more copies stacked on one atom gets an
                              // approximate status (never a wrong state)
-__device__ inline u32 atom_epoch(const DocInfo& di, const ResolveTables& t, u32 p, i32 c) {
+__device__ inline u32 atom_epoch(const DocInfo& di, const BatchTables& t, u32 p, i32 c) {
     const DocPeer& dp = t.dpeer[di.peer0 + p];
     if (c < 0 || c >= dp.end_counter) return EPOCH_NEVER;
     const u32* lst = t.ch_order + di.ch0 + dp.ch_first;
@@ -274,7 +240,7 @@ __device__ inline u32 atom_epoch(const DocInfo& di, const ResolveTables& t, u32 
     }
     return best;
 }
-__device__ inline u32 copy_epoch(const DocInfo& di, const ResolveTables& t, const BlockInfo* blocks, u32 ch, u32 p) {
+__device__ inline u32 copy_epoch(const DocInfo& di, const BatchTables& t, const BlockInfo* blocks, u32 ch, u32 p) {
     const BlockInfo& bi = blocks[t.ch_block[ch]];
     const u32 k = bi.blob_rank;
     u32 E = k;
@@ -302,7 +268,7 @@ __device__ inline u32 copy_epoch(const DocInfo& di, const ResolveTables& t, cons
 // frontier (consecutive in the counter-ordered list) the one with the lowest (T, parked, rank) is returned; *soft is set
 // when some candidate's dependencies are not applied YET, i.e. a better copy may still turn up.  During the walk
 // ch_epoch holds the epoch of every APPLIED copy (exact, because the copy applied for an atom is the reference's).
-__device__ inline u32 pick_copy_multi(const DocInfo& di, const ResolveTables& t, const BlockInfo* blocks, u32 p, u32 from,
+__device__ inline u32 pick_copy_multi(const DocInfo& di, const BatchTables& t, const BlockInfo* blocks, u32 p, u32 from,
                                       u32* lam_out, u32* epoch_out, bool* soft) {
     const DocPeer& dp = t.dpeer[di.peer0 + p];
     u32 best = 0xFFFFFFFFu, best_lam = 0, best_e = 0;
@@ -348,7 +314,7 @@ __device__ inline u32 pick_copy_multi(const DocInfo& di, const ResolveTables& t,
 }
 
 __global__ void k_doc_causal(DocInfo* __restrict__ docs, u32 n_docs, const BlockInfo* __restrict__ blocks,
-                             ResolveTables t, u32* __restrict__ peer_cursor, const u32* __restrict__ doc_blob0,
+                             const __grid_constant__ BatchTables t, u32* __restrict__ peer_cursor, const u32* __restrict__ doc_blob0,
                              i32* __restrict__ pend_scratch) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
@@ -592,7 +558,7 @@ __global__ void k_doc_causal(DocInfo* __restrict__ docs, u32 n_docs, const Block
 // update_frontiers_on_new_change, oplog/loro_dag.rs:251-269).  The last id of peer p is a head unless it lies in the
 // causal past of another peer's change; version vectors grow along a peer's chain, so looking at every peer's LAST
 // applied change is enough.
-__global__ void k_doc_frontiers(const DocInfo* __restrict__ docs, u32 n_docs, ResolveTables t) {
+__global__ void k_doc_frontiers(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
     const DocInfo& di = docs[d];

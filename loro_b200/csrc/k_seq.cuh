@@ -27,7 +27,7 @@
 // Rare paths (splits, the sibling scan) are separate __noinline__ functions working on per-warp state in
 // shared memory: the v2 kernel inlined them everywhere and stalled on instruction fetch (44k SASS lines).
 #pragma once
-#include "lb_defs.h"
+#include "lb_tables.cuh"
 
 #define NODE_NONE 0xFFFFFFFFu
 #define LEAF_NONE 0xFFFFFFFFu
@@ -50,15 +50,6 @@ struct SeqPools {
     uint4* a_org;        // origins, valid at span starts: x = ol_peer | or_peer << 16, y = ol_ctr, z = or_ctr
     i32* cvv;            // per container: tracker current_vv (P entries)
     u32* cont_epoch;     // per container: last walk index that checked out / applied an op
-    u32* out_row; u32* out_off; u32* out_len;
-};
-
-struct SeqTables {
-    const DocPeer* dpeer; DocContainer* dcont;
-    const u32* ch_walk; const u64* ch_op0; const u32* ch_nops; const u16* ch_peer; const i32* ch_vv;
-    const u32* ch_order; const i32* ch_counter; const u32* ch_ndeps; const u8* ch_dep_self; const u32* ch_pos;
-    const uint4* op_rec; const u32* op_aux; const u32* op_change; const i32* op_counter;
-    const u32* atom_row;
 };
 
 struct SeqSmem {   // one per warp
@@ -417,14 +408,14 @@ __device__ __forceinline__ i32 toggle_lane(const SeqPools& p, const Cx& c, u32 p
 // ---- retreat (dir=-1) / forward (dir=+1) the ops of peer `q` with counters [a,b) that touch container `cidx`.
 // The peer's changes covering [a,b) are enumerated 32 at a time, their op rows flattened over the lanes, so the
 // op records and the atom -> leaf lookups of 32 rows cost one round trip each.
-__device__ __noinline__ void toggle_ops(const SeqPools& p, const SeqTables& t, Cx c, u64 ch0, u32 cidx, u32 q, i32 a, i32 b, int dir) {
+__device__ __noinline__ void toggle_ops(const SeqPools& p, const BatchTables& t, Cx c, u64 ch0, u32 cidx, u32 q, i32 a, i32 b, int dir) {
     int lane = c.lane;
     u32 row_a = t.atom_row[atom_index(c, q, a)], row_b = t.atom_row[atom_index(c, q, b - 1)];
     u32 pos_a = t.ch_pos[t.op_change[row_a]], pos_b = t.ch_pos[t.op_change[row_b]];
     for (u32 pb = pos_a; pb <= pos_b && !c.sm->err; pb += 32) {
         u32 pos = pb + (u32)lane;
         bool cv = pos <= pos_b;
-        u32 ch = cv ? t.ch_order[ch0 + pos] : 0;
+        u32 ch = cv ? t.ch_aorder[ch0 + pos] : 0;
         u32 r0 = cv ? (u32)t.ch_op0[ch] : 0;
         i32 nr = cv ? (i32)t.ch_nops[ch] : 0;
         i32 incl = warp_incl_scan(nr, lane);
@@ -479,7 +470,7 @@ __device__ __noinline__ void toggle_ops(const SeqPools& p, const SeqTables& t, C
 }
 
 // ---- move the tracker of the active container to version vv (+ the author's own counter)
-__device__ __forceinline__ void checkout(const SeqPools& p, const SeqTables& t, const Cx& c, u64 ch0, u32 cidx, const i32* vv,
+__device__ __forceinline__ void checkout(const SeqPools& p, const BatchTables& t, const Cx& c, u64 ch0, u32 cidx, const i32* vv,
                                          u32 own_peer, i32 own_ctr) {
     int lane = c.lane;
     for (u32 q0 = 0; q0 < c.P && !c.sm->err; q0 += 32) {
@@ -826,7 +817,7 @@ __device__ __forceinline__ u32 predict_leaf(const Cx& c, i32 pos) {
 
 // ---- container switching: internal nodes < NS and the tracker version live in shared memory while a
 // container is active
-__device__ __noinline__ void store_container(const SeqPools& p, const SeqTables& t, Cx c, u64 cid0, u32 cidx) {
+__device__ __noinline__ void store_container(const SeqPools& p, const BatchTables& t, Cx c, u64 cid0, u32 cidx) {
     if (cidx == 0xFFFFFFFFu) return;
     SeqSmem* sm = c.sm;
     int lane = c.lane;
@@ -853,7 +844,7 @@ __device__ __noinline__ void store_container(const SeqPools& p, const SeqTables&
 }
 // returns the container's Cx (pool bases); Tracker::new_with_unknown (tracker.rs:38-63) on first use: one
 // placeholder span of length u32::MAX/4
-__device__ __noinline__ Cx load_container(const SeqPools& p, const SeqTables& t, Cx c, u64 cid0, u32 cidx) {
+__device__ __noinline__ Cx load_container(const SeqPools& p, const BatchTables& t, Cx c, u64 cid0, u32 cidx) {
     SeqSmem* sm = c.sm;
     int lane = c.lane;
     const DocContainer& dc = t.dcont[cid0 + cidx];
@@ -905,7 +896,7 @@ __device__ __noinline__ Cx load_container(const SeqPools& p, const SeqTables& t,
 }
 
 // ---- emit the final visible runs of the active container (after checkout to the final version)
-__device__ __noinline__ void emit_output(const SeqPools& p, const SeqTables& t, Cx c, u64 cid0, u32 cidx) {
+__device__ __noinline__ void emit_output(const SeqPools& p, const BatchTables& t, Cx c, u64 cid0, u32 cidx) {
     int lane = c.lane;
     DocContainer& dc = t.dcont[cid0 + cidx];
     u32 n_out = 0;
@@ -922,9 +913,9 @@ __device__ __noinline__ void emit_output(const SeqPools& p, const SeqTables& t, 
             u32 o = n_out + __popc(m & ((1u << lane) - 1));
             if (o < out_cap) {
                 u32 row = t.atom_row[atom_index(c, pe, (i32)L.y)];
-                p.out_row[out0 + o] = row;
-                p.out_off[out0 + o] = (u32)((i32)L.y - t.op_counter[row]);
-                p.out_len[out0 + o] = L.z;
+                t.out_row[out0 + o] = row;
+                t.out_off[out0 + o] = (u32)((i32)L.y - t.op_counter[row]);
+                t.out_len[out0 + o] = L.z;
             }
         }
         total += (u32)warp_sum(live ? (i32)L.z : 0);
@@ -946,7 +937,7 @@ __device__ __noinline__ void emit_output(const SeqPools& p, const SeqTables& t, 
 #define LB_SEQ_MINB 8         // 8 CTAs x 4 warps = 32 resident documents per SM (64 registers/thread)
 __global__ void __launch_bounds__(32 * LB_SEQ_WARPS, LB_SEQ_MINB)
 k_seq_integrate(DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ SeqPools pools,
-                const __grid_constant__ SeqTables tables) {
+                const __grid_constant__ BatchTables tables) {
     __shared__ SeqSmem smem[LB_SEQ_WARPS];
     u32 warp_in_cta = threadIdx.x >> 5;
     u32 warp_global = blockIdx.x * LB_SEQ_WARPS + warp_in_cta;

@@ -7,27 +7,10 @@
 // its own tests compare parsed JSON).  Round-1 shape: one thread per document, two passes over the same
 // emitter (count bytes, then write) with an explicit frame stack instead of recursion.
 #pragma once
-#include "lb_defs.h"
+#include "lb_tables.cuh"
 #include "k_frame.cuh"
 #include "k_tree.cuh"
 #include "lb_f64.cuh"
-
-struct StateTables {
-    const u8* bytes;
-    const DocPeer* dpeer; const DocContainer* dcont;
-    const u64* dkey_off; const u32* dkey_len;
-    const u32* map_row; const unsigned long long* map_best;
-    const u8* op_kind; const u8* op_vtype; const u32* op_len; const i32* op_counter; const u32* op_change;
-    const u64* op_val_off; const u32* op_val_len;
-    const u16* ch_peer;
-    const u32* ch_block; const u64* bkey_off; const u32* bkey_len;   // keys of nested map values index the block's key arena
-    const u32* out_row; const u32* out_off; const u32* out_len;
-    // movable tree (k_tree.cuh): node tables per document (base DocInfo::tree0) + positions
-    const BlockInfo* blocks;
-    const u32* tn_parent; const u32* tn_move; const u32* tn_base; const u32* tn_cnt; const u32* tn_sib; const u32* tn_child;
-    const u32* tn_root; const u32* tn_aopen; const u32* tn_aclose; const u64* ns_key;   // lane-parallel layout (k_tree.cuh)
-    const uint4* tr_rec; const u64* pos_off; const u32* pos_len; const u8* pos_pool;
-};
 
 struct Sink {
     u8* dst;   // nullptr = counting pass
@@ -90,7 +73,7 @@ struct TreeEmitSmem {
 };
 
 struct Emitter {
-    const StateTables& t;
+    const BatchTables& t;
     const DocInfo& di;
     Sink& out;
     Frame st[MAX_FRAMES];
@@ -99,7 +82,7 @@ struct Emitter {
     int lane;
     u32 cur_blk;   // block of the op whose value is being printed (nested map keys are block-local indices)
     TreeEmitSmem* tsm;
-    __device__ Emitter(const StateTables& t_, const DocInfo& di_, Sink& o, int lane_, TreeEmitSmem* tsm_) : t(t_), di(di_), out(o), sp(0), err(0), lane(lane_), cur_blk(0), tsm(tsm_) {}
+    __device__ Emitter(const BatchTables& t_, const DocInfo& di_, Sink& o, int lane_, TreeEmitSmem* tsm_) : t(t_), di(di_), out(o), sp(0), err(0), lane(lane_), cur_blk(0), tsm(tsm_) {}
 
     __device__ int cmp_bytes(const u8* a, u32 al, const u8* b, u32 bl) {
         u32 n = al < bl ? al : bl;
@@ -532,12 +515,12 @@ struct Emitter {
                     u8 k = c.get();
                     skip_loro_value_content(c, k, nullptr);
                     if (ki >= vb.n_keys) { err = LB_ERR(DOC_ERR_CORRUPT); break; }
-                    const u8* kb = t.bytes + t.bkey_off[vb.key0 + ki];
-                    u32 kl = t.bkey_len[vb.key0 + ki];
+                    const u8* kb = t.bytes + t.key_off[vb.key0 + ki];
+                    u32 kl = t.key_len[vb.key0 + ki];
                     if (f.c != 0xFFFFFFFFu &&
-                        cmp_bytes(kb, kl, t.bytes + t.bkey_off[vb.key0 + f.c], t.bkey_len[vb.key0 + f.c]) <= 0) continue;
+                        cmp_bytes(kb, kl, t.bytes + t.key_off[vb.key0 + f.c], t.key_len[vb.key0 + f.c]) <= 0) continue;
                     if (best == 0xFFFFFFFFu ||
-                        cmp_bytes(kb, kl, t.bytes + t.bkey_off[vb.key0 + best], t.bkey_len[vb.key0 + best]) <= 0) { best = (u32)ki; best_val = val; }
+                        cmp_bytes(kb, kl, t.bytes + t.key_off[vb.key0 + best], t.key_len[vb.key0 + best]) <= 0) { best = (u32)ki; best_val = val; }
                 }
                 if (c.err) err = LB_ERR(DOC_ERR_CORRUPT);
             }
@@ -547,7 +530,7 @@ struct Emitter {
             f.first = 0;
             f.c = best;
             out.put('"');
-            out.put_escaped(t.bytes + t.bkey_off[vb.key0 + best], t.bkey_len[vb.key0 + best]);
+            out.put_escaped(t.bytes + t.key_off[vb.key0 + best], t.key_len[vb.key0 + best]);
             out.put('"');
             out.put(':');
             cur_blk = f.b;
@@ -683,7 +666,7 @@ struct Emitter {
 };
 
 // pass = 0: count bytes into docs[d].json_len ; pass = 1: write at docs[d].json_off
-__global__ void __launch_bounds__(128, 8) k_json(DocInfo* __restrict__ docs, u32 n_docs, StateTables t, u8* __restrict__ json, int pass) {
+__global__ void __launch_bounds__(128, 8) k_json(DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t, u8* __restrict__ json, int pass) {
     __shared__ TreeEmitSmem tsm[4];   // 128 threads: one entry per warp
     u32 d = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // one warp per document
     int lane = threadIdx.x & 31;

@@ -19,34 +19,9 @@
 // Nodes of different tree containers share the atom-indexed tables: in a well-formed document their ids are
 // disjoint; a hostile blob that moves a node of one tree inside another gets a memory-safe, cycle-free result.
 #pragma once
-#include "lb_defs.h"
+#include "lb_tables.cuh"
 
-struct TreeTables {
-    const DocPeer* dpeer;
-    const BlockInfo* blocks;
-    const u32* op_cidx; const u32* op_lamport;
-    const uint4* tr_rec;      // per tree op (k_op_classify): target atom, parent atom | TREE_ROOT | TREE_DELETED, position, row
-    const u64* tr_key;        // (lamport << 32 | peer rank << 16), ~0 for ops that are not applied
-    u64* ts_key; u32* ts_val; // sort space, one entry per tree op
-    uint4* ts_rec;            // the records in apply order (w = 0xFFFFFFFF from the first op that is not applied)
-    const u64* pos_off; const u32* pos_len; const u8* pos_pool;
-    // per document: S = atom_total + C slots starting at DocInfo::tree0.  Slots [0, atom_total) are nodes, slot
-    // atom_total + c is the root of tree container c.
-    u32* tn_parent;           // [node] TREE_UNEXIST | TREE_ROOT | TREE_DELETED | parent node
-    u32* tn_move;             // [node] tree op of the last effective move (position, lamport, peer of the node)
-    u32* tn_base;             // [slot] first child in tn_child
-    u32* tn_cnt;              // [slot] number of children
-    u32* tn_sib;              // [node] index among its siblings
-    u64* ns_key;              // [slot] sort key: parent slot << 32 | first four position bytes; after the sort the space holds
-                              //        tn_sub (JSON bytes of the subtree, [slot]) and tn_rel (offset among siblings, [node])
-    u32* tn_child;            // [node] after the sort: nodes grouped by parent slot, in sibling order
-    // hierarchy JSON layout (k_state.cuh writes the nodes lane-parallel when no node has a meta map with content)
-    u32* tn_root;             // [node] root slot of the tree the node is alive in, TREE_UNEXIST when dead
-    u32* tn_aopen;            // [node] offset of the node's `{"children":[` inside its container's JSON
-    u32* tn_aclose;           // [node] offset of the part after its children
-    const DocContainer* dcont;
-};
-__device__ __forceinline__ u32* tree_sub(const TreeTables& t, const DocInfo& di) { return (u32*)(t.ns_key + di.tree0); }
+__device__ __forceinline__ u32* tree_sub(const BatchTables& t, const DocInfo& di) { return (u32*)(t.ns_key + di.tree0); }
 
 // decimal digits of v: compare against powers of ten around the estimate from the bit length (no 64-bit divisions)
 __device__ const u64 LB_P10[20] = {1ull, 10ull, 100ull, 1000ull, 10000ull, 100000ull, 1000000ull, 10000000ull, 100000000ull, 1000000000ull,
@@ -117,7 +92,7 @@ __device__ inline void warp_sort_vals(u32* val, u32 n, int lane, Before before) 
 }
 
 // lexicographic comparison of two fractional indexes (FractionalIndex derives Ord on its bytes)
-__device__ inline int pos_cmp(const TreeTables& t, u32 pa, u32 pb) {
+__device__ inline int pos_cmp(const BatchTables& t, u32 pa, u32 pb) {
     if (pa == pb) return 0;
     const u8* a = t.pos_pool + t.pos_off[pa];
     const u8* b = t.pos_pool + t.pos_off[pb];
@@ -148,7 +123,7 @@ struct ParentArr {
     __device__ __forceinline__ void set(u32 i, u32 v) const { if (s) s[i] = (u16)v; else g[i] = v; }   // (special values keep their low 16 bits)
 };
 
-__global__ void k_tree_sort(const DocInfo* __restrict__ docs, u32 n_docs, TreeTables t) {
+__global__ void k_tree_sort(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t) {
     u32 d = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     int lane = threadIdx.x & 31;
     if (d >= n_docs) return;
@@ -223,7 +198,7 @@ __global__ void k_tree_sort(const DocInfo* __restrict__ docs, u32 n_docs, TreeTa
     }
 }
 
-__global__ void __launch_bounds__(32 * TREE_WARPS) k_tree_apply(const DocInfo* __restrict__ docs, u32 n_docs, TreeTables t, u32 s_nodes) {
+__global__ void __launch_bounds__(32 * TREE_WARPS) k_tree_apply(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t, u32 s_nodes) {
 #ifdef LB_SIMT_EMU
     LB_DYN_SMEM(u16, tree_smem);
 #else
@@ -299,7 +274,7 @@ __global__ void __launch_bounds__(32 * TREE_WARPS) k_tree_apply(const DocInfo* _
     if (parent.s) for (u32 i = lane; i < A; i += 32) parent.g[i] = parent.get(i);   // the later passes read the global table
 }
 
-__global__ void k_tree_layout(DocInfo* __restrict__ docs, u32 n_docs, TreeTables t) {
+__global__ void k_tree_layout(DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t) {
     u32 d = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     int lane = threadIdx.x & 31;
     if (d >= n_docs) return;
