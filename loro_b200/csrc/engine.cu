@@ -6,6 +6,7 @@
 #include "../../include/loro_b200.h"
 
 #include <algorithm>
+#include <atomic>
 #include <chrono>
 #include <memory>
 #include <mutex>
@@ -376,6 +377,30 @@ void launch_exp_encode(cudaStream_t st, DocInfo* docs, u64 NOB, const BatchTable
     else LB_LAUNCH(k_exp_encode<0>, nblk(NOB, 64), 64, 0, st, docs, NOB, xt, xb, xscratch, out, pass);
 }
 
+// CTAs of k_seq_integrate that the device holds at once, computed once per device: a batch that needs more gets that
+// many, whose warps take documents from a queue until none are left.  The emulated build has no occupancy query: one
+// CTA, so that its tests pass many documents through each warp.
+unsigned seq_resident_ctas(int device) {
+#ifdef LB_SIMT_EMU
+    (void)device;
+    return 1;
+#else
+    static std::atomic<unsigned> ctas[64];
+    std::atomic<unsigned>& n = ctas[(unsigned)device % 64];
+    if (!n.load(std::memory_order_relaxed)) {
+        int per_sm = 0, sms = 0;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_seq_integrate<1>, 32 * LB_SEQ_WARPS, 0));
+        CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+        if (per_sm < 1 || sms < 1) {
+            g_last_error = "k_seq_integrate: no CTA fits a multiprocessor";
+            throw lb_status(LB_ERR_CUDA);
+        }
+        n.store((unsigned)per_sm * (unsigned)sms, std::memory_order_relaxed);
+    }
+    return n.load(std::memory_order_relaxed);
+#endif
+}
+
 // LB_PHASE_TRACE=1: host wall clock between named points (each one synchronises the stream: diagnosis only)
 void trace_point(lb_batch* b, const char* name);
 void mark(lb_batch* b) {
@@ -641,12 +666,15 @@ void pipeline(lb_batch* b) {
     sp.a_org = dv.alloc<uint4>(NATOM);
     sp.cvv = dv.alloc<i32>(NCVV, true);
     sp.cont_epoch = dv.alloc<u32>(NC + 1);
+    sp.next_doc = dv.alloc<u32>(1, true);
     t.out_row = dv.alloc<u32>(NOUT); t.out_off = dv.alloc<u32>(NOUT); t.out_len = dv.alloc<u32>(NOUT);
-    LB_LAUNCH(k_seq_integrate, nblk(D, LB_SEQ_WARPS), 32 * LB_SEQ_WARPS, 0, st, b->d_docs, D, sp, t);
+    const unsigned seq_ctas = seq_resident_ctas(b->device);
+    if (nblk(D, LB_SEQ_WARPS) > seq_ctas) LB_LAUNCH(k_seq_integrate<1>, seq_ctas, 32 * LB_SEQ_WARPS, 0, st, b->d_docs, D, sp, t);
+    else LB_LAUNCH(k_seq_integrate<0>, nblk(D, LB_SEQ_WARPS), 32 * LB_SEQ_WARPS, 0, st, b->d_docs, D, sp, t);
     tm.kernel_launches += 1;
     if (!(b->flags & LB_FLAG_KEEP_DEVICE)) {   // the tracker pools are the largest tables of the batch: free them early
         dv.release(sp.leaf); dv.release(sp.node); dv.release(sp.node_parent); dv.release(sp.atom_leaf); dv.release(sp.a_org);
-        dv.release(sp.cvv); dv.release(sp.cont_epoch); dv.release(t.atom_row); dv.release(t.op_rec);
+        dv.release(sp.cvv); dv.release(sp.cont_epoch); dv.release(sp.next_doc); dv.release(t.atom_row); dv.release(t.op_rec);
     }
     mark(b);  // [5] list/text integration done
     // ------------------------------------------------------------ phase 5b: movable trees

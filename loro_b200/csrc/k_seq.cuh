@@ -1,4 +1,4 @@
-// loro_b200 -- phase 5: eg-walker (Fugue) integration of List/Text containers, one warp per document.
+// loro_b200 -- phase 5: eg-walker (Fugue) integration of List/Text containers, one warp per document at a time.
 //
 // Replaces (reference, relative to crates/loro-internal/src):
 //   container/richtext/tracker.rs:84-232 (insert/delete), :330-526 (checkout: retreat / forward)
@@ -50,6 +50,7 @@ struct SeqPools {
     uint4* a_org;        // origins, valid at span starts: x = ol_peer | or_peer << 16, y = ol_ctr, z = or_ctr
     i32* cvv;            // per container: tracker current_vv (P entries)
     u32* cont_epoch;     // per container: last walk index that checked out / applied an op
+    u32* next_doc;       // the launch's work queue: index of the next document to hand to a warp (zero at launch)
 };
 
 struct SeqSmem {   // one per warp
@@ -932,18 +933,10 @@ __device__ __noinline__ void emit_output(const SeqPools& p, const BatchTables& t
 }
 
 // (single-peer documents do not skip the origin records, although nothing is ever concurrent in them: such a flag costs
-//  a register in every helper of a kernel that sits at its 64-register budget)
-// one warp per document, LB_SEQ_WARPS documents per CTA
-#define LB_SEQ_MINB 8         // 8 CTAs x 4 warps = 32 resident documents per SM (64 registers/thread)
-__global__ void __launch_bounds__(32 * LB_SEQ_WARPS, LB_SEQ_MINB)
-k_seq_integrate(DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ SeqPools pools,
-                const __grid_constant__ BatchTables tables) {
-    __shared__ SeqSmem smem[LB_SEQ_WARPS];
-    u32 warp_in_cta = threadIdx.x >> 5;
-    u32 warp_global = blockIdx.x * LB_SEQ_WARPS + warp_in_cta;
-    int lane = threadIdx.x & 31;
-    if (warp_global >= n_docs) return;
-    DocInfo& di = docs[warp_global];
+//  a register in every helper of a kernel that spills at its register budget)
+// One document by one warp.  Every per-document field of `sm` (err, abase, the active container, cvv) is set again
+// here before it is read: the warp's previous document left its values there.
+__device__ __forceinline__ void integrate_doc(DocInfo& di, SeqSmem* sm, int lane, const SeqPools& pools, const BatchTables& tables) {
     if (di.code != DOC_OK || di.n_applied == 0) return;
     const u64 cid0 = di.cid0, ch0 = di.ch0, vv0 = di.vv0;
     const u32 P = di.P, C = di.C, n_applied = di.n_applied;
@@ -952,13 +945,12 @@ k_seq_integrate(DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ 
         if (tables.dcont[cid0 + ci].leaf_cap) any = true;
     if (!any) return;
     Cx c;
-    c.sm = &smem[warp_in_cta];
+    c.sm = sm;
     c.dpeer = tables.dpeer + di.peer0;
     c.leaf0 = c.node0 = c.cvv0 = 0;
     c.atom0 = di.atom0;
     c.P = P;
     c.lane = lane;
-    SeqSmem* sm = c.sm;
     sm->abase[lane] = (u32)lane < P ? c.dpeer[lane].atom_base : 0;
     if (lane == 0) sm->err = 0;
     __syncwarp();
@@ -1067,4 +1059,35 @@ k_seq_integrate(DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ 
     store_container(pools, tables, c, cid0, cidx);
     __syncwarp();
     if (lane == 0 && sm->err) di.code = sm->err;
+}
+
+// QUEUE = 1, for batches with more documents than the device holds warps: the launch holds only as many CTAs as can be
+// resident at once (engine.cu), and every warp takes the next document from `pools.next_doc` until none are left.  A
+// warp whose document ends early starts another instead of holding its slot until the slowest warp of its CTA is done,
+// and no last wave of CTAs runs half full.  QUEUE = 0: warp w of the grid integrates document w; with every document
+// on a warp of its own the queue has nothing to balance, and its loop made the one-document C4 0.8 % slower (at 8 CTAs
+// per SM, DESIGN.md section 6).
+// 5 CTAs x 4 warps = 20 resident documents per SM (96 registers/thread).  Fewer documents per SM spill less and leave
+// each warp more L1 for its leaves and stack: on H100, C3 integrates fastest at 5 of the 4-12 measured (DESIGN.md
+// section 3).
+#define LB_SEQ_MINB 5
+template <int QUEUE>
+__global__ void __launch_bounds__(32 * LB_SEQ_WARPS, LB_SEQ_MINB)
+k_seq_integrate(DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ SeqPools pools,
+                const __grid_constant__ BatchTables tables) {
+    __shared__ SeqSmem smem[LB_SEQ_WARPS];
+    SeqSmem* sm = &smem[threadIdx.x >> 5];
+    int lane = threadIdx.x & 31;
+    if (!QUEUE) {
+        u32 d = blockIdx.x * LB_SEQ_WARPS + (threadIdx.x >> 5);
+        if (d < n_docs) integrate_doc(docs[d], sm, lane, pools, tables);
+        return;
+    }
+    while (true) {
+        u32 d = 0;
+        if (lane == 0) d = atomicAdd(pools.next_doc, 1u);
+        d = __shfl_sync(LB_FULL, d, 0);
+        if (d >= n_docs) return;
+        integrate_doc(docs[d], sm, lane, pools, tables);
+    }
 }
