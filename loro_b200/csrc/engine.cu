@@ -368,13 +368,13 @@ namespace {
 const int TPB = 128;
 inline unsigned nblk(u64 n, int tpb = TPB) { return (unsigned)((n + tpb - 1) / tpb); }
 
-// one pass of the export encoder over NOB output blocks (pass 1 only touches the blocks that outgrew their staging
-// slot), in the build that is faster for that many (k_export.cuh)
+// the export encoder over NOB output blocks (retry = 1: only the blocks that outgrew their staging slot, into their
+// retry slots), in the build that is faster for that many (k_export.cuh)
 void launch_exp_encode(cudaStream_t st, DocInfo* docs, u64 NOB, const BatchTables& xt, XBlock* xb, u32* xscratch, u8* out,
-                       int pass) {
+                       int retry) {
     if (!NOB) return;
-    if (NOB >= LB_XENC_BOUNDED_MIN_BLOCKS) LB_LAUNCH(k_exp_encode<1>, nblk(NOB, 64), 64, 0, st, docs, NOB, xt, xb, xscratch, out, pass);
-    else LB_LAUNCH(k_exp_encode<0>, nblk(NOB, 64), 64, 0, st, docs, NOB, xt, xb, xscratch, out, pass);
+    if (NOB >= LB_XENC_BOUNDED_MIN_BLOCKS) LB_LAUNCH(k_exp_encode<1>, nblk(NOB, 64), 64, 0, st, docs, NOB, xt, xb, xscratch, out, retry);
+    else LB_LAUNCH(k_exp_encode<0>, nblk(NOB, 64), 64, 0, st, docs, NOB, xt, xb, xscratch, out, retry);
 }
 
 // CTAs of k_seq_integrate that the device holds at once, computed once per device: a batch that needs more gets that
@@ -440,9 +440,10 @@ void run_scans(lb_batch* b, std::vector<ScanJob> jobs) {
             sizeof(type), sizeof(type), (u64)(count)}
 
 // The encode end of phase 7, after the stores (k_exp_store) have cut every document's changes into output blocks;
-// shared by the batch's export and export_from.  Block list with scratch and staging slots, one encode pass into the
-// slots, layout (the lengths are exact, so are the offsets), the direct encode of the blocks that outgrew their slot
-// (only when there are any: their count comes back with the blob sizes), then the blobs assembled per document.
+// shared by the batch's export and export_from.  Block list with scratch and staging slots, one encode into the slots,
+// layout (the lengths are exact, so are the offsets and the retry slots), the encode again of the blocks that outgrew
+// their slot, into retry slots of their exact size (only when there are any: the retry bytes come back with the blob
+// sizes), then the blobs assembled per document.
 // Returns the export buffer (*total bytes, document d's blob at xt.xdoc[d].exp_off).
 u8* export_encode(lb_batch* b, const BatchTables& xt, u64* total) {
     Dev& dv = b->dev;
@@ -461,29 +462,35 @@ u8* export_encode(lb_batch* b, const BatchTables& xt, u64* total) {
     XBlock* xb = dv.alloc<XBlock>(NOB + 1);
     u32* xscratch = dv.alloc<u32>(NSCR + 1);
     u8* xstage = dv.alloc<u8>(NSTG + 16);
-    const char* cap_env = getenv("LB_EXPORT_STAGE_CAP");   // testing hook: smaller slots send blocks to the direct encode
+    const char* cap_env = getenv("LB_EXPORT_STAGE_CAP");   // testing hook: smaller slots send blocks through the retry
     const u32 stage_max = cap_env ? (u32)strtoul(cap_env, nullptr, 10) : 0xFFFFFFFFu;
     trace_point(b, "store+sizes");
     LB_LAUNCH(k_exp_list, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb, stage_max);
     launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, xstage, 0);
-    LB_LAUNCH(k_exp_layout, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb, n_a, n_b);
+    LB_LAUNCH(k_exp_layout, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb, n_a, n_b, n_c);
     tm.kernel_launches += 3;
     trace_point(b, "encode");
     run_scans(b, {ScanJob{(const u8*)n_a, (u8*)xt.xdoc + offsetof(XDoc, exp_off), 4, sizeof(XDoc), D},
-                  ScanJob{(const u8*)n_b, (u8*)xt.xdoc + offsetof(XDoc, ovf0), 4, sizeof(XDoc), D}});
+                  ScanJob{(const u8*)n_b, (u8*)xt.xdoc + offsetof(XDoc, ovf0), 4, sizeof(XDoc), D},
+                  ScanJob{(const u8*)n_c, (u8*)xt.xdoc + offsetof(XDoc, restage0), 4, sizeof(XDoc), D}});
     xtot = d2h_one(b, xt.xdoc + D);
-    const u64 XT = xtot.exp_off, NOVF = xtot.ovf0;
+    const u64 XT = xtot.exp_off, NOVF = xtot.ovf0, NRST = xtot.restage0;
     if (getenv("LB_PHASE_TRACE"))
         fprintf(stderr, "[trace] export: %llu blocks, %llu outgrew their staging slot; %llu staging bytes for %llu exported\n",
                 (unsigned long long)NOB, (unsigned long long)NOVF, (unsigned long long)NSTG, (unsigned long long)XT);
     trace_point(b, "layout scan + size d2h");
     u8* out = dv.alloc<u8>(XT + 16, true);
     trace_point(b, "export buffer alloc+zero");
-    if (NOVF) { launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, out, 1); tm.kernel_launches += 1; }
-    LB_LAUNCH(k_exp_finish, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, xt, xb, xstage, out);
+    u8* xrestage = nullptr;
+    if (NOVF) {
+        xrestage = dv.alloc<u8>(NRST + 16);
+        launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, xrestage, 1);
+        tm.kernel_launches += 1;
+    }
+    LB_LAUNCH(k_exp_finish, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, xt, xb, xstage, xrestage, out);
     tm.kernel_launches += 1;
     trace_point(b, "assemble");
-    dv.release(cnt); dv.release(xb); dv.release(xscratch); dv.release(xstage);
+    dv.release(cnt); dv.release(xb); dv.release(xscratch); dv.release(xstage); dv.release(xrestage);
     *total = XT;
     return out;
 }

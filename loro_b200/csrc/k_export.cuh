@@ -20,7 +20,7 @@
 // look at the boundary ops only.  A thread per output block then gathers its ops into scratch columns and
 // encodes them once, into a staging slot sized from the block's rows and store estimate; the lengths it records
 // place the block in its document's blob, and a warp per document assembles the blob from the staged pieces and the
-// length prefixes.  A block that outgrows its slot is encoded a second time, straight into the blob.
+// length prefixes.  A block that outgrows its slot is encoded again by the same code, into a slot of its exact size.
 // Whether two neighbouring inserts merge depends on where their payloads landed in the importing document's
 // arenas (arena.rs:237-263): values are adjacent when nothing else was allocated in between (decode order),
 // strings additionally need the append-only buffer not to have been reallocated (capacity doubles from 32;
@@ -49,20 +49,22 @@ struct XDoc {          // per document
     u32 scratch_words;
     u64 stage0;        // first staging byte of this doc's blocks
     u64 ovf0;          // blocks of the documents before this one that outgrew their staging slot (scan)
+    u64 restage0;      // first retry-slot byte of this doc's blocks that outgrew their staging slot (scan)
 };
 struct XBlock {        // one output block
     u32 doc;
     u32 fc0, fc1;      // final-change range (absolute indices into fc_*)
     u32 len;           // encoded bytes (without the ULEB length prefix)
     u32 sec_len[8];
-    u32 col_len[10];   // ops columns 0-3, delete columns 4-6, [7] = register sizes, [8..9] = position columns
+    u32 col_len[9];    // ops columns 0-3, delete columns 4-6, position columns 7-8
     u64 off;           // offset of the block bytes inside the document's blob
     u64 scratch;       // scratch words of this block
     u32 n_rows, n_dels;            // scratch capacities: rows, delete ops
-    u32 n_ops, n_del_ops, n_cids, n_pos; // after the gather: merged ops, merged deletes, containers, positions
+    u32 n_ops, n_del_ops, n_pos;   // after the gather: merged ops, merged deletes, positions
     u64 stage;         // staging slot: first byte, capacity; the block's pieces without their length prefixes
     u32 stage_cap;
-    u32 ovf;           // 1 = the pieces did not fit the slot: encoded straight into the blob instead
+    u32 ovf;           // 1 = the pieces did not fit the first slot: encoded again into a retry slot (k_exp_layout;
+                       //     `stage` is then relative to the document's restage0)
 };
 
 // ---------------------------------------------------------------------------------------------- byte sink
@@ -815,14 +817,21 @@ __global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, const 
 // Staging slot of an output block, in bytes: the store's size estimate of its changes (text bytes, 4 per list item,
 // 8 per delete span, 3 per map op) plus room for the op and delete columns, the per-change metadata and the
 // registers.  This is what the blocks usually need, not a bound (a bound is about 40 bytes per row against about 8
-// used): the few blocks that outgrow their slot are encoded again, straight into the export buffer.
+// used): the few blocks that outgrow their slot are encoded again, into a slot of their exact size (k_exp_layout).
 __device__ __forceinline__ u64 xstage_change(const BatchTables& t, u64 k) {
     return t.fc_est[k] + 4ull * t.fc_nrows[k] + 4ull * t.fc_ndel[k] + 16;
 }
 __device__ __forceinline__ u64 xstage_block(const DocInfo& di) { return 64 + 8ull * (di.P + di.C); }
+// Scratch words of an output block, as the encoder carves them: the peer, key and container registers (order and
+// inverse each), then four op columns per row (five in documents with tree ops: the position ranks) and three delete
+// columns per delete.
+__device__ __forceinline__ u64 xscratch_change(const BatchTables& t, const XDoc& x, u64 k) {
+    return (4ull + ((x.flags >> 1) & 1u)) * t.fc_nrows[k] + 3ull * t.fc_ndel[k];
+}
+__device__ __forceinline__ u64 xscratch_block(const DocInfo& di) { return 2ull * (di.P + di.K + di.C); }
 
 // thread per document: list the output blocks (after the scans of n_mb, scratch and staging sizes).  stage_max caps
-// every slot's capacity (testing: forces the blocks that need more onto the direct encode)
+// every slot's capacity (testing: sends the blocks that need more through the retry)
 __global__ void k_exp_list(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t, XBlock* __restrict__ xb, u32 stage_max) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
@@ -830,15 +839,14 @@ __global__ void k_exp_list(const DocInfo* __restrict__ docs, u32 n_docs, const _
     const XDoc& x = t.xdoc[d];
     if (di.code != DOC_OK || x.n_mb == 0) return;
     u64 f0 = di.ch0 + t.ch_seg0[di.ch0];
-    u32 regs = 2 * (di.P + di.K + di.C);
-    u64 scr = x.scratch0, stg = x.stage0, slot = 0;
+    u64 scr = x.scratch0, stg = x.stage0, words = 0, slot = 0;
     int idx = -1;
     XBlock b;
     memset(&b, 0, sizeof(b));
     auto close = [&]() {
         b.stage_cap = (u32)(slot < stage_max ? slot : stage_max);
         xb[x.ob0 + idx] = b;
-        scr += regs + (5 + ((x.flags >> 1) & 1u)) * b.n_rows + 3 * b.n_dels;
+        scr += words;
         stg += slot;
     };
     for (u64 k = f0; k < f0 + x.n_fc; k++) {
@@ -847,15 +855,17 @@ __global__ void k_exp_list(const DocInfo* __restrict__ docs, u32 n_docs, const _
             idx++;
             memset(&b, 0, sizeof(b));
             b.doc = d; b.fc0 = (u32)k; b.scratch = scr; b.stage = stg;
+            words = xscratch_block(di);
             slot = xstage_block(di);
         }
         b.n_rows += t.fc_nrows[k];
         b.n_dels += t.fc_ndel[k];
+        words += xscratch_change(t, x, k);
         slot += xstage_change(t, k);
     }
     if (idx >= 0) { b.fc1 = (u32)(f0 + x.n_fc); close(); }
 }
-// thread per document: scratch words (registers + op columns + delete columns) and staging bytes of its blocks
+// thread per document: scratch words and staging bytes of its blocks
 __global__ void k_exp_sizes(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t, u32* __restrict__ n_blocks,
                             u32* __restrict__ n_scratch, u32* __restrict__ n_stage) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
@@ -866,10 +876,10 @@ __global__ void k_exp_sizes(const DocInfo* __restrict__ docs, u32 n_docs, const 
     u64 words = 0, bytes = 0;
     if (nb) {
         u64 f0 = di.ch0 + t.ch_seg0[di.ch0];
-        words = (u64)nb * 2 * (di.P + di.K + di.C);
-        bytes = (u64)nb * xstage_block(di);
+        words = nb * xscratch_block(di);
+        bytes = nb * xstage_block(di);
         for (u64 k = f0; k < f0 + x.n_fc; k++) {
-            words += (5ull + ((x.flags >> 1) & 1u)) * t.fc_nrows[k] + 3ull * t.fc_ndel[k];
+            words += xscratch_change(t, x, k);
             bytes += xstage_change(t, k);
         }
     }
@@ -1019,8 +1029,8 @@ struct XReg {
 };
 // LoroValues [p, p + n) copied into `s` with the key indices of nested maps translated from the source block's key
 // arena (doc-level key = key_map[src_key0 + idx]) to the output block's register (write_loro_value registers a map's
-// keys as it meets them: encoding/value.rs:1027-1036).  reg = true: first use registers (the sizing pass).
-__device__ inline void xvalue_copy(XSink& s, const u8* p, u32 n, const BatchTables& t, u64 src_key0, XReg& keys, bool reg) {
+// keys as it meets them: encoding/value.rs:1027-1036).
+__device__ inline void xvalue_copy(XSink& s, const u8* p, u32 n, const BatchTables& t, u64 src_key0, XReg& keys) {
     Cur c(p, n);
     u32 stack[24];
     int sp = 0;
@@ -1031,7 +1041,7 @@ __device__ inline void xvalue_copy(XSink& s, const u8* p, u32 n, const BatchTabl
             stack[sp - 1]--;
             if (stack[sp - 1] & 0x80000000u) {
                 u32 dk = t.key_map[src_key0 + (u32)c.varint()];
-                s.varint(reg ? keys.reg(dk) : keys.inv[dk]);
+                s.varint(keys.reg(dk));
             }
         }
         u8 kind = c.get();
@@ -1131,14 +1141,16 @@ __global__ void k_exp_posrank(const DocInfo* __restrict__ docs, u32 n_docs, cons
     if (lane == 0) t.xdoc[d].n_prank = carry;
 }
 
-// thread per output block.  pass 0: gather ops into scratch columns and registers while writing the values section
-// into the block's staging slot (`out` = the staging buffer), then every other section (column) writer stores its body
-// after it and its length into the XBlock;
-// a block whose pieces outgrow the slot only counts from there on and is flagged (XBlock::ovf).  pass 1, flagged
-// blocks only: the same writers once more, with the length prefixes, straight into the blob (`out` = the export
-// buffer, after k_exp_layout).
+// thread per output block: gather ops into scratch columns and registers while writing the values section into the
+// block's staging slot (`out` = the staging buffer), then every other section (column) writer stores its body after it
+// and its length into the XBlock.  A block whose pieces outgrow the slot only counts from there on, so its lengths are
+// exact, and is flagged (XBlock::ovf).  retry = 1, flagged blocks only: the same encode once more, into the slot
+// k_exp_layout gave the block in the retry buffer (`out`, from the document's restage0 on), which its lengths fill.
 // Two builds of the same code: <1> is compiled with __launch_bounds__(64, 5) (the compiler then schedules for 64-thread
-// CTAs: 136 registers against 124 without bounds, other load / store placement), <0> without bounds.
+// CTAs: 132 registers against 128 without bounds, other load / store placement), <0> without bounds.  Registers decide
+// the CTAs an SM holds: up to 128 give 8, up to 136 give 7, and each build is faster at its own count.  On one H100
+// 80GB HBM3 (700 W power limit), the bounded build at 127 registers (8 CTAs) took C5's re-export from 107 to 120 ms,
+// and the unbounded one at 132 (7 CTAs) took C3's at 4 k documents from 38.6 to 45.9 ms.
 // The host picks by the number of output blocks.  Re-export phase on one H100 80GB HBM3 (400 W power limit), unbounded
 // against bounded: C3 at 4 k documents (~55 k blocks) 39.1 against 46.6 ms; C5 at 10 k documents (160 k blocks) 128.5
 // against 106.4 ms; C3 at 40 k documents (~550 k blocks) 346.4 against 325.3 / 323.4 ms.  So batches of at least
@@ -1146,11 +1158,14 @@ __global__ void k_exp_posrank(const DocInfo* __restrict__ docs, u32 n_docs, cons
 #define LB_XENC_BOUNDED_MIN_BLOCKS 100000ull
 __device__ __forceinline__ void exp_encode_body(
     const DocInfo* __restrict__ docs, u64 n_blocks, const BatchTables& t, XBlock* __restrict__ xb,
-                             u32* __restrict__ scratch, u8* __restrict__ out, int pass) {
+                             u32* __restrict__ scratch, u8* __restrict__ out, int retry) {
     u64 bi_ = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (bi_ >= n_blocks) return;
     XBlock B = xb[bi_];
-    if (pass == 1 && !B.ovf) return;
+    if (retry) {
+        if (!B.ovf) return;
+        out += t.xdoc[B.doc].restage0;
+    }
     const DocInfo& di = docs[B.doc];
     const u32 P = di.P, K = di.K, C = di.C;
     u32* sc = scratch + B.scratch;
@@ -1162,8 +1177,7 @@ __device__ __forceinline__ void exp_encode_body(
     u32* c_prop = c_cidx + B.n_rows;
     u32* c_vt = c_prop + B.n_rows;
     u32* c_atoms = c_vt + B.n_rows;
-    u32* c_bytes = c_atoms + B.n_rows;         // text: payload bytes ; other: first row of the op
-    u32* d_peer = c_bytes + B.n_rows;          // delete columns, capacity n_dels each
+    u32* d_peer = c_atoms + B.n_rows;          // delete columns, capacity n_dels each
     u32* d_ctr = d_peer + B.n_dels;
     u32* d_len = d_ctr + B.n_dels;
     const bool has_tree = (t.xdoc[B.doc].flags & 2u) != 0;
@@ -1192,122 +1206,111 @@ __device__ __forceinline__ void exp_encode_body(
     const u32 first_src = t.fc_src[fc0];
     u32 n_dep = 0;
     for (u32 j = 0; j < N; j++) n_dep += t.fc_from[fc0 + j] ? 0u : t.ch_ndeps[t.fc_src[fc0 + j]];
-    if (pass == 0) {
-        for (u32 i = 0; i < P; i++) peers.inv[i] = 0xFFFFFFFFu;
-        for (u32 i = 0; i < K; i++) keys.inv[i] = 0xFFFFFFFFu;
-        for (u32 i = 0; i < C; i++) cids.inv[i] = 0xFFFFFFFFu;
-        peers.n = keys.n = cids.n = 0;
-        peers.reg(t.peer_map[t.blocks[t.ch_block[first_src]].peer0]);   // the author of the block's changes
-        B.n_pos = 0;
-        if (has_tree) {
-            // position register, pre-filled in sorted order (block_encode.rs:156-178): ranks of the block's create /
-            // move ops, heap-sorted, duplicates dropped
-            u32 m = 0;
-            for (u32 j = 0; j < N; j++) {
-                XRows it(t, t.fc_pos[fc0 + j], t.fc_r0[fc0 + j]);
-                u32 left = t.fc_nrows[fc0 + j];
-                while (left) {
-                    uint4 r = xr_rec(t, it.row());
-                    if ((r.x & 7u) == XK_TREE && t.tr_pos[r.w] != 0xFFFFFFFFu) p_rank[m++] = t.pos_rank[t.tr_pos[r.w]];
-                    left--;
-                    if (left) it.next();
-                }
-            }
-            auto sift = [&](u32 root, u32 end) {
-                while (true) {
-                    u32 c = 2 * root + 1;
-                    if (c >= end) break;
-                    if (c + 1 < end && p_rank[c + 1] > p_rank[c]) c++;
-                    if (p_rank[root] >= p_rank[c]) break;
-                    u32 tmp = p_rank[root]; p_rank[root] = p_rank[c]; p_rank[c] = tmp;
-                    root = c;
-                }
-            };
-            for (u32 i = m / 2; i-- > 0;) sift(i, m);
-            for (u32 e = m; e-- > 1;) { u32 tmp = p_rank[0]; p_rank[0] = p_rank[e]; p_rank[e] = tmp; sift(0, e); }
-            u32 w = 0;
-            for (u32 i = 0; i < m; i++) if (i == 0 || p_rank[i] != p_rank[w - 1]) p_rank[w++] = p_rank[i];
-            B.n_pos = w;
-        }
-        // ops in order: containers, map keys, delete targets (block_encode.rs:180-236).  The values section is written
-        // on the way, at the start of the staging slot: the op's value prefix once its rows are merged, then the
-        // payloads of those rows, which were just loaded (w_values is the same walk, for the direct encode)
-        XSink vs(out + B.stage, B.stage_cap);
-        u32 n_ops = 0, n_del = 0;
-        u32 prev_cidx = 0, prev_prop = 0, prev_dp = 0, prev_dc = 0, prev_dl = 0;   // 32-bit wrap-around deltas
+    for (u32 i = 0; i < P; i++) peers.inv[i] = 0xFFFFFFFFu;
+    for (u32 i = 0; i < K; i++) keys.inv[i] = 0xFFFFFFFFu;
+    for (u32 i = 0; i < C; i++) cids.inv[i] = 0xFFFFFFFFu;
+    peers.n = keys.n = cids.n = 0;
+    peers.reg(t.peer_map[t.blocks[t.ch_block[first_src]].peer0]);   // the author of the block's changes
+    B.n_pos = 0;
+    if (has_tree) {
+        // position register, pre-filled in sorted order (block_encode.rs:156-178): ranks of the block's create /
+        // move ops, heap-sorted, duplicates dropped
+        u32 m = 0;
         for (u32 j = 0; j < N; j++) {
             XRows it(t, t.fc_pos[fc0 + j], t.fc_r0[fc0 + j]);
             u32 left = t.fc_nrows[fc0 + j];
-            u32 skip = t.fc_skip[fc0 + j];   // only the first op of a change cut at the `from` version
             while (left) {
-                u32 first_row = (u32)it.row();
-                XRows it0 = it;
-                const u32 left0 = left;
-                const u32 skip0 = skip;
-                XOp o = xop_gather(t, di, it, left, nullptr, skip);
-                skip = left ? it.skip : 0u;   // (the next op may start on the first kept row of a trimmed change)
-                if (o.xk == XK_LIST) { vs.put(7); vs.varint(o.atoms); }
-                else if (o.xk == XK_TEXT) vs.varint(o.f1 - o.f0);
-                // DeltaRle columns are stored as deltas right away (the encoders then read every value once)
-                u32 lc = cids.reg(o.cidx);
-                u32 lp = (o.xk == XK_MAPSET || o.xk == XK_MAPDEL) ? keys.reg((u32)o.prop) : (u32)o.prop;
-                if (o.xk == XK_LIST || o.xk == XK_TEXT || o.xk == XK_MAPSET) {
-                    // payloads after the op's own registrations: nested keys register in value order
-                    u32 k = left0 - left;
-                    while (k) {
-                        const u8* pp;
-                        u32 pn;
-                        xr_payload_skip(t, it0.row(), o.xk, k == left0 - left ? skip0 : it0.skip, &pp, &pn);
-                        if (has_maps && o.xk != XK_TEXT) xvalue_copy(vs, pp, pn, t, t.blocks[t.ch_block[it0.ch]].key0, keys, true);
-                        else vs.copy(pp, pn);
-                        k--;
-                        if (k) it0.next();
-                    }
-                }
-                c_cidx[n_ops] = lc - prev_cidx; prev_cidx = lc;
-                c_prop[n_ops] = lp - prev_prop; prev_prop = lp;
-                c_vt[n_ops] = xk_value_type(o.xk) | ((u32)o.xk << 8);
-                c_atoms[n_ops] = o.atoms;
-                c_bytes[n_ops] = o.xk == XK_TEXT ? o.f1 - o.f0 : first_row;
-                if (o.xk == XK_TREE) {      // encode_tree_op (block_encode.rs:324-362): subject peer, then parent peer
-                    uint4 ids = t.tr_ids[o.f0];
-                    peers.reg(ids.x);
-                    if ((ids.z & 3u) != TRP_ROOT) peers.reg(ids.z >> 2);
-                    w_tree_value(vs, o.f0);
-                }
-                if (o.xk == XK_DEL) {
-                    u32 dp = peers.reg(o.f0);
-                    d_peer[n_del] = dp - prev_dp; prev_dp = dp;
-                    d_ctr[n_del] = o.f1 - prev_dc; prev_dc = o.f1;
-                    d_len[n_del] = (u32)o.f2 - prev_dl; prev_dl = (u32)o.f2;
-                    n_del++;
-                }
-                n_ops++;
+                uint4 r = xr_rec(t, it.row());
+                if ((r.x & 7u) == XK_TREE && t.tr_pos[r.w] != 0xFFFFFFFFu) p_rank[m++] = t.pos_rank[t.tr_pos[r.w]];
+                left--;
+                if (left) it.next();
             }
         }
-        B.n_ops = n_ops;
-        B.n_del_ops = n_del;
-        B.sec_len[7] = (u32)vs.n;   // values section: written with the gather, no second walk
-        // ContainerArena::from_containers (arena.rs:103-147): roots register their name, normals their peer
-        for (u32 i = 0; i < cids.n; i++) {
-            const DocContainer& dc = t.dcont[di.cid0 + cids.ord[i]];
-            if (dc.is_root) keys.reg(dc.key_or_peer); else peers.reg(dc.key_or_peer);
-        }
-        // encode_changes (block_meta_encode.rs:13-88): dependency peers
-        for (u32 j = 0; j < N; j++) {
-            if (t.fc_from[fc0 + j]) continue;
-            u32 src = t.fc_src[fc0 + j];
-            const BlockInfo& sb = t.blocks[t.ch_block[src]];
-            for (u32 k = 0; k < t.ch_ndeps[src]; k++) peers.reg(t.peer_map[sb.peer0 + t.dep_peer_idx[t.ch_dep0[src] + k]]);
-        }
-        B.col_len[7] = peers.n | (keys.n << 16);
-        B.n_cids = cids.n;
-    } else {
-        peers.n = B.col_len[7] & 0xFFFFu;
-        keys.n = B.col_len[7] >> 16;
-        cids.n = B.n_cids;
+        auto sift = [&](u32 root, u32 end) {
+            while (true) {
+                u32 c = 2 * root + 1;
+                if (c >= end) break;
+                if (c + 1 < end && p_rank[c + 1] > p_rank[c]) c++;
+                if (p_rank[root] >= p_rank[c]) break;
+                u32 tmp = p_rank[root]; p_rank[root] = p_rank[c]; p_rank[c] = tmp;
+                root = c;
+            }
+        };
+        for (u32 i = m / 2; i-- > 0;) sift(i, m);
+        for (u32 e = m; e-- > 1;) { u32 tmp = p_rank[0]; p_rank[0] = p_rank[e]; p_rank[e] = tmp; sift(0, e); }
+        u32 w = 0;
+        for (u32 i = 0; i < m; i++) if (i == 0 || p_rank[i] != p_rank[w - 1]) p_rank[w++] = p_rank[i];
+        B.n_pos = w;
     }
-    const u32 n_ops = B.n_ops, n_del = B.n_del_ops;
+    // ops in order: containers, map keys, delete targets (block_encode.rs:180-236).  The values section is written
+    // on the way, at the start of the staging slot: the op's value prefix once its rows are merged, then the
+    // payloads of those rows, which were just loaded
+    XSink vs(out + B.stage, B.stage_cap);
+    u32 n_ops = 0, n_del = 0;
+    u32 prev_cidx = 0, prev_prop = 0, prev_dp = 0, prev_dc = 0, prev_dl = 0;   // 32-bit wrap-around deltas
+    for (u32 j = 0; j < N; j++) {
+        XRows it(t, t.fc_pos[fc0 + j], t.fc_r0[fc0 + j]);
+        u32 left = t.fc_nrows[fc0 + j];
+        u32 skip = t.fc_skip[fc0 + j];   // only the first op of a change cut at the `from` version
+        while (left) {
+            XRows it0 = it;
+            const u32 left0 = left;
+            const u32 skip0 = skip;
+            XOp o = xop_gather(t, di, it, left, nullptr, skip);
+            skip = left ? it.skip : 0u;   // (the next op may start on the first kept row of a trimmed change)
+            if (o.xk == XK_LIST) { vs.put(7); vs.varint(o.atoms); }
+            else if (o.xk == XK_TEXT) vs.varint(o.f1 - o.f0);
+            // DeltaRle columns are stored as deltas right away (the encoders then read every value once)
+            u32 lc = cids.reg(o.cidx);
+            u32 lp = (o.xk == XK_MAPSET || o.xk == XK_MAPDEL) ? keys.reg((u32)o.prop) : (u32)o.prop;
+            if (o.xk == XK_LIST || o.xk == XK_TEXT || o.xk == XK_MAPSET) {
+                // payloads after the op's own registrations: nested keys register in value order
+                u32 k = left0 - left;
+                while (k) {
+                    const u8* pp;
+                    u32 pn;
+                    xr_payload_skip(t, it0.row(), o.xk, k == left0 - left ? skip0 : it0.skip, &pp, &pn);
+                    if (has_maps && o.xk != XK_TEXT) xvalue_copy(vs, pp, pn, t, t.blocks[t.ch_block[it0.ch]].key0, keys);
+                    else vs.copy(pp, pn);
+                    k--;
+                    if (k) it0.next();
+                }
+            }
+            c_cidx[n_ops] = lc - prev_cidx; prev_cidx = lc;
+            c_prop[n_ops] = lp - prev_prop; prev_prop = lp;
+            c_vt[n_ops] = xk_value_type(o.xk);
+            c_atoms[n_ops] = o.atoms;
+            if (o.xk == XK_TREE) {      // encode_tree_op (block_encode.rs:324-362): subject peer, then parent peer
+                uint4 ids = t.tr_ids[o.f0];
+                peers.reg(ids.x);
+                if ((ids.z & 3u) != TRP_ROOT) peers.reg(ids.z >> 2);
+                w_tree_value(vs, o.f0);
+            }
+            if (o.xk == XK_DEL) {
+                u32 dp = peers.reg(o.f0);
+                d_peer[n_del] = dp - prev_dp; prev_dp = dp;
+                d_ctr[n_del] = o.f1 - prev_dc; prev_dc = o.f1;
+                d_len[n_del] = (u32)o.f2 - prev_dl; prev_dl = (u32)o.f2;
+                n_del++;
+            }
+            n_ops++;
+        }
+    }
+    B.n_ops = n_ops;
+    B.n_del_ops = n_del;
+    B.sec_len[7] = (u32)vs.n;   // values section: written with the gather
+    // ContainerArena::from_containers (arena.rs:103-147): roots register their name, normals their peer
+    for (u32 i = 0; i < cids.n; i++) {
+        const DocContainer& dc = t.dcont[di.cid0 + cids.ord[i]];
+        if (dc.is_root) keys.reg(dc.key_or_peer); else peers.reg(dc.key_or_peer);
+    }
+    // encode_changes (block_meta_encode.rs:13-88): dependency peers
+    for (u32 j = 0; j < N; j++) {
+        if (t.fc_from[fc0 + j]) continue;
+        u32 src = t.fc_src[fc0 + j];
+        const BlockInfo& sb = t.blocks[t.ch_block[src]];
+        for (u32 k = 0; k < t.ch_ndeps[src]; k++) peers.reg(t.peer_map[sb.peer0 + t.dep_peer_idx[t.ch_dep0[src] + k]]);
+    }
 
     // ------------------------------------------------------------------ section writers (count or write)
     auto dep_self = [&](u32 j) -> bool { return t.fc_from[fc0 + j] ? true : t.ch_dep_self[t.fc_src[fc0 + j]] != 0; };
@@ -1361,7 +1364,7 @@ __device__ __forceinline__ void exp_encode_body(
         switch (col) {
             case 0: enc_anyrle(s, n_ops, [&](u32 i) -> i64 { return (i64)(i32)c_cidx[i]; }, WrZigzag()); break;
             case 1: enc_anyrle(s, n_ops, [&](u32 i) -> i64 { return (i64)(i32)c_prop[i]; }, WrZigzag()); break;
-            case 2: enc_anyrle(s, n_ops, [&](u32 i) -> i64 { return (i64)(c_vt[i] & 0xFFu); }, WrByte()); break;
+            case 2: enc_anyrle(s, n_ops, [&](u32 i) -> i64 { return (i64)c_vt[i]; }, WrByte()); break;
             default: enc_anyrle(s, n_ops, [&](u32 i) -> i64 { return (i64)c_atoms[i]; }, WrVarint());
         }
     };
@@ -1370,36 +1373,6 @@ __device__ __forceinline__ void exp_encode_body(
             case 0: enc_anyrle(s, n_del, [&](u32 i) -> i64 { return (i64)(i32)d_peer[i]; }, WrZigzag()); break;
             case 1: enc_anyrle(s, n_del, [&](u32 i) -> i64 { return (i64)(i32)d_ctr[i]; }, WrZigzag()); break;
             default: enc_anyrle(s, n_del, [&](u32 i) -> i64 { return (i64)(i32)d_len[i]; }, WrZigzag());
-        }
-    };
-    auto w_values = [&](XSink& s) {
-        u32 op = 0;
-        u32 xk = XK_NONE;
-        for (u32 j = 0; j < N; j++) {
-            XRows it(t, t.fc_pos[fc0 + j], t.fc_r0[fc0 + j]);
-            u32 left = t.fc_nrows[fc0 + j];
-            u32 skip = t.fc_skip[fc0 + j];
-            bool fresh = true;
-            while (left) {
-                u64 row = it.row();
-                if (fresh || (xr_flag(t, row) & XF_HEAD)) {
-                    xk = c_vt[op] >> 8;
-                    if (xk == XK_LIST) { s.put(7); s.varint(c_atoms[op]); }
-                    else if (xk == XK_TEXT) s.varint(c_bytes[op]);
-                    else if (xk == XK_TREE) w_tree_value(s, xr_rec(t, row).w);
-                    op++;
-                }
-                fresh = false;
-                if (xk == XK_LIST || xk == XK_TEXT || xk == XK_MAPSET) {
-                    const u8* pp;
-                    u32 pn;
-                    xr_payload_skip(t, row, xk, skip, &pp, &pn);
-                    if (has_maps && xk != XK_TEXT) xvalue_copy(s, pp, pn, t, t.blocks[t.ch_block[it.ch]].key0, keys, false);
-                    else s.copy(pp, pn);
-                }
-                left--;
-                if (left) { it.next(); skip = it.skip; }
-            }
         }
     };
     // PositionArena::from_positions + encode_v2 (arena.rs:168-183, 218-224): common prefix with the predecessor
@@ -1429,90 +1402,61 @@ __device__ __forceinline__ void exp_encode_body(
     u32 counter0 = (u32)t.ch_counter[first_src] + t.fc_from[fc0];
     u32 lam0 = (u32)lamport(0);
     u32 lam_len = (u32)lamport(N - 1) + t.fc_atoms[B.fc1 - 1] - lam0;
-    if (pass == 0) {
-        // staged pieces: the values (written by the gather), then in blob order the five header varints, the bodies of
-        // sections 0-3, the position columns, the op columns, the delete columns (k_exp_finish adds the prefixes)
-        XSink s(out + B.stage, B.stage_cap);
-        s.n = B.sec_len[7];
-        s.varint(counter0);
-        s.varint(counter_len);
-        s.varint(lam0);
-        s.varint(lam_len);
-        s.varint(N);
-        u64 m = s.n;
-        w_header(s); B.sec_len[0] = (u32)(s.n - m); m = s.n;
-        w_meta(s); B.sec_len[1] = (u32)(s.n - m); m = s.n;
-        w_cids(s); B.sec_len[2] = (u32)(s.n - m); m = s.n;
-        w_keys(s); B.sec_len[3] = (u32)(s.n - m); m = s.n;
-        u32 tot = 0;
-        if (B.n_pos) {
-            tot = 2;   // varint(1) varint(2)
-            for (int c = 0; c < 2; c++) { w_poscol(s, c); B.col_len[8 + c] = (u32)(s.n - m); m = s.n; tot += varint_len(B.col_len[8 + c]) + B.col_len[8 + c]; }
-        }
-        B.sec_len[4] = tot;
-        tot = 2;   // varint(1) varint(4)
-        for (int c = 0; c < 4; c++) { w_opcol(s, c); B.col_len[c] = (u32)(s.n - m); m = s.n; tot += varint_len(B.col_len[c]) + B.col_len[c]; }
-        B.sec_len[5] = tot;
-        if (n_del) {
-            tot = 2;
-            for (int c = 0; c < 3; c++) { w_delcol(s, c); B.col_len[4 + c] = (u32)(s.n - m); m = s.n; tot += varint_len(B.col_len[4 + c]) + B.col_len[4 + c]; }
-            B.sec_len[6] = tot;
-        } else B.sec_len[6] = 0;
-        B.ovf = s.n > s.cap;
-        u32 len = varint_len(counter0) + varint_len(counter_len) + varint_len(lam0) + varint_len(lam_len) + varint_len(N);
-        for (int i = 0; i < 8; i++) len += varint_len(B.sec_len[i]) + B.sec_len[i];
-        B.len = len;
-        xb[bi_] = B;
-        return;
-    }
-    // ---- pass 1 (blocks that outgrew their slot): ULEB length prefix + block bytes at the document's slot
-    u64 base = t.xdoc[B.doc].exp_off + B.off;
-    XSink s(out + base - varint_len(B.len), ~0ull);
-    s.varint(B.len);
+    // staged pieces: the values (written by the gather), then in blob order the five header varints, the bodies of
+    // sections 0-3, the position columns, the op columns, the delete columns (k_exp_finish adds the prefixes)
+    XSink s(out + B.stage, B.stage_cap);
+    s.n = B.sec_len[7];
     s.varint(counter0);
     s.varint(counter_len);
     s.varint(lam0);
     s.varint(lam_len);
     s.varint(N);
-    s.varint(B.sec_len[0]); w_header(s);
-    s.varint(B.sec_len[1]); w_meta(s);
-    s.varint(B.sec_len[2]); w_cids(s);
-    s.varint(B.sec_len[3]); w_keys(s);
-    s.varint(B.sec_len[4]);
+    u64 m = s.n;
+    w_header(s); B.sec_len[0] = (u32)(s.n - m); m = s.n;
+    w_meta(s); B.sec_len[1] = (u32)(s.n - m); m = s.n;
+    w_cids(s); B.sec_len[2] = (u32)(s.n - m); m = s.n;
+    w_keys(s); B.sec_len[3] = (u32)(s.n - m); m = s.n;
+    u32 tot = 0;
     if (B.n_pos) {
-        s.varint(1); s.varint(2);
-        for (int c = 0; c < 2; c++) { s.varint(B.col_len[8 + c]); w_poscol(s, c); }
+        tot = 2;   // varint(1) varint(2)
+        for (int c = 0; c < 2; c++) { w_poscol(s, c); B.col_len[7 + c] = (u32)(s.n - m); m = s.n; tot += varint_len(B.col_len[7 + c]) + B.col_len[7 + c]; }
     }
-    s.varint(B.sec_len[5]);
-    s.varint(1); s.varint(4);
-    for (int c = 0; c < 4; c++) { s.varint(B.col_len[c]); w_opcol(s, c); }
-    s.varint(B.sec_len[6]);
+    B.sec_len[4] = tot;
+    tot = 2;   // varint(1) varint(4)
+    for (int c = 0; c < 4; c++) { w_opcol(s, c); B.col_len[c] = (u32)(s.n - m); m = s.n; tot += varint_len(B.col_len[c]) + B.col_len[c]; }
+    B.sec_len[5] = tot;
     if (n_del) {
-        s.varint(1); s.varint(3);
-        for (int c = 0; c < 3; c++) { s.varint(B.col_len[4 + c]); w_delcol(s, c); }
-    }
-    s.varint(B.sec_len[7]); w_values(s);
+        tot = 2;
+        for (int c = 0; c < 3; c++) { w_delcol(s, c); B.col_len[4 + c] = (u32)(s.n - m); m = s.n; tot += varint_len(B.col_len[4 + c]) + B.col_len[4 + c]; }
+        B.sec_len[6] = tot;
+    } else B.sec_len[6] = 0;
+    B.ovf |= s.n > s.cap;   // still set after the retry: k_exp_finish then reads the retry slot
+    u32 len = varint_len(counter0) + varint_len(counter_len) + varint_len(lam0) + varint_len(lam_len) + varint_len(N);
+    for (int i = 0; i < 8; i++) len += varint_len(B.sec_len[i]) + B.sec_len[i];
+    B.len = len;
+    xb[bi_] = B;
 }
 
 template <int CAPPED> __global__ void k_exp_encode(const DocInfo* __restrict__ docs, u64 n_blocks, const __grid_constant__ BatchTables t, XBlock* __restrict__ xb,
-                                                 u32* __restrict__ scratch, u8* __restrict__ out, int pass);
+                                                 u32* __restrict__ scratch, u8* __restrict__ out, int retry);
 template <> __global__ void k_exp_encode<0>(const DocInfo* __restrict__ docs, u64 n_blocks, const __grid_constant__ BatchTables t, XBlock* __restrict__ xb,
-                                            u32* __restrict__ scratch, u8* __restrict__ out, int pass) {
-    exp_encode_body(docs, n_blocks, t, xb, scratch, out, pass);
+                                            u32* __restrict__ scratch, u8* __restrict__ out, int retry) {
+    exp_encode_body(docs, n_blocks, t, xb, scratch, out, retry);
 }
 template <> __global__ void __launch_bounds__(64, 5) k_exp_encode<1>(const DocInfo* __restrict__ docs, u64 n_blocks, const __grid_constant__ BatchTables t,
                                                                      XBlock* __restrict__ xb, u32* __restrict__ scratch,
-                                                                     u8* __restrict__ out, int pass) {
-    exp_encode_body(docs, n_blocks, t, xb, scratch, out, pass);
+                                                                     u8* __restrict__ out, int retry) {
+    exp_encode_body(docs, n_blocks, t, xb, scratch, out, retry);
 }
 
-// thread per document: block offsets inside the blob, blob length, blocks that outgrew their slot (after encode pass 0)
+// thread per document, after the encode: block offsets inside the blob, blob length, and the blocks that outgrew their
+// slot, each given a retry slot of its block length (an upper bound on its pieces) at a document-relative offset
 __global__ void k_exp_layout(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t, XBlock* __restrict__ xb,
-                             u32* __restrict__ padded_len, u32* __restrict__ n_ovf) {
+                             u32* __restrict__ padded_len, u32* __restrict__ n_ovf, u32* __restrict__ n_restage) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
     XDoc& x = t.xdoc[d];
-    u32 len = 0, ovf = 0;
+    u32 len = 0, ovf = 0, restage = 0;
     if (docs[d].code == DOC_OK && !(x.flags & 1)) {
         len = 22;
         for (u32 i = 0; i < x.n_mb; i++) {
@@ -1520,18 +1464,24 @@ __global__ void k_exp_layout(const DocInfo* __restrict__ docs, u32 n_docs, const
             len += varint_len(b.len);
             b.off = len;
             len += b.len;
-            ovf += b.ovf;
+            if (b.ovf) {
+                ovf++;
+                b.stage = restage;
+                b.stage_cap = b.len;
+                restage += b.len;
+            }
         }
     }
     x.exp_len = len;
     padded_len[d] = (len + 15u) & ~15u;
     n_ovf[d] = ovf;
+    n_restage[d] = restage;
 }
 
-// warp per document: the blob from the staged pieces of its blocks and their length prefixes (the blocks that
-// outgrew their slot are in place already), then header, mode, checksum (encoding.rs:397-416)
+// warp per document: the blob from the staged pieces of its blocks (in the retry buffer for the blocks that outgrew
+// their first slot) and their length prefixes, then header, mode, checksum (encoding.rs:397-416)
 __global__ void k_exp_finish(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t, const XBlock* __restrict__ xb,
-                             const u8* __restrict__ stage, u8* __restrict__ out) {
+                             const u8* __restrict__ stage, const u8* __restrict__ restage, u8* __restrict__ out) {
     u32 d = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // warp per document: the checksum walks the whole blob
     int lane = threadIdx.x & 31;
     if (d >= n_docs) return;
@@ -1540,9 +1490,8 @@ __global__ void k_exp_finish(const DocInfo* __restrict__ docs, u32 n_docs, const
     u8* b = out + x.exp_off;
     for (u32 i = 0; i < x.n_mb; i++) {
         const XBlock& B = xb[x.ob0 + i];
-        if (B.ovf) continue;
         u8* dst = b + B.off - varint_len(B.len);
-        const u8* src = stage + B.stage;
+        const u8* src = (B.ovf ? restage + x.restage0 : stage) + B.stage;
         u64 o = 0, so = B.sec_len[7];   // the values come first in the slot and last in the block
         auto prefix = [&](u32 v) {
             if (lane == 0) { XSink s(dst + o, ~0ull); s.varint(v); }
@@ -1568,7 +1517,7 @@ __global__ void k_exp_finish(const DocInfo* __restrict__ docs, u32 n_docs, const
         prefix(B.sec_len[4]);
         if (B.n_pos) {
             prefix(1); prefix(2);
-            for (int c = 0; c < 2; c++) { prefix(B.col_len[8 + c]); piece(B.col_len[8 + c]); }
+            for (int c = 0; c < 2; c++) { prefix(B.col_len[7 + c]); piece(B.col_len[7 + c]); }
         }
         prefix(B.sec_len[5]);
         prefix(1); prefix(4);

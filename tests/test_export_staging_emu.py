@@ -1,9 +1,9 @@
 """Phase 7 (re-export) on the emulated kernels with staging slots smaller than the blocks need.
 
 The encoder writes each output block once, into a staging slot sized from the block's rows and store estimate, and
-the blobs are assembled from the slots.  A block that outgrows its slot is encoded a second time, straight into the
-blob.  LB_EXPORT_STAGE_CAP caps every slot's capacity (in bytes): 0 sends every block down that second path, a
-small cap only the larger blocks.  Either way the bytes must stay the oracle's."""
+the blobs are assembled from the slots.  A block that outgrows its slot is encoded again by the same code, into a
+retry slot of its exact size.  LB_EXPORT_STAGE_CAP caps every first slot's capacity (in bytes): 0 sends every block
+through the retry, a small cap only the larger blocks.  Either way the bytes must stay the oracle's."""
 import gzip
 import os
 import re
