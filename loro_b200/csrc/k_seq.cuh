@@ -59,42 +59,44 @@ struct SeqSmem {   // one per warp
     u32 parent[LB_SEQ_NS];
     u32 abase[32];     // atom_base of the document's first 32 peers
     i32 cvv[32];       // tracker version of the active container, first 32 peers
+    // The same for all 32 lanes and changed only per document or per container switch: kept here rather than in
+    // registers, where every helper call would carry them and the kernel spilled them at its register budget.
+    const DocPeer* dpeer;   // the document's peers
+    u64 atom0;              // the document's first atom
+    u64 leaf0, node0, cvv0; // pool bases of the active container
+    u32 P;                  // the document's peers
     // active container
     u32 root, height, first_leaf, n_leaves, n_nodes, unk_leaf, leaf_cap, node_cap;
     u32 err;
-    u32 pad;
 };
 
-// Everything a helper needs besides the pools; passed by value, lives in registers.
-struct Cx {
-    SeqSmem* sm;
-    const DocPeer* dpeer;   // the document's peers
-    u64 leaf0, node0, atom0, cvv0;
-    u32 P;
-    int lane;
-};
+// The warp's SeqSmem.  The __noinline__ helpers take it from here instead of as an argument: a shared-memory address
+// computed from the thread index needs no register across a call.
+__shared__ SeqSmem seq_smem[LB_SEQ_WARPS];
+__device__ __forceinline__ SeqSmem* seq_sm() { return &seq_smem[threadIdx.x >> 5]; }
+__device__ __forceinline__ int seq_lane() { return (int)(threadIdx.x & 31); }
 
 __device__ __forceinline__ uint4 mk4(u32 x, u32 y, u32 z, u32 w) { uint4 r; r.x = x; r.y = y; r.z = z; r.w = w; return r; }
 __device__ __forceinline__ uint2 mk2(u32 x, u32 y) { uint2 r; r.x = x; r.y = y; return r; }
-__device__ __forceinline__ void seq_fail(const Cx& c, u32 code) {
-    if (c.lane == 0 && c.sm->err == 0) c.sm->err = code;
+__device__ __forceinline__ void seq_fail(SeqSmem* sm, u32 code) {
+    if (seq_lane() == 0 && sm->err == 0) sm->err = code;
     __syncwarp();
 }
-__device__ __forceinline__ u64 atom_index(const Cx& c, u32 peer, i32 ctr) {
-    u32 base = peer < 32 ? c.sm->abase[peer] : c.dpeer[peer].atom_base;
-    return c.atom0 + base + (u32)ctr;
+__device__ __forceinline__ u64 atom_index(SeqSmem* sm, u32 peer, i32 ctr) {
+    u32 base = peer < 32 ? sm->abase[peer] : sm->dpeer[peer].atom_base;
+    return sm->atom0 + base + (u32)ctr;
 }
-__device__ __forceinline__ i32 cvv_get(const SeqPools& p, const Cx& c, u32 q) { return q < 32 ? c.sm->cvv[q] : p.cvv[c.cvv0 + q]; }
-__device__ __forceinline__ void cvv_set(const SeqPools& p, const Cx& c, u32 q, i32 v) { if (q < 32) c.sm->cvv[q] = v; else p.cvv[c.cvv0 + q] = v; }
+__device__ __forceinline__ i32 cvv_get(const SeqPools& p, SeqSmem* sm, u32 q) { return q < 32 ? sm->cvv[q] : p.cvv[sm->cvv0 + q]; }
+__device__ __forceinline__ void cvv_set(const SeqPools& p, SeqSmem* sm, u32 q, i32 v) { if (q < 32) sm->cvv[q] = v; else p.cvv[sm->cvv0 + q] = v; }
 
 // ---- slots
 __device__ __forceinline__ u32 s_peer(const uint4& s) { return s.x & 0xFFFFu; }
 __device__ __forceinline__ u32 s_st(const uint4& s) { return s.x >> 16; }
 __device__ __forceinline__ i32 s_vis(const uint4& s) { return (s.x >> 16) == 0 ? (i32)s.z : 0; }
-__device__ __forceinline__ uint4 leaf_load(const SeqPools& p, const Cx& c, u32 leaf) { return p.leaf[(c.leaf0 + leaf) * 32 + c.lane]; }
+__device__ __forceinline__ uint4 leaf_load(const SeqPools& p, SeqSmem* sm, u32 leaf) { return p.leaf[(sm->leaf0 + leaf) * 32 + seq_lane()]; }
 // slots below `from` are unchanged by the caller: only the shifted tail goes back to HBM
-__device__ __forceinline__ void leaf_store(const SeqPools& p, const Cx& c, u32 leaf, const uint4& L, int from = 0) {
-    if (c.lane >= from) p.leaf[(c.leaf0 + leaf) * 32 + c.lane] = L;
+__device__ __forceinline__ void leaf_store(const SeqPools& p, SeqSmem* sm, u32 leaf, const uint4& L, int from = 0) {
+    if (seq_lane() >= from) p.leaf[(sm->leaf0 + leaf) * 32 + seq_lane()] = L;
     __syncwarp();
 }
 __device__ __forceinline__ int leaf_count(const uint4& L) { return __popc(__ballot_sync(LB_FULL, s_peer(L) != PEER_NONE)); }
@@ -105,43 +107,43 @@ __device__ __forceinline__ int slot_of(const uint4& L, u32 peer, i32 ctr) {
 }
 
 // ---- nodes (shared-memory cache for ids < NS)
-__device__ __forceinline__ uint2 nd_get(const SeqPools& p, const Cx& c, u32 nd, int i) {
-    return nd < LB_SEQ_NS ? mk2(c.sm->child[nd][i], (u32)c.sm->vis[nd][i]) : p.node[(c.node0 + nd) * 32 + i];
+__device__ __forceinline__ uint2 nd_get(const SeqPools& p, SeqSmem* sm, u32 nd, int i) {
+    return nd < LB_SEQ_NS ? mk2(sm->child[nd][i], (u32)sm->vis[nd][i]) : p.node[(sm->node0 + nd) * 32 + i];
 }
-__device__ __forceinline__ void nd_set(const SeqPools& p, const Cx& c, u32 nd, int i, u32 child, i32 vis) {
-    if (nd < LB_SEQ_NS) { c.sm->child[nd][i] = child; c.sm->vis[nd][i] = vis; }
-    else p.node[(c.node0 + nd) * 32 + i] = mk2(child, (u32)vis);
+__device__ __forceinline__ void nd_set(const SeqPools& p, SeqSmem* sm, u32 nd, int i, u32 child, i32 vis) {
+    if (nd < LB_SEQ_NS) { sm->child[nd][i] = child; sm->vis[nd][i] = vis; }
+    else p.node[(sm->node0 + nd) * 32 + i] = mk2(child, (u32)vis);
 }
-__device__ __forceinline__ u32 nd_parent(const SeqPools& p, const Cx& c, u32 nd) {
-    return nd < LB_SEQ_NS ? c.sm->parent[nd] : p.node_parent[c.node0 + nd];
+__device__ __forceinline__ u32 nd_parent(const SeqPools& p, SeqSmem* sm, u32 nd) {
+    return nd < LB_SEQ_NS ? sm->parent[nd] : p.node_parent[sm->node0 + nd];
 }
-__device__ __forceinline__ void nd_set_parent(const SeqPools& p, const Cx& c, u32 nd, u32 v) {
-    if (nd < LB_SEQ_NS) c.sm->parent[nd] = v; else p.node_parent[c.node0 + nd] = v;
+__device__ __forceinline__ void nd_set_parent(const SeqPools& p, SeqSmem* sm, u32 nd, u32 v) {
+    if (nd < LB_SEQ_NS) sm->parent[nd] = v; else p.node_parent[sm->node0 + nd] = v;
 }
-__device__ __forceinline__ void nd_add_vis(const SeqPools& p, const Cx& c, u32 nd, int i, i32 d) {
-    if (nd < LB_SEQ_NS) c.sm->vis[nd][i] += d;
-    else { uint2* q = &p.node[(c.node0 + nd) * 32 + i]; q->y = (u32)((i32)q->y + d); }
+__device__ __forceinline__ void nd_add_vis(const SeqPools& p, SeqSmem* sm, u32 nd, int i, i32 d) {
+    if (nd < LB_SEQ_NS) sm->vis[nd][i] += d;
+    else { uint2* q = &p.node[(sm->node0 + nd) * 32 + i]; q->y = (u32)((i32)q->y + d); }
 }
-__device__ __forceinline__ void set_child_link(const SeqPools& p, const Cx& c, bool kids_are_leaves, u32 child, u32 link) {
-    if (kids_are_leaves) p.leaf[(c.leaf0 + child) * 32].w = link; else nd_set_parent(p, c, child, link);
+__device__ __forceinline__ void set_child_link(const SeqPools& p, SeqSmem* sm, bool kids_are_leaves, u32 child, u32 link) {
+    if (kids_are_leaves) p.leaf[(sm->leaf0 + child) * 32].w = link; else nd_set_parent(p, sm, child, link);
 }
 // add `delta` visible atoms on the path (parent link of a leaf) -> root
-__device__ __forceinline__ void add_vis(const SeqPools& p, const Cx& c, u32 link, i32 delta) {
-    if (delta != 0 && c.lane == 0) {
+__device__ __forceinline__ void add_vis(const SeqPools& p, SeqSmem* sm, u32 link, i32 delta) {
+    if (delta != 0 && seq_lane() == 0) {
         while (link != NODE_NONE) {
             u32 nd = link >> 5;
-            nd_add_vis(p, c, nd, (int)(link & 31), delta);
-            link = nd_parent(p, c, nd);
+            nd_add_vis(p, sm, nd, (int)(link & 31), delta);
+            link = nd_parent(p, sm, nd);
         }
     }
     __syncwarp();
 }
 
 // ---- insert (child, vis) into node `nd` right after index `after`; room must exist
-__device__ __forceinline__ void node_insert_no_split(const SeqPools& p, const Cx& c, u32 nd, int after, u32 child, i32 vis,
+__device__ __forceinline__ void node_insert_no_split(const SeqPools& p, SeqSmem* sm, u32 nd, int after, u32 child, i32 vis,
                                                      bool kids_are_leaves) {
-    int lane = c.lane;
-    uint2 e = nd_get(p, c, nd, lane);
+    int lane = seq_lane();
+    uint2 e = nd_get(p, sm, nd, lane);
     int n = __popc(__ballot_sync(LB_FULL, e.x != NODE_NONE));
     u32 c_up = __shfl_up_sync(LB_FULL, e.x, 1);
     u32 v_up = __shfl_up_sync(LB_FULL, e.y, 1);
@@ -149,22 +151,22 @@ __device__ __forceinline__ void node_insert_no_split(const SeqPools& p, const Cx
     if (lane == at) { e.x = child; e.y = (u32)vis; }
     else if (lane > at) { e.x = c_up; e.y = v_up; }
     __syncwarp();
-    if (lane <= n) nd_set(p, c, nd, lane, e.x, (i32)e.y);
-    if (lane >= at && lane <= n) set_child_link(p, c, kids_are_leaves, e.x, (nd << 5) | (u32)lane);
+    if (lane <= n) nd_set(p, sm, nd, lane, e.x, (i32)e.y);
+    if (lane >= at && lane <= n) set_child_link(p, sm, kids_are_leaves, e.x, (nd << 5) | (u32)lane);
     __syncwarp();
 }
-__device__ __forceinline__ i32 node_total(const SeqPools& p, const Cx& c, u32 nd) {
-    return warp_sum((i32)nd_get(p, c, nd, c.lane).y);
+__device__ __forceinline__ i32 node_total(const SeqPools& p, SeqSmem* sm, u32 nd) {
+    return warp_sum((i32)nd_get(p, sm, nd, seq_lane()).y);
 }
 // ---- insert with splits propagating upward
-__device__ __noinline__ void node_insert(const SeqPools& p, Cx c, u32 nd, int after, u32 child, i32 vis, bool kids_are_leaves) {
-    SeqSmem* sm = c.sm;
-    int lane = c.lane;
+__device__ __noinline__ void node_insert(const SeqPools& p, u32 nd, int after, u32 child, i32 vis, bool kids_are_leaves) {
+    SeqSmem* sm = seq_sm();
+    int lane = seq_lane();
     while (true) {
-        uint2 e = nd_get(p, c, nd, lane);
+        uint2 e = nd_get(p, sm, nd, lane);
         int n = __popc(__ballot_sync(LB_FULL, e.x != NODE_NONE));
-        if (n < 32) { node_insert_no_split(p, c, nd, after, child, vis, kids_are_leaves); return; }
-        if (sm->n_nodes >= sm->node_cap) { seq_fail(c, LB_ERR(DOC_ERR_CAPACITY)); return; }
+        if (n < 32) { node_insert_no_split(p, sm, nd, after, child, vis, kids_are_leaves); return; }
+        if (sm->n_nodes >= sm->node_cap) { seq_fail(sm, LB_ERR(DOC_ERR_CAPACITY)); return; }
         __syncwarp();
         u32 nn = sm->n_nodes;
         __syncwarp();
@@ -173,29 +175,29 @@ __device__ __noinline__ void node_insert(const SeqPools& p, Cx c, u32 nd, int af
         u32 uc = __shfl_down_sync(LB_FULL, e.x, 16);
         u32 uv = __shfl_down_sync(LB_FULL, e.y, 16);
         if (lane < 16) {
-            nd_set(p, c, nn, lane, uc, (i32)uv);
-            set_child_link(p, c, kids_are_leaves, uc, (nn << 5) | (u32)lane);
+            nd_set(p, sm, nn, lane, uc, (i32)uv);
+            set_child_link(p, sm, kids_are_leaves, uc, (nn << 5) | (u32)lane);
         } else {
-            nd_set(p, c, nn, lane, NODE_NONE, 0);
-            nd_set(p, c, nd, lane, NODE_NONE, 0);
+            nd_set(p, sm, nn, lane, NODE_NONE, 0);
+            nd_set(p, sm, nd, lane, NODE_NONE, 0);
         }
         __syncwarp();
-        if (after >= 16) node_insert_no_split(p, c, nn, after - 16, child, vis, kids_are_leaves);
-        else node_insert_no_split(p, c, nd, after, child, vis, kids_are_leaves);
-        i32 tot_old = node_total(p, c, nd), tot_new = node_total(p, c, nn);
-        u32 plink = nd_parent(p, c, nd);
+        if (after >= 16) node_insert_no_split(p, sm, nn, after - 16, child, vis, kids_are_leaves);
+        else node_insert_no_split(p, sm, nd, after, child, vis, kids_are_leaves);
+        i32 tot_old = node_total(p, sm, nd), tot_new = node_total(p, sm, nn);
+        u32 plink = nd_parent(p, sm, nd);
         __syncwarp();   // every lane has read the parent link before it is rewritten
         if (plink == NODE_NONE) {
-            if (sm->n_nodes >= sm->node_cap) { seq_fail(c, LB_ERR(DOC_ERR_CAPACITY)); return; }
+            if (sm->n_nodes >= sm->node_cap) { seq_fail(sm, LB_ERR(DOC_ERR_CAPACITY)); return; }
             __syncwarp();
             u32 nr = sm->n_nodes;
             u32 h = sm->height;
             __syncwarp();
-            nd_set(p, c, nr, lane, lane == 0 ? nd : (lane == 1 ? nn : NODE_NONE), lane == 0 ? tot_old : (lane == 1 ? tot_new : 0));
+            nd_set(p, sm, nr, lane, lane == 0 ? nd : (lane == 1 ? nn : NODE_NONE), lane == 0 ? tot_old : (lane == 1 ? tot_new : 0));
             if (lane == 0) {
-                nd_set_parent(p, c, nr, NODE_NONE);
-                nd_set_parent(p, c, nd, (nr << 5) | 0u);
-                nd_set_parent(p, c, nn, (nr << 5) | 1u);
+                nd_set_parent(p, sm, nr, NODE_NONE);
+                nd_set_parent(p, sm, nd, (nr << 5) | 0u);
+                nd_set_parent(p, sm, nn, (nr << 5) | 1u);
                 sm->n_nodes = nr + 1;
                 sm->root = nr;
                 sm->height = h + 1;
@@ -205,7 +207,7 @@ __device__ __noinline__ void node_insert(const SeqPools& p, Cx c, u32 nd, int af
         }
         u32 parent = plink >> 5;
         int idx = (int)(plink & 31);
-        if (lane == 0) nd_set(p, c, parent, idx, nd, tot_old);
+        if (lane == 0) nd_set(p, sm, parent, idx, nd, tot_old);
         __syncwarp();
         child = nn;
         vis = tot_new;
@@ -216,15 +218,15 @@ __device__ __noinline__ void node_insert(const SeqPools& p, Cx c, u32 nd, int af
 }
 
 // ---- split a full leaf: upper 16 slots move to a new leaf (their atom -> leaf entries follow)
-__device__ __noinline__ void leaf_split(const SeqPools& p, Cx c, u32 leaf) {
-    SeqSmem* sm = c.sm;
-    int lane = c.lane;
-    if (sm->n_leaves >= sm->leaf_cap) { seq_fail(c, LB_ERR(DOC_ERR_CAPACITY)); return; }
+__device__ __noinline__ void leaf_split(const SeqPools& p, u32 leaf) {
+    SeqSmem* sm = seq_sm();
+    int lane = seq_lane();
+    if (sm->n_leaves >= sm->leaf_cap) { seq_fail(sm, LB_ERR(DOC_ERR_CAPACITY)); return; }
     __syncwarp();
     u32 nl = sm->n_leaves;
     __syncwarp();
     if (lane == 0) sm->n_leaves = nl + 1;
-    uint4 L = leaf_load(p, c, leaf);
+    uint4 L = leaf_load(p, sm, leaf);
     u32 link = __shfl_sync(LB_FULL, L.w, 0);
     u32 next = __shfl_sync(LB_FULL, L.w, 1);
     uint4 U;
@@ -234,15 +236,15 @@ __device__ __noinline__ void leaf_split(const SeqPools& p, Cx c, u32 leaf) {
     U.w = lane == 1 ? next : 0;   // parent link (slot 0) is set by node_insert below
     if (lane >= 16) { U.x = SLOT_EMPTY; U.y = 0; U.z = 0; }
     __syncwarp();
-    p.leaf[(c.leaf0 + nl) * 32 + lane] = U;
+    p.leaf[(sm->leaf0 + nl) * 32 + lane] = U;
     uint4 O = L;
     if (lane >= 16) { O.x = SLOT_EMPTY; O.y = 0; O.z = 0; }
     if (lane == 1) O.w = nl;
-    p.leaf[(c.leaf0 + leaf) * 32 + lane] = O;
+    p.leaf[(sm->leaf0 + leaf) * 32 + lane] = O;
     // atoms of the moved spans get their new home
     u32 pe = s_peer(L);
     bool moved_real = lane >= 16 && pe != PEER_NONE && pe != PEER_UNKNOWN;
-    if (moved_real) p.atom_leaf[atom_index(c, pe, (i32)L.y)] = nl;
+    if (moved_real) p.atom_leaf[atom_index(sm, pe, (i32)L.y)] = nl;
     unsigned longm = __ballot_sync(LB_FULL, moved_real && (i32)L.z > 1);
     while (longm) {
         int s = __ffs(longm) - 1;
@@ -250,7 +252,7 @@ __device__ __noinline__ void leaf_split(const SeqPools& p, Cx c, u32 leaf) {
         u32 sp = __shfl_sync(LB_FULL, pe, s);
         i32 sc = (i32)__shfl_sync(LB_FULL, L.y, s);
         i32 sl = (i32)__shfl_sync(LB_FULL, L.z, s);
-        u64 a0 = atom_index(c, sp, sc);
+        u64 a0 = atom_index(sm, sp, sc);
         for (i32 i = 1 + lane; i < sl; i += 32) p.atom_leaf[a0 + i] = nl;
     }
     unsigned unk = __ballot_sync(LB_FULL, lane >= 16 && pe == PEER_UNKNOWN);
@@ -258,27 +260,28 @@ __device__ __noinline__ void leaf_split(const SeqPools& p, Cx c, u32 leaf) {
     i32 moved = warp_sum(lane >= 16 ? s_vis(L) : 0);
     u32 parent = link >> 5;
     int idx = (int)(link & 31);
-    if (lane == 0) nd_add_vis(p, c, parent, idx, -moved);
+    if (lane == 0) nd_add_vis(p, sm, parent, idx, -moved);
     __syncwarp();
-    node_insert(p, c, parent, idx, nl, moved, true);
+    node_insert(p, parent, idx, nl, moved, true);
 }
 
 // ---- split the span containing atom (peer, ctr) right before that atom (FugueSpan::_slice,
 // fugue_span.rs:257-279); visible totals unchanged.  No-op when (peer, ctr) already starts a span.
-__device__ __noinline__ void split_before(const SeqPools& p, Cx c, u32 peer, i32 ctr) {
-    int lane = c.lane;
+__device__ __noinline__ void split_before(const SeqPools& p, u32 peer, i32 ctr) {
+    SeqSmem* sm = seq_sm();
+    int lane = seq_lane();
     for (int attempt = 0; attempt < 2; attempt++) {
-        u32 leaf = p.atom_leaf[atom_index(c, peer, ctr)];
-        if (leaf == LEAF_NONE) { seq_fail(c, LB_ERR(DOC_ERR_CORRUPT)); return; }
-        uint4 L = leaf_load(p, c, leaf);
+        u32 leaf = p.atom_leaf[atom_index(sm, peer, ctr)];
+        if (leaf == LEAF_NONE) { seq_fail(sm, LB_ERR(DOC_ERR_CORRUPT)); return; }
+        uint4 L = leaf_load(p, sm, leaf);
         int slot = slot_of(L, peer, ctr);
-        if (slot < 0) { seq_fail(c, LB_ERR(DOC_ERR_CORRUPT)); return; }
+        if (slot < 0) { seq_fail(sm, LB_ERR(DOC_ERR_CORRUPT)); return; }
         i32 s_ctr = (i32)__shfl_sync(LB_FULL, L.y, slot);
         if (s_ctr == ctr) return;
         if (leaf_count(L) >= 32) {   // make room first; the span (still whole) may move to the new leaf
-            if (attempt) { seq_fail(c, LB_ERR(DOC_ERR_CAPACITY)); return; }
-            leaf_split(p, c, leaf);
-            if (c.sm->err) return;
+            if (attempt) { seq_fail(sm, LB_ERR(DOC_ERR_CAPACITY)); return; }
+            leaf_split(p, leaf);
+            if (sm->err) return;
             continue;
         }
         i32 s_len = (i32)__shfl_sync(LB_FULL, L.z, slot);
@@ -290,10 +293,10 @@ __device__ __noinline__ void split_before(const SeqPools& p, Cx c, u32 peer, i32
         if (lane == slot) L.z = (u32)k;                       // left part keeps its slot
         else if (lane == slot + 1) { L.x = s_x; L.y = (u32)ctr; L.z = (u32)(s_len - k); }
         else if (lane > slot + 1) { L.x = ux; L.y = uy; L.z = uz; }
-        leaf_store(p, c, leaf, L, slot);
+        leaf_store(p, sm, leaf, L, slot);
         // origins of the new span start: left origin is its predecessor, right origin is inherited
-        uint4 og = p.a_org[atom_index(c, peer, s_ctr)];
-        if (lane == 0) p.a_org[atom_index(c, peer, ctr)] = mk4(peer | (og.x & 0xFFFF0000u), (u32)(ctr - 1), og.z, 0);
+        uint4 og = p.a_org[atom_index(sm, peer, s_ctr)];
+        if (lane == 0) p.a_org[atom_index(sm, peer, ctr)] = mk4(peer | (og.x & 0xFFFF0000u), (u32)(ctr - 1), og.z, 0);
         __syncwarp();
         return;
     }
@@ -301,20 +304,21 @@ __device__ __noinline__ void split_before(const SeqPools& p, Cx c, u32 peer, i32
 
 // ---- apply a status change to the inserted atoms [t0,t1) of `peer`: set_future 1/0/-1 (set, clear, keep),
 // del_diff added to the delete counter.  `hint` is a (possibly stale) atom -> leaf lookup of (peer, t0).
-__device__ __noinline__ void range_apply(const SeqPools& p, Cx c, u32 peer, i32 t0, i32 t1, int set_future, int del_diff, u32 hint) {
-    int lane = c.lane;
+__device__ __noinline__ void range_apply(const SeqPools& p, u32 peer, i32 t0, i32 t1, int set_future, int del_diff, u32 hint) {
+    SeqSmem* sm = seq_sm();
+    int lane = seq_lane();
     i32 cur = t0;
     u32 leaf = hint;
     int guard = 0;
     while (cur < t1) {
         if (leaf == LEAF_NONE) {
-            leaf = p.atom_leaf[atom_index(c, peer, cur)];
+            leaf = p.atom_leaf[atom_index(sm, peer, cur)];
             if (leaf == LEAF_NONE) { cur++; continue; }   // never integrated here (foreign container)
         }
-        uint4 L = leaf_load(p, c, leaf);
+        uint4 L = leaf_load(p, sm, leaf);
         int slot = slot_of(L, peer, cur);
         if (slot < 0) {            // stale hint (a leaf split moved the span): look the atom up again
-            if (++guard > 2) { seq_fail(c, LB_ERR(DOC_ERR_CORRUPT)); return; }
+            if (++guard > 2) { seq_fail(sm, LB_ERR(DOC_ERR_CORRUPT)); return; }
             leaf = LEAF_NONE;
             continue;
         }
@@ -322,9 +326,9 @@ __device__ __noinline__ void range_apply(const SeqPools& p, Cx c, u32 peer, i32 
         i32 s_len = (i32)__shfl_sync(LB_FULL, L.z, slot);
         if (s_ctr != cur || cur + s_len > t1) {
             // boundaries do not line up with the span: cut it, then look again
-            if (s_ctr != cur) split_before(p, c, peer, cur);
-            if (!c.sm->err && s_ctr + s_len > t1) split_before(p, c, peer, t1);
-            if (c.sm->err) return;
+            if (s_ctr != cur) split_before(p, peer, cur);
+            if (!sm->err && s_ctr + s_len > t1) split_before(p, peer, t1);
+            if (sm->err) return;
             leaf = LEAF_NONE;
             guard = 0;
             continue;
@@ -345,10 +349,10 @@ __device__ __noinline__ void range_apply(const SeqPools& p, Cx c, u32 peer, i32 
             if (set_future == 0) st &= ~ST_FUTURE;
             st = (st & ST_FUTURE) | (((st & 0x7FFFu) + (u32)del_diff) & 0x7FFFu);
             L.x = (L.x & 0xFFFFu) | (st << 16);
-            p.leaf[(c.leaf0 + leaf) * 32 + lane].x = L.x;
+            p.leaf[(sm->leaf0 + leaf) * 32 + lane].x = L.x;
         }
         i32 delta = warp_sum((mine ? s_vis(L) : 0) - before);
-        add_vis(p, c, __shfl_sync(LB_FULL, L.w, 0), delta);
+        add_vis(p, sm, __shfl_sync(LB_FULL, L.w, 0), delta);
         leaf = LEAF_NONE;
         guard = 0;
     }
@@ -359,16 +363,16 @@ __device__ __noinline__ void range_apply(const SeqPools& p, Cx c, u32 peer, i32 
 // overlap.  Handles the spans that line up with the range; returns the first counter that needs the
 // warp-cooperative path (a span must be cut, or the atom is unknown here), t1 when done.  No structure
 // changes happen while lanes run this, so the hints taken at the start of the batch stay valid.
-__device__ __forceinline__ i32 toggle_lane(const SeqPools& p, const Cx& c, u32 peer, i32 t0, i32 t1, int set_future, int del_diff,
+__device__ __forceinline__ i32 toggle_lane(const SeqPools& p, SeqSmem* sm, u32 peer, i32 t0, i32 t1, int set_future, int del_diff,
                                            u32 hint) {
     i32 cur = t0;
     u32 leaf = hint;
     while (cur < t1) {
         if (leaf == LEAF_NONE) {
-            leaf = p.atom_leaf[atom_index(c, peer, cur)];
+            leaf = p.atom_leaf[atom_index(sm, peer, cur)];
             if (leaf == LEAF_NONE) return cur;
         }
-        uint4* base = p.leaf + (c.leaf0 + leaf) * 32;
+        uint4* base = p.leaf + (sm->leaf0 + leaf) * 32;
         int found = -1;
         uint4 sl = mk4(0, 0, 0, 0);
         u32 link = NODE_NONE;
@@ -395,9 +399,9 @@ __device__ __forceinline__ i32 toggle_lane(const SeqPools& p, const Cx& c, u32 p
             while (link != NODE_NONE) {
                 u32 nd = link >> 5;
                 int idx = (int)(link & 31);
-                if (nd < LB_SEQ_NS) atomicAdd(&c.sm->vis[nd][idx], delta);
-                else atomicAdd((i32*)&p.node[(c.node0 + nd) * 32 + idx].y, delta);
-                link = nd_parent(p, c, nd);
+                if (nd < LB_SEQ_NS) atomicAdd(&sm->vis[nd][idx], delta);
+                else atomicAdd((i32*)&p.node[(sm->node0 + nd) * 32 + idx].y, delta);
+                link = nd_parent(p, sm, nd);
             }
         }
         cur += len;
@@ -409,11 +413,12 @@ __device__ __forceinline__ i32 toggle_lane(const SeqPools& p, const Cx& c, u32 p
 // ---- retreat (dir=-1) / forward (dir=+1) the ops of peer `q` with counters [a,b) that touch container `cidx`.
 // The peer's changes covering [a,b) are enumerated 32 at a time, their op rows flattened over the lanes, so the
 // op records and the atom -> leaf lookups of 32 rows cost one round trip each.
-__device__ __noinline__ void toggle_ops(const SeqPools& p, const BatchTables& t, Cx c, u64 ch0, u32 cidx, u32 q, i32 a, i32 b, int dir) {
-    int lane = c.lane;
-    u32 row_a = t.atom_row[atom_index(c, q, a)], row_b = t.atom_row[atom_index(c, q, b - 1)];
+__device__ __noinline__ void toggle_ops(const SeqPools& p, const BatchTables& t, u64 ch0, u32 cidx, u32 q, i32 a, i32 b, int dir) {
+    SeqSmem* sm = seq_sm();
+    int lane = seq_lane();
+    u32 row_a = t.atom_row[atom_index(sm, q, a)], row_b = t.atom_row[atom_index(sm, q, b - 1)];
     u32 pos_a = t.ch_pos[t.op_change[row_a]], pos_b = t.ch_pos[t.op_change[row_b]];
-    for (u32 pb = pos_a; pb <= pos_b && !c.sm->err; pb += 32) {
+    for (u32 pb = pos_a; pb <= pos_b && !sm->err; pb += 32) {
         u32 pos = pb + (u32)lane;
         bool cv = pos <= pos_b;
         u32 ch = cv ? t.ch_aorder[ch0 + pos] : 0;
@@ -422,7 +427,7 @@ __device__ __noinline__ void toggle_ops(const SeqPools& p, const BatchTables& t,
         i32 incl = warp_incl_scan(nr, lane);
         i32 total = __shfl_sync(LB_FULL, incl, 31);
         i32 excl = incl - nr;
-        for (i32 g0 = 0; g0 < total && !c.sm->err; g0 += 32) {
+        for (i32 g0 = 0; g0 < total && !sm->err; g0 += 32) {
             i32 g = g0 + lane;
             bool gv = g < total;
             int j = 0;   // change of flat row g: number of lanes whose inclusive count is <= g
@@ -454,16 +459,16 @@ __device__ __noinline__ void toggle_ops(const SeqPools& p, const BatchTables& t,
                 mode = -1;
                 dd = dir;
             }
-            u32 hint = act ? p.atom_leaf[atom_index(c, tp, t0)] : LEAF_NONE;
+            u32 hint = act ? p.atom_leaf[atom_index(sm, tp, t0)] : LEAF_NONE;
             // lane-parallel: each lane flips the spans of its own row; what needs a cut comes back for the warp
             i32 done = t1;
-            if (act) done = toggle_lane(p, c, tp, t0, t1, mode, dd, hint);
+            if (act) done = toggle_lane(p, sm, tp, t0, t1, mode, dd, hint);
             __syncwarp();
             unsigned m = __ballot_sync(LB_FULL, act && done < t1);
-            while (m && !c.sm->err) {
+            while (m && !sm->err) {
                 int s = __ffs(m) - 1;
                 m &= m - 1;
-                range_apply(p, c, __shfl_sync(LB_FULL, tp, s), __shfl_sync(LB_FULL, done, s), __shfl_sync(LB_FULL, t1, s),
+                range_apply(p, __shfl_sync(LB_FULL, tp, s), __shfl_sync(LB_FULL, done, s), __shfl_sync(LB_FULL, t1, s),
                             __shfl_sync(LB_FULL, mode, s), __shfl_sync(LB_FULL, dd, s), LEAF_NONE);
             }
         }
@@ -471,64 +476,64 @@ __device__ __noinline__ void toggle_ops(const SeqPools& p, const BatchTables& t,
 }
 
 // ---- move the tracker of the active container to version vv (+ the author's own counter)
-__device__ __forceinline__ void checkout(const SeqPools& p, const BatchTables& t, const Cx& c, u64 ch0, u32 cidx, const i32* vv,
+__device__ __forceinline__ void checkout(const SeqPools& p, const BatchTables& t, SeqSmem* sm, u64 ch0, u32 cidx, const i32* vv,
                                          u32 own_peer, i32 own_ctr) {
-    int lane = c.lane;
-    for (u32 q0 = 0; q0 < c.P && !c.sm->err; q0 += 32) {
+    int lane = seq_lane();
+    for (u32 q0 = 0; q0 < sm->P && !sm->err; q0 += 32) {
         u32 q = q0 + (u32)lane;
         i32 tgt = 0, cur = 0;
-        if (q < c.P) {
+        if (q < sm->P) {
             tgt = vv ? vv[q] : 0;
             if (q == own_peer && own_ctr > tgt) tgt = own_ctr;
-            cur = cvv_get(p, c, q);
+            cur = cvv_get(p, sm, q);
         }
         unsigned m = __ballot_sync(LB_FULL, cur != tgt);
-        while (m && !c.sm->err) {
+        while (m && !sm->err) {
             int s = __ffs(m) - 1;
             m &= m - 1;
             i32 cu = __shfl_sync(LB_FULL, cur, s), tg = __shfl_sync(LB_FULL, tgt, s);
-            if (cu > tg) toggle_ops(p, t, c, ch0, cidx, q0 + (u32)s, tg, cu, -1);
-            else toggle_ops(p, t, c, ch0, cidx, q0 + (u32)s, cu, tg, +1);
+            if (cu > tg) toggle_ops(p, t, ch0, cidx, q0 + (u32)s, tg, cu, -1);
+            else toggle_ops(p, t, ch0, cidx, q0 + (u32)s, cu, tg, +1);
         }
         __syncwarp();
-        if (q < c.P && cur != tgt) cvv_set(p, c, q, tgt);
+        if (q < sm->P && cur != tgt) cvv_set(p, sm, q, tgt);
         __syncwarp();
     }
 }
 
 // ---- position key of slot (leaf, slot) for cmp_pos (crdt_rope.rs:433-446)
-__device__ __forceinline__ u64 order_key(const SeqPools& p, const Cx& c, u32 leaf, int slot) {
+__device__ __forceinline__ u64 order_key(const SeqPools& p, SeqSmem* sm, u32 leaf, int slot) {
     u64 key = (u64)slot;
     int shift = 6;
-    u32 link = p.leaf[(c.leaf0 + leaf) * 32].w;
+    u32 link = p.leaf[(sm->leaf0 + leaf) * 32].w;
     while (link != NODE_NONE) {
         key |= (u64)(link & 31) << shift;
         shift += 6;
-        link = nd_parent(p, c, link >> 5);
+        link = nd_parent(p, sm, link >> 5);
     }
     return key;
 }
-__device__ __forceinline__ u64 order_key_of_atom(const SeqPools& p, const Cx& c, u32 peer, i32 ctr) {
+__device__ __forceinline__ u64 order_key_of_atom(const SeqPools& p, SeqSmem* sm, u32 peer, i32 ctr) {
     u32 leaf;
     uint4 L;
     int slot;
     if (peer == PEER_UNKNOWN) {
-        leaf = c.sm->unk_leaf;
-        L = leaf_load(p, c, leaf);
+        leaf = sm->unk_leaf;
+        L = leaf_load(p, sm, leaf);
         slot = __ffs(__ballot_sync(LB_FULL, s_peer(L) == PEER_UNKNOWN)) - 1;
     } else {
-        leaf = p.atom_leaf[atom_index(c, peer, ctr)];
-        L = leaf_load(p, c, leaf);
+        leaf = p.atom_leaf[atom_index(sm, peer, ctr)];
+        L = leaf_load(p, sm, leaf);
         slot = slot_of(L, peer, ctr);
     }
-    return order_key(p, c, leaf, slot);
+    return order_key(p, sm, leaf, slot);
 }
 // origin_left of atom (peer, ctr): stored for span starts, implied inside a span
-__device__ __forceinline__ void atom_origin_left(const SeqPools& p, const Cx& c, u32 peer, i32 ctr, u32* op, i32* oc) {
+__device__ __forceinline__ void atom_origin_left(const SeqPools& p, SeqSmem* sm, u32 peer, i32 ctr, u32* op, i32* oc) {
     if (peer == PEER_UNKNOWN) { *op = PEER_NONE; *oc = -1; return; }
-    u64 ai = atom_index(c, peer, ctr);
+    u64 ai = atom_index(sm, peer, ctr);
     u32 leaf = p.atom_leaf[ai];
-    uint4 L = leaf_load(p, c, leaf);
+    uint4 L = leaf_load(p, sm, leaf);
     int slot = slot_of(L, peer, ctr);
     i32 s_ctr = (i32)__shfl_sync(LB_FULL, L.y, slot < 0 ? 0 : slot);
     if (slot >= 0 && s_ctr == ctr) { uint4 og = p.a_org[ai]; *op = og.x & 0xFFFFu; *oc = (i32)og.y; }
@@ -544,7 +549,8 @@ struct SibIn {
     u64 my_peer_id;
 };
 struct SibOut { bool after_valid; u32 after_peer; i32 after_ctr; };
-__device__ __noinline__ SibOut sibling_scan(const SeqPools& p, Cx c, SibIn in) {
+__device__ __noinline__ SibOut sibling_scan(const SeqPools& p, SibIn in) {
+    SeqSmem* sm = seq_sm();
     SibOut out;
     out.after_valid = false;
     out.after_peer = 0;
@@ -558,9 +564,9 @@ __device__ __noinline__ SibOut sibling_scan(const SeqPools& p, Cx c, SibIn in) {
         u32 e_olp;
         i32 e_olc;
         if (or_peer == PEER_UNKNOWN) { e_olp = PEER_NONE; e_olc = -1; }
-        else { uint4 og = p.a_org[atom_index(c, or_peer, or_ctr)]; e_olp = og.x & 0xFFFFu; e_olc = (i32)og.y; }
+        else { uint4 og = p.a_org[atom_index(sm, or_peer, or_ctr)]; e_olp = og.x & 0xFFFFu; e_olc = (i32)og.y; }
         pr_valid = e_olp == ol_peer && (ol_peer == PEER_NONE || e_olc == ol_ctr);
-        if (pr_valid) pr_key = order_key(p, c, in.pr_leaf, in.pr_slot);
+        if (pr_valid) pr_key = order_key(p, sm, in.pr_leaf, in.pr_slot);
     }
     bool scanning = false;
     u64 first_key = 0;
@@ -570,31 +576,31 @@ __device__ __noinline__ SibOut sibling_scan(const SeqPools& p, Cx c, SibIn in) {
     u32 seen = 0;
     bool stop = false;
     while (l2 != LEAF_NONE && seen < in.n_between && !stop) {
-        uint4 S = leaf_load(p, c, l2);
+        uint4 S = leaf_load(p, sm, l2);
         int n = leaf_count(S);
         u32 next = __shfl_sync(LB_FULL, S.w, 1);
         for (int s = from; s < n && seen < in.n_between && !stop; s++) {
             u32 o_peer = __shfl_sync(LB_FULL, S.x, s) & 0xFFFFu;
             i32 o_ctr = (i32)__shfl_sync(LB_FULL, S.y, s);
             seen++;
-            u64 o_key = order_key(p, c, l2, s);
+            u64 o_key = order_key(p, sm, l2, s);
             if (!have_first) { first_key = o_key; have_first = true; }
-            uint4 oo = p.a_org[atom_index(c, o_peer, o_ctr)];
+            uint4 oo = p.a_org[atom_index(sm, o_peer, o_ctr)];
             u32 o_olp = oo.x & 0xFFFFu, o_orp = oo.x >> 16;
             i32 o_olc = (i32)oo.y, o_orc = (i32)oo.z;
             bool same_ol = o_olp == ol_peer && (ol_peer == PEER_NONE || o_olc == ol_ctr);
             if (!same_ol) {
                 // "visited" is a prefix of the in-between spans: membership is a position test
                 bool in_visited = false;
-                if (o_olp != PEER_NONE && o_olp != PEER_UNKNOWN && p.atom_leaf[atom_index(c, o_olp, o_olc)] != LEAF_NONE) {
-                    u64 lk = order_key_of_atom(p, c, o_olp, o_olc);
+                if (o_olp != PEER_NONE && o_olp != PEER_UNKNOWN && p.atom_leaf[atom_index(sm, o_olp, o_olc)] != LEAF_NONE) {
+                    u64 lk = order_key_of_atom(p, sm, o_olp, o_olc);
                     in_visited = lk >= first_key && lk < o_key;
                 }
                 if (!in_visited) { stop = true; break; }
             }
             if (same_ol) {
                 bool same_or = o_orp == or_peer && (or_peer == PEER_NONE || o_orc == or_ctr);
-                u64 o_peer_id = c.dpeer[o_peer].id;
+                u64 o_peer_id = sm->dpeer[o_peer].id;
                 if (same_or) {
                     if (o_peer_id > in.my_peer_id) { stop = true; break; }
                     scanning = false;
@@ -604,10 +610,10 @@ __device__ __noinline__ SibOut sibling_scan(const SeqPools& p, Cx c, SibIn in) {
                     if (o_orp != PEER_NONE) {
                         u32 e_olp;
                         i32 e_olc;
-                        atom_origin_left(p, c, o_orp, o_orc, &e_olp, &e_olc);
+                        atom_origin_left(p, sm, o_orp, o_orc, &e_olp, &e_olc);
                         if (e_olp == ol_peer && (ol_peer == PEER_NONE || e_olc == ol_ctr)) {
                             o_pr = true;
-                            o_pr_key = order_key_of_atom(p, c, o_orp, o_orc);
+                            o_pr_key = order_key_of_atom(p, sm, o_orp, o_orc);
                         }
                     }
                     int cmp;
@@ -629,9 +635,8 @@ __device__ __noinline__ SibOut sibling_scan(const SeqPools& p, Cx c, SibIn in) {
 }
 
 // ---- CrdtRope::insert (crdt_rope.rs:43-227)
-__device__ __forceinline__ void seq_insert(const SeqPools& p, const Cx& c, u32 peer, i32 ctr, i32 len, i32 pos) {
-    SeqSmem* sm = c.sm;
-    int lane = c.lane;
+__device__ __forceinline__ void seq_insert(const SeqPools& p, SeqSmem* sm, u32 peer, i32 ctr, i32 len, i32 pos) {
+    int lane = seq_lane();
     for (int attempt = 0; attempt < 4; attempt++) {
         // 1. cursor: right after the pos-th visible atom (prefer-left)
         u32 leaf = sm->first_leaf;
@@ -642,12 +647,12 @@ __device__ __forceinline__ void seq_insert(const SeqPools& p, const Cx& c, u32 p
             u32 nd = sm->root;
             u32 height = sm->height;
             for (u32 lvl = height; lvl >= 1; lvl--) {
-                uint2 e = nd_get(p, c, nd, lane);
+                uint2 e = nd_get(p, sm, nd, lane);
                 i32 v = (i32)e.y;
                 i32 incl = warp_incl_scan(v, lane);
                 unsigned m = __ballot_sync(LB_FULL, e.x != NODE_NONE && incl >= rem);
                 int idx = __ffs(m) - 1;
-                if (idx < 0) { seq_fail(c, LB_ERR(DOC_ERR_CORRUPT)); return; }
+                if (idx < 0) { seq_fail(sm, LB_ERR(DOC_ERR_CORRUPT)); return; }
                 if ((u32)lane == lvl) my_link = (nd << 5) | (u32)idx;
                 rem -= __shfl_sync(LB_FULL, incl - v, idx);
                 nd = __shfl_sync(LB_FULL, e.x, idx);
@@ -655,7 +660,7 @@ __device__ __forceinline__ void seq_insert(const SeqPools& p, const Cx& c, u32 p
             leaf = nd;
             have_path = height < 32;
         }
-        uint4 L = leaf_load(p, c, leaf);
+        uint4 L = leaf_load(p, sm, leaf);
         int n = leaf_count(L);
         int slot = 0;
         i32 off = 0;
@@ -668,12 +673,12 @@ __device__ __forceinline__ void seq_insert(const SeqPools& p, const Cx& c, u32 p
             i32 incl = warp_incl_scan(v, lane);
             unsigned m = __ballot_sync(LB_FULL, incl >= rem && v > 0);
             slot = __ffs(m) - 1;
-            if (slot < 0) { seq_fail(c, LB_ERR(DOC_ERR_CORRUPT)); return; }
+            if (slot < 0) { seq_fail(sm, LB_ERR(DOC_ERR_CORRUPT)); return; }
             off = rem - __shfl_sync(LB_FULL, incl - v, slot);
             cur_x = __shfl_sync(LB_FULL, L.x, slot);
             cur_ctr = (i32)__shfl_sync(LB_FULL, L.y, slot);
             cur_len = (i32)__shfl_sync(LB_FULL, L.z, slot);
-            if ((cur_x & 0xFFFFu) == PEER_UNKNOWN) { seq_fail(c, LB_ERR(DOC_ERR_CORRUPT)); return; }  // beyond the content
+            if ((cur_x & 0xFFFFu) == PEER_UNKNOWN) { seq_fail(sm, LB_ERR(DOC_ERR_CORRUPT)); return; }  // beyond the content
             ol_peer = cur_x & 0xFFFFu;
             ol_ctr = cur_ctr + off - 1;
         }
@@ -712,7 +717,7 @@ __device__ __forceinline__ void seq_insert(const SeqPools& p, const Cx& c, u32 p
                 l2 = __shfl_sync(LB_FULL, S.w, 1);
                 if (l2 == LEAF_NONE) break;
                 from = 0;
-                S = leaf_load(p, c, l2);
+                S = leaf_load(p, sm, l2);
             }
         }
         // 3. where to put it
@@ -723,25 +728,25 @@ __device__ __forceinline__ void seq_insert(const SeqPools& p, const Cx& c, u32 p
             in.leaf = leaf; in.from = scan_from; in.n_between = n_between;
             in.ol_peer = ol_peer; in.ol_ctr = ol_ctr; in.or_peer = or_peer; in.or_ctr = or_ctr;
             in.pr_valid = pr_valid; in.pr_leaf = pr_leaf; in.pr_slot = pr_slot;
-            in.my_peer_id = c.dpeer[peer].id;
-            SibOut so = sibling_scan(p, c, in);
+            in.my_peer_id = sm->dpeer[peer].id;
+            SibOut so = sibling_scan(p, in);
             if (so.after_valid) {
-                tgt_leaf = p.atom_leaf[atom_index(c, so.after_peer, so.after_ctr)];
-                if (tgt_leaf != leaf) { L = leaf_load(p, c, tgt_leaf); n = leaf_count(L); }
+                tgt_leaf = p.atom_leaf[atom_index(sm, so.after_peer, so.after_ctr)];
+                if (tgt_leaf != leaf) { L = leaf_load(p, sm, tgt_leaf); n = leaf_count(L); }
                 at = slot_of(L, so.after_peer, so.after_ctr) + 1;
-                if (at <= 0) { seq_fail(c, LB_ERR(DOC_ERR_CORRUPT)); return; }
+                if (at <= 0) { seq_fail(sm, LB_ERR(DOC_ERR_CORRUPT)); return; }
                 mid = false;
             }
         }
         // 4. physical insertion into the loaded image: one new slot, two when the cursor span is cut
         int need = mid ? 2 : 1;
         if (n + need > 32) {
-            leaf_split(p, c, tgt_leaf);
+            leaf_split(p, tgt_leaf);
             if (sm->err) return;
             continue;   // positions moved: locate the cursor again
         }
         uint4 og = mk4(0, 0, 0, 0);
-        if (mid) og = p.a_org[atom_index(c, cur_peer, cur_ctr)];   // right origin inherited by the cut-off tail
+        if (mid) og = p.a_org[atom_index(sm, cur_peer, cur_ctr)];   // right origin inherited by the cut-off tail
         u32 link = __shfl_sync(LB_FULL, L.w, 0);
         u32 ux = __shfl_up_sync(LB_FULL, L.x, need);
         u32 uy = __shfl_up_sync(LB_FULL, L.y, need);
@@ -752,83 +757,35 @@ __device__ __forceinline__ void seq_insert(const SeqPools& p, const Cx& c, u32 p
             if (lane == at - 1) L.z = (u32)off;
             if (lane == at + 1) { L.x = cur_x; L.y = (u32)(cur_ctr + off); L.z = (u32)(cur_len - off); }
         }
-        leaf_store(p, c, tgt_leaf, L, at > 0 ? at - 1 : 0);
-        u64 a0 = atom_index(c, peer, ctr);
+        leaf_store(p, sm, tgt_leaf, L, at > 0 ? at - 1 : 0);
+        u64 a0 = atom_index(sm, peer, ctr);
         if (lane == 0) p.a_org[a0] = mk4(ol_peer | (or_peer << 16), (u32)ol_ctr, (u32)or_ctr, 0);
         if (mid && lane == 1)
-            p.a_org[atom_index(c, cur_peer, cur_ctr + off)] = mk4(cur_peer | (og.x & 0xFFFF0000u), (u32)(cur_ctr + off - 1), og.z, 0);
+            p.a_org[atom_index(sm, cur_peer, cur_ctr + off)] = mk4(cur_peer | (og.x & 0xFFFF0000u), (u32)(cur_ctr + off - 1), og.z, 0);
         if (lane < len) p.atom_leaf[a0 + lane] = tgt_leaf;
         for (i32 i = 32 + lane; i < len; i += 32) p.atom_leaf[a0 + i] = tgt_leaf;
         if (have_path && tgt_leaf == leaf) {   // every level of the recorded path at once
-            if (my_link != NODE_NONE) nd_add_vis(p, c, my_link >> 5, (int)(my_link & 31), len);
+            if (my_link != NODE_NONE) nd_add_vis(p, sm, my_link >> 5, (int)(my_link & 31), len);
             __syncwarp();
-        } else add_vis(p, c, link, len);
+        } else add_vis(p, sm, link, len);
         return;
     }
-    seq_fail(c, LB_ERR(DOC_ERR_CAPACITY));
-}
-
-// ---- leaf prefetch (NOT enabled).  The kernel is bound by the latency of the leaf round trip of every op (one
-// dependent 512-byte HBM read per op).  With LB_SEQ_PF, when 32 op records arrive, every lane
-// predicts the leaf ITS record will touch -- deletes from the atom -> leaf lookup they do anyway, inserts by walking the
-// shared-memory nodes on its own (lane-serial, the warp runs 32 descents at once) -- and asks L2 (or L1) for it.
-// The predicted descents add issue slots to every op.  On an H100, C3, prefetching delete targets only (=1) measured
-// about 0.2 % faster than off and inserts too (=2) about 6 % slower (DESIGN.md section 3); whether to turn =1 on is
-// left to an optimisation change.
-#ifndef LB_SEQ_PF
-#define LB_SEQ_PF 0           // 0: off, 1: delete targets only, 2: inserts too
-#endif
-__device__ __forceinline__ void prefetch_leaf(const SeqPools& p, const Cx& c, u32 leaf) {
-#ifndef LB_SIMT_EMU
-    const char* a = (const char*)(p.leaf + (c.leaf0 + leaf) * 32);
-#ifdef LB_SEQ_PF_L1
-    asm volatile("prefetch.global.L1 [%0];" ::"l"(a));
-    asm volatile("prefetch.global.L1 [%0];" ::"l"(a + 128));
-    asm volatile("prefetch.global.L1 [%0];" ::"l"(a + 256));
-    asm volatile("prefetch.global.L1 [%0];" ::"l"(a + 384));
-#else
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(a));
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(a + 128));
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(a + 256));
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(a + 384));
-#endif
-#else
-    (void)p; (void)c; (void)leaf;
-#endif
-}
-__device__ __forceinline__ u32 predict_leaf(const Cx& c, i32 pos) {
-    const SeqSmem* sm = c.sm;
-    if (pos <= 0) return sm->first_leaf;
-    u32 nd = sm->root;
-    i32 rem = pos;
-    for (u32 lvl = sm->height; lvl >= 1; lvl--) {
-        if (nd >= LB_SEQ_NS) return LEAF_NONE;       // this node lives in HBM: no prediction
-        int i = 0;
-        for (; i < 32; i++) {
-            if (sm->child[nd][i] == NODE_NONE) return LEAF_NONE;
-            i32 v = sm->vis[nd][i];
-            if (v >= rem) break;
-            rem -= v;
-        }
-        if (i == 32) return LEAF_NONE;
-        nd = sm->child[nd][i];
-    }
-    return nd;
+    seq_fail(sm, LB_ERR(DOC_ERR_CAPACITY));
 }
 
 // ---- container switching: internal nodes < NS and the tracker version live in shared memory while a
 // container is active
-__device__ __noinline__ void store_container(const SeqPools& p, const BatchTables& t, Cx c, u64 cid0, u32 cidx) {
+__device__ __noinline__ void store_container(const SeqPools& p, const BatchTables& t, u64 cid0, u32 cidx) {
     if (cidx == 0xFFFFFFFFu) return;
-    SeqSmem* sm = c.sm;
-    int lane = c.lane;
+    SeqSmem* sm = seq_sm();
+    int lane = seq_lane();
     __syncwarp();
     u32 cached = sm->n_nodes < LB_SEQ_NS ? sm->n_nodes : LB_SEQ_NS;
     for (u32 nd = 0; nd < cached; nd++) {
-        p.node[(c.node0 + nd) * 32 + lane] = mk2(sm->child[nd][lane], (u32)sm->vis[nd][lane]);
-        if (lane == 0) p.node_parent[c.node0 + nd] = sm->parent[nd];
+        p.node[(sm->node0 + nd) * 32 + lane] = mk2(sm->child[nd][lane], (u32)sm->vis[nd][lane]);
+        if (lane == 0) p.node_parent[sm->node0 + nd] = sm->parent[nd];
     }
-    if ((u32)lane < c.P) p.cvv[c.cvv0 + lane] = sm->cvv[lane];
+    if ((u32)lane < sm->P) p.cvv[sm->cvv0 + lane] = sm->cvv[lane];
 #ifdef LB_SIMT_EMU
     if (lane == 0 && getenv("LB_EMU_STATS")) fprintf(stderr, "container %u: leaves %u nodes %u height %u root %u\n", cidx, sm->n_leaves, sm->n_nodes, sm->height, sm->root);
 #endif
@@ -843,18 +800,18 @@ __device__ __noinline__ void store_container(const SeqPools& p, const BatchTable
     }
     __syncwarp();
 }
-// returns the container's Cx (pool bases); Tracker::new_with_unknown (tracker.rs:38-63) on first use: one
-// placeholder span of length u32::MAX/4
-__device__ __noinline__ Cx load_container(const SeqPools& p, const BatchTables& t, Cx c, u64 cid0, u32 cidx) {
-    SeqSmem* sm = c.sm;
-    int lane = c.lane;
+// Tracker::new_with_unknown (tracker.rs:38-63) on first use: one placeholder span of length u32::MAX/4
+__device__ __noinline__ void load_container(const SeqPools& p, const BatchTables& t, u64 cid0, u32 cidx) {
+    SeqSmem* sm = seq_sm();
+    int lane = seq_lane();
     const DocContainer& dc = t.dcont[cid0 + cidx];
-    c.leaf0 = dc.leaf0;
-    c.node0 = dc.node0;
-    c.cvv0 = dc.cvv0;
+    const u64 leaf0 = dc.leaf0, node0 = dc.node0, cvv0 = dc.cvv0;
     u32 n_leaves = dc.n_leaves, n_nodes = dc.n_nodes;
     __syncwarp();
     if (lane == 0) {
+        sm->leaf0 = leaf0;
+        sm->node0 = node0;
+        sm->cvv0 = cvv0;
         sm->leaf_cap = dc.leaf_cap;
         sm->node_cap = dc.node_cap;
         sm->n_leaves = n_leaves;
@@ -865,7 +822,7 @@ __device__ __noinline__ Cx load_container(const SeqPools& p, const BatchTables& 
         sm->unk_leaf = dc.unk_sid;
     }
     if (n_leaves == 0) {
-        if (dc.leaf_cap < 1 || dc.node_cap < 1) { seq_fail(c, LB_ERR(DOC_ERR_CAPACITY)); return c; }
+        if (dc.leaf_cap < 1 || dc.node_cap < 1) { seq_fail(sm, LB_ERR(DOC_ERR_CAPACITY)); return; }
         if (lane == 0) {
             sm->n_leaves = 1;
             sm->n_nodes = 1;
@@ -875,45 +832,45 @@ __device__ __noinline__ Cx load_container(const SeqPools& p, const BatchTables& 
             sm->unk_leaf = 0;
         }
         // leaf 0: the placeholder span; parent link (node 0, index 0) in slot 0, no next leaf in slot 1
-        p.leaf[c.leaf0 * 32 + lane] = mk4(lane == 0 ? (u32)PEER_UNKNOWN : SLOT_EMPTY, 0, lane == 0 ? (u32)UNKNOWN_LEN : 0u,
-                                          lane == 1 ? LEAF_NONE : 0u);
-        nd_set(p, c, 0, lane, lane == 0 ? 0u : NODE_NONE, lane == 0 ? (i32)UNKNOWN_LEN : 0);
-        if (lane == 0) nd_set_parent(p, c, 0, NODE_NONE);
+        p.leaf[leaf0 * 32 + lane] = mk4(lane == 0 ? (u32)PEER_UNKNOWN : SLOT_EMPTY, 0, lane == 0 ? (u32)UNKNOWN_LEN : 0u,
+                                        lane == 1 ? LEAF_NONE : 0u);
+        nd_set(p, sm, 0, lane, lane == 0 ? 0u : NODE_NONE, lane == 0 ? (i32)UNKNOWN_LEN : 0);
+        if (lane == 0) nd_set_parent(p, sm, 0, NODE_NONE);
         sm->cvv[lane] = 0;
-        for (u32 q = 32 + (u32)lane; q < c.P; q += 32) p.cvv[c.cvv0 + q] = 0;
+        for (u32 q = 32 + (u32)lane; q < sm->P; q += 32) p.cvv[cvv0 + q] = 0;
         __syncwarp();
-        return c;
+        return;
     }
     u32 cached = n_nodes < LB_SEQ_NS ? n_nodes : LB_SEQ_NS;
     for (u32 nd = 0; nd < cached; nd++) {
-        uint2 e = p.node[(c.node0 + nd) * 32 + lane];
+        uint2 e = p.node[(node0 + nd) * 32 + lane];
         sm->child[nd][lane] = e.x;
         sm->vis[nd][lane] = (i32)e.y;
-        if (lane == 0) sm->parent[nd] = p.node_parent[c.node0 + nd];
+        if (lane == 0) sm->parent[nd] = p.node_parent[node0 + nd];
     }
-    sm->cvv[lane] = (u32)lane < c.P ? p.cvv[c.cvv0 + lane] : 0;
+    sm->cvv[lane] = (u32)lane < sm->P ? p.cvv[cvv0 + lane] : 0;
     __syncwarp();
-    return c;
 }
 
 // ---- emit the final visible runs of the active container (after checkout to the final version)
-__device__ __noinline__ void emit_output(const SeqPools& p, const BatchTables& t, Cx c, u64 cid0, u32 cidx) {
-    int lane = c.lane;
+__device__ __noinline__ void emit_output(const SeqPools& p, const BatchTables& t, u64 cid0, u32 cidx) {
+    SeqSmem* sm = seq_sm();
+    int lane = seq_lane();
     DocContainer& dc = t.dcont[cid0 + cidx];
     u32 n_out = 0;
     u32 total = 0;
-    u32 l2 = c.sm->first_leaf;
+    u32 l2 = sm->first_leaf;
     u32 out_cap = dc.out_cap;
     u64 out0 = dc.out0;
     while (l2 != LEAF_NONE) {
-        uint4 L = leaf_load(p, c, l2);
+        uint4 L = leaf_load(p, sm, l2);
         u32 pe = s_peer(L);
         bool live = pe != PEER_NONE && pe != PEER_UNKNOWN && s_st(L) == 0;
         unsigned m = __ballot_sync(LB_FULL, live);
         if (live) {
             u32 o = n_out + __popc(m & ((1u << lane) - 1));
             if (o < out_cap) {
-                u32 row = t.atom_row[atom_index(c, pe, (i32)L.y)];
+                u32 row = t.atom_row[atom_index(sm, pe, (i32)L.y)];
                 t.out_row[out0 + o] = row;
                 t.out_off[out0 + o] = (u32)((i32)L.y - t.op_counter[row]);
                 t.out_len[out0 + o] = L.z;
@@ -923,7 +880,7 @@ __device__ __noinline__ void emit_output(const SeqPools& p, const BatchTables& t
         n_out += __popc(m);
         l2 = __shfl_sync(LB_FULL, L.w, 1);
     }
-    if (n_out > out_cap) seq_fail(c, LB_ERR(DOC_ERR_CAPACITY));
+    if (n_out > out_cap) seq_fail(sm, LB_ERR(DOC_ERR_CAPACITY));
     __syncwarp();
     if (lane == 0) {
         dc.n_out = n_out < out_cap ? n_out : out_cap;
@@ -944,15 +901,14 @@ __device__ __forceinline__ void integrate_doc(DocInfo& di, SeqSmem* sm, int lane
     for (u32 ci = 0; ci < C; ci++)
         if (tables.dcont[cid0 + ci].leaf_cap) any = true;
     if (!any) return;
-    Cx c;
-    c.sm = sm;
-    c.dpeer = tables.dpeer + di.peer0;
-    c.leaf0 = c.node0 = c.cvv0 = 0;
-    c.atom0 = di.atom0;
-    c.P = P;
-    c.lane = lane;
-    sm->abase[lane] = (u32)lane < P ? c.dpeer[lane].atom_base : 0;
-    if (lane == 0) sm->err = 0;
+    const DocPeer* dpeer = tables.dpeer + di.peer0;
+    sm->abase[lane] = (u32)lane < P ? dpeer[lane].atom_base : 0;
+    if (lane == 0) {
+        sm->dpeer = dpeer;
+        sm->atom0 = di.atom0;
+        sm->P = P;
+        sm->err = 0;
+    }
     __syncwarp();
     for (u32 ci = lane; ci < C; ci += 32) pools.cont_epoch[cid0 + ci] = 0xFFFFFFFFu;
     __syncwarp();
@@ -991,17 +947,7 @@ __device__ __forceinline__ void integrate_doc(DocInfo& di, SeqSmem* sm, int lane
                 if (rb + (u32)lane < nr) { rec = tables.op_rec[r0 + rb + lane]; aux = tables.op_aux[r0 + rb + lane]; }
                 u32 kind_l = REC_KIND(rec.x);
                 // deletes: (possibly stale) home leaf of the first target atom
-                u32 hint_l = kind_l == OPK_SEQ_DEL ? pools.atom_leaf[atom_index(c, aux, (i32)rec.w)] : LEAF_NONE;
-#if LB_SEQ_PF
-                if (REC_CIDX(rec.x) == cidx && cidx != 0xFFFFFFFFu) {
-                    u32 pl = LEAF_NONE;
-                    if (kind_l == OPK_SEQ_DEL) pl = hint_l;
-#if LB_SEQ_PF > 1
-                    else if (kind_l == OPK_SEQ_INS) pl = predict_leaf(c, (i32)rec.w);
-#endif
-                    if (pl != LEAF_NONE && pl < sm->n_leaves) prefetch_leaf(pools, c, pl);
-                }
-#endif
+                u32 hint_l = kind_l == OPK_SEQ_DEL ? pools.atom_leaf[atom_index(sm, aux, (i32)rec.w)] : LEAF_NONE;
                 unsigned m = __ballot_sync(LB_FULL, kind_l == OPK_SEQ_INS || kind_l == OPK_SEQ_DEL);
                 while (m && !sm->err) {
                     int s = __ffs(m) - 1;
@@ -1013,26 +959,26 @@ __device__ __forceinline__ void integrate_doc(DocInfo& di, SeqSmem* sm, int lane
                     u32 ci = REC_CIDX(rx);
                     if (ci != cidx) {
                         if (cidx != 0xFFFFFFFFu && lane == 0) pools.cont_epoch[cid0 + cidx] = cur_epoch;
-                        if (cvv_dirty >= 0) { __syncwarp(); if (lane == 0) cvv_set(pools, c, peer, cvv_dirty); cvv_dirty = -1; }
-                        store_container(pools, tables, c, cid0, cidx);
-                        c = load_container(pools, tables, c, cid0, ci);
+                        if (cvv_dirty >= 0) { __syncwarp(); if (lane == 0) cvv_set(pools, sm, peer, cvv_dirty); cvv_dirty = -1; }
+                        store_container(pools, tables, cid0, cidx);
+                        load_container(pools, tables, cid0, ci);
                         cidx = ci;
                         if (sm->err) break;
                         cur_epoch = pools.cont_epoch[cid0 + ci];
                     }
                     if (cur_epoch != k) {
-                        if (!(chain && cur_epoch == k - 1)) checkout(pools, tables, c, ch0, cidx, vv, peer, ctr);
+                        if (!(chain && cur_epoch == k - 1)) checkout(pools, tables, sm, ch0, cidx, vv, peer, ctr);
                         cur_epoch = k;
                     }
-                    if (REC_KIND(rx) == OPK_SEQ_INS) seq_insert(pools, c, peer, ctr, len, prop);
+                    if (REC_KIND(rx) == OPK_SEQ_INS) seq_insert(pools, sm, peer, ctr, len, prop);
                     else   // delete by target id (crdt_rope.rs:236-315 ; tracker.rs:173-232)
-                        range_apply(pools, c, __shfl_sync(LB_FULL, aux, s), prop, prop + len, -1, +1, __shfl_sync(LB_FULL, hint_l, s));
+                        range_apply(pools, __shfl_sync(LB_FULL, aux, s), prop, prop + len, -1, +1, __shfl_sync(LB_FULL, hint_l, s));
                     // current_vv of the tracker follows its own ops (tracker.rs:131-139, 228-231); in causal order
                     // this entry only grows: written back when the container or the change ends
                     cvv_dirty = ctr + len;
                 }
             }
-            if (cvv_dirty >= 0) { __syncwarp(); if (lane == 0) cvv_set(pools, c, peer, cvv_dirty); __syncwarp(); }
+            if (cvv_dirty >= 0) { __syncwarp(); if (lane == 0) cvv_set(pools, sm, peer, cvv_dirty); __syncwarp(); }
             prev_peer = peer;
         }
     }
@@ -1041,22 +987,22 @@ __device__ __forceinline__ void integrate_doc(DocInfo& di, SeqSmem* sm, int lane
         const DocContainer& dc = tables.dcont[cid0 + ci];
         if (!dc.leaf_cap || (dc.n_leaves == 0 && ci != cidx)) continue;
         if (ci != cidx) {
-            store_container(pools, tables, c, cid0, cidx);
-            c = load_container(pools, tables, c, cid0, ci);
+            store_container(pools, tables, cid0, cidx);
+            load_container(pools, tables, cid0, ci);
             cidx = ci;
         }
         for (u32 q = 0; q < P && !sm->err; q++) {
-            i32 tgt = c.dpeer[q].end_counter;
-            i32 cur = cvv_get(pools, c, q);
-            if (cur > tgt) toggle_ops(pools, tables, c, ch0, cidx, q, tgt, cur, -1);
-            else if (cur < tgt) toggle_ops(pools, tables, c, ch0, cidx, q, cur, tgt, +1);
+            i32 tgt = sm->dpeer[q].end_counter;
+            i32 cur = cvv_get(pools, sm, q);
+            if (cur > tgt) toggle_ops(pools, tables, ch0, cidx, q, tgt, cur, -1);
+            else if (cur < tgt) toggle_ops(pools, tables, ch0, cidx, q, cur, tgt, +1);
             __syncwarp();
-            if (lane == 0) cvv_set(pools, c, q, tgt);
+            if (lane == 0) cvv_set(pools, sm, q, tgt);
             __syncwarp();
         }
-        if (!sm->err) emit_output(pools, tables, c, cid0, cidx);
+        if (!sm->err) emit_output(pools, tables, cid0, cidx);
     }
-    store_container(pools, tables, c, cid0, cidx);
+    store_container(pools, tables, cid0, cidx);
     __syncwarp();
     if (lane == 0 && sm->err) di.code = sm->err;
 }
@@ -1067,17 +1013,16 @@ __device__ __forceinline__ void integrate_doc(DocInfo& di, SeqSmem* sm, int lane
 // and no last wave of CTAs runs half full.  QUEUE = 0: warp w of the grid integrates document w; with every document
 // on a warp of its own the queue has nothing to balance, and its loop made the one-document C4 0.8 % slower (at 8 CTAs
 // per SM, DESIGN.md section 6).
-// 5 CTAs x 4 warps = 20 resident documents per SM (96 registers/thread).  Fewer documents per SM spill less and leave
-// each warp more L1 for its leaves and stack: on H100, C3 integrates fastest at 5 of the 4-12 measured (DESIGN.md
-// section 3).
-#define LB_SEQ_MINB 5
+// 8 CTAs x 4 warps = 32 resident documents per SM (64 registers/thread).  With the warp-uniform context in shared
+// memory the kernel spills little enough that more documents in flight win: on H100, C3 integrates fastest at 8 of the
+// 4, 5, 6, 8 and 10 measured (DESIGN.md section 3).
+#define LB_SEQ_MINB 8
 template <int QUEUE>
 __global__ void __launch_bounds__(32 * LB_SEQ_WARPS, LB_SEQ_MINB)
 k_seq_integrate(DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ SeqPools pools,
                 const __grid_constant__ BatchTables tables) {
-    __shared__ SeqSmem smem[LB_SEQ_WARPS];
-    SeqSmem* sm = &smem[threadIdx.x >> 5];
-    int lane = threadIdx.x & 31;
+    SeqSmem* sm = seq_sm();
+    int lane = seq_lane();
     if (!QUEUE) {
         u32 d = blockIdx.x * LB_SEQ_WARPS + (threadIdx.x >> 5);
         if (d < n_docs) integrate_doc(docs[d], sm, lane, pools, tables);
