@@ -20,6 +20,8 @@
  *   lb_docset_import         crates/loro/src/lib.rs:639, :425 on a document that already holds history
  *                            (crates/loro-internal/src/loro.rs:562-643, 1183-1290, oplog.rs:130-196)
  *   lb_batch_counters        crates/loro-internal/src/loro.rs:1458 len_ops / len_changes (summed over the batch)
+ *   lb_import_batch_at       crates/loro-internal/src/loro.rs:1353-1433 LoroDoc::checkout(&frontiers) after the import,
+ *   lb_docset_checkout       then get_deep_value() (the state at an earlier version: time travel)
  *
  * Conventions (mirroring the reference): input buffers are borrowed for the duration of the call only;
  * outputs are owned by the batch handle until lb_batch_free; a bad blob never aborts the batch -- it yields a
@@ -58,7 +60,8 @@ typedef enum lb_doc_code {
     LB_DOC_ERR_UNSUPPORTED = 5,     /* well-formed, but outside this path: an intact FastSnapshot blob    */
                                     /* (mode 3, SURVEY 8f.1), or ops the engine does not merge yet        */
                                     /* (rich-text styles, movable list, counter)                          */
-    LB_DOC_ERR_CAPACITY = 6         /* internal capacity bound exceeded (engine bug or adversarial input) */
+    LB_DOC_ERR_CAPACITY = 6,        /* internal capacity bound exceeded (engine bug or adversarial input) */
+    LB_DOC_ERR_FRONTIERS = 7        /* LoroError::FrontiersNotFound: a checkout id is not in the document  */
 } lb_doc_code;
 
 typedef struct lb_blob {
@@ -195,6 +198,35 @@ lb_status lb_docset_import(lb_docset* set, const lb_blob* blobs, size_t n_blobs,
 size_t lb_docset_doc_count(const lb_docset* set);
 uint64_t lb_docset_stored_bytes(const lb_docset* set);   /* device bytes of the stored documents */
 void lb_docset_free(lb_docset* set);
+
+/* ---- checkout: a document's state at an earlier version -----------------------------------------------------------
+ * LoroDoc::checkout(&frontiers) followed by get_deep_value() (crates/loro-internal/src/loro.rs:1353-1433).  The state at
+ * Frontiers F is built from every atom in the causal closure of F and from nothing else: a change that straddles the
+ * version is cut inside, its op under the cut inside the op.  Every id of F must be an atom the document holds (not an
+ * unknown peer, not a counter at or past the oplog vv, not inside a pending change), otherwise the document's code is
+ * LB_DOC_ERR_FRONTIERS (LoroError::FrontiersNotFound, loro.rs:1394-1410).  Redundant ids are allowed; n_frontiers = 0 is
+ * the empty version.  Every root container the document has registered is listed, with or without ops inside F
+ * (state.rs:894-924).  What a result handle answers for a requested document:
+ *   lb_doc_json                  get_deep_value() after the checkout;
+ *   lb_doc_status                the import's code and spans (LB_DOC_ERR_FRONTIERS when the import succeeded but F is
+ *                                not in the document; LB_DOC_ERR_UNSUPPORTED is decided over the whole applied history);
+ *   lb_doc_vv / lb_doc_frontiers the OPLOG's version vector and frontiers (the state's version is the request);
+ *   lb_doc_export_updates        LB_ERR_INVALID_ARG: a checked-out document is not exported. */
+typedef struct lb_version {
+    uint64_t doc_id;                 /* document doc_id at Frontiers `frontiers`: one span [counter, counter + 1) per id, */
+    const lb_id_span* frontiers;     /* the form lb_doc_frontiers returns; n_frontiers = 0 is the empty version            */
+    size_t n_frontiers;
+} lb_version;
+/* lb_import_batch(blobs), then checkout(F) of every document named in `at` (documents are numbered as in
+ * lb_import_batch).  A document that is not named stays at the latest version and answers byte for byte like
+ * lb_import_batch; naming it with n_frontiers = 0 asks for the empty version.  LB_ERR_INVALID_ARG: a doc_id named twice or
+ * carried by no blob, null frontiers with n_frontiers > 0, LB_FLAG_EXPORT or LB_FLAG_COMPACT in the flags. */
+lb_status lb_import_batch_at(const lb_blob* blobs, size_t n_blobs, const lb_version* at, size_t n_at,
+                             const lb_options* opt, lb_batch** out);
+/* One document per request, in request order: the stored document doc_id at Frontiers F (a doc_id may repeat, at different
+ * versions; one the set has never seen is an empty document).  The status spans are empty: nothing is imported.  The
+ * docset is not modified.  LB_ERR_INVALID_ARG: null frontiers with n_frontiers > 0, LB_FLAG_EXPORT or LB_FLAG_COMPACT. */
+lb_status lb_docset_checkout(lb_docset* set, const lb_version* at, size_t n_at, const lb_options* opt, lb_batch** out);
 
 /* test hooks (need LB_FLAG_KEEP_DEVICE): copy one decoded SoA table to the host.
  * name in {"op_cid","op_prop","op_vtype","op_len","op_counter","ch_counter","ch_len","ch_lamport",

@@ -13,7 +13,7 @@ LB_FLAG_EXPORT = 4
 LB_FLAG_COMPACT = 8
 
 DOC_CODES = {0: "Ok", 1: "DecodeError", 2: "DecodeChecksumMismatchError", 3: "IncompatibleFutureEncodingError",
-             4: "DecodeDataCorruptionError", 5: "Unsupported", 6: "CapacityExceeded"}
+             4: "DecodeDataCorruptionError", 5: "Unsupported", 6: "CapacityExceeded", 7: "FrontiersNotFound"}
 
 ImportStatus = namedtuple("ImportStatus", "code success pending")
 
@@ -38,6 +38,10 @@ class _Options(ctypes.Structure):
 
 class _IdSpan(ctypes.Structure):
     _fields_ = [("peer", ctypes.c_uint64), ("start", ctypes.c_int32), ("end", ctypes.c_int32)]
+
+
+class _Version(ctypes.Structure):
+    _fields_ = [("doc_id", ctypes.c_uint64), ("frontiers", ctypes.POINTER(_IdSpan)), ("n_frontiers", ctypes.c_size_t)]
 
 
 class _Status(ctypes.Structure):
@@ -98,6 +102,10 @@ def load_library(path=None):
                                  ctypes.POINTER(ctypes.c_size_t)]
     L.lb_docset_new.argtypes = [ctypes.POINTER(_Options), ctypes.POINTER(vp)]
     L.lb_docset_import.argtypes = [vp, ctypes.POINTER(_Blob), ctypes.c_size_t, ctypes.POINTER(_Options), ctypes.POINTER(vp)]
+    L.lb_import_batch_at.argtypes = [ctypes.POINTER(_Blob), ctypes.c_size_t, ctypes.POINTER(_Version), ctypes.c_size_t,
+                                     ctypes.POINTER(_Options), ctypes.POINTER(vp)]
+    L.lb_docset_checkout.argtypes = [vp, ctypes.POINTER(_Version), ctypes.c_size_t, ctypes.POINTER(_Options),
+                                     ctypes.POINTER(vp)]
     L.lb_docset_doc_count.restype = ctypes.c_size_t
     L.lb_docset_doc_count.argtypes = [vp]
     L.lb_docset_stored_bytes.restype = ctypes.c_uint64
@@ -377,6 +385,38 @@ def import_batch(blobs, device=0, flags=0, lib_path=None, doc_ids=None, split=No
     return Batch(L, h.value)
 
 
+def import_batch_at(blobs, versions, doc_ids=None, device=0, flags=0, lib_path=None):
+    """import_batch(blobs, doc_ids=doc_ids) followed by LoroDoc::checkout(frontiers) of every document named in
+    `versions`: {doc_id: [(peer, counter), ...]} (an empty list is the empty version).  Documents not named stay at the
+    latest version.  A frontier id the document does not hold gives that document code 7 (FrontiersNotFound)."""
+    L = load_library(lib_path)
+    arr, keep = _blob_array(blobs, doc_ids)
+    ver, vkeep = _version_array(list(versions.items()))
+    opt = _Options(device=device, flags=flags)
+    h = ctypes.c_void_p()
+    _check(L, L.lb_import_batch_at(arr, len(blobs), ver, len(versions), ctypes.byref(opt), ctypes.byref(h)),
+           "lb_import_batch_at")
+    return Batch(L, h.value)
+
+
+def _version_array(requests):
+    """[(doc_id, [(peer, counter), ...]), ...] -> lb_version array (+ the span arrays it points into)"""
+    arr = (_Version * max(len(requests), 1))()
+    keep = []
+    for i, (doc_id, frontiers) in enumerate(requests):
+        frontiers = list(frontiers)
+        spans = (_IdSpan * max(len(frontiers), 1))()
+        for k, (peer, ctr) in enumerate(frontiers):
+            spans[k].peer = int(peer)
+            spans[k].start = int(ctr)
+            spans[k].end = int(ctr) + 1
+        keep.append(spans)
+        arr[i].doc_id = int(doc_id)
+        arr[i].frontiers = spans
+        arr[i].n_frontiers = len(frontiers)
+    return arr, keep
+
+
 def _blob_array(blobs, doc_ids):
     n = len(blobs)
     arr = (_Blob * max(n, 1))()
@@ -410,6 +450,18 @@ class DocSet:
         opt = _Options(device=self._device, flags=flags)
         h = ctypes.c_void_p()
         _check(self._L, self._L.lb_docset_import(self._h, arr, len(blobs), ctypes.byref(opt), ctypes.byref(h)), "lb_docset_import")
+        return Batch(self._L, h.value)
+
+    def checkout(self, requests, flags=0):
+        """The stored documents at earlier versions: `requests` = [(doc_id, [(peer, counter), ...]), ...].  Document i of
+        the returned Batch is request i (a doc_id may repeat; one the set has never seen is an empty document).  The set is
+        not modified."""
+        requests = list(requests)
+        ver, keep = _version_array(requests)
+        opt = _Options(device=self._device, flags=flags)
+        h = ctypes.c_void_p()
+        _check(self._L, self._L.lb_docset_checkout(self._h, ver, len(requests), ctypes.byref(opt), ctypes.byref(h)),
+               "lb_docset_checkout")
         return Batch(self._L, h.value)
 
     @property

@@ -25,6 +25,7 @@
 #include "k_decode_warp.cuh"
 #include "k_resolve.cuh"
 #include "k_classify.cuh"
+#include "k_checkout.cuh"
 #include "k_seq.cuh"
 #include "k_tree.cuh"
 #include "k_state.cuh"
@@ -313,6 +314,12 @@ struct lb_batch {
     size_t n_blobs = 0;                       // blobs in the byte buffer (>= n_docs: import_batch groups)
     std::vector<u32> blob_doc, doc_blob0;     // blob -> document ; document -> first blob (n_docs + 1)
     std::vector<u32> doc_nprior;              // lb_docset_import: leading blobs of each document that restate its earlier state
+    // checkout requests (k_checkout.cuh), empty when the batch has none: document d is built at the ids
+    // [ck_range[2d], ck_range[2d + 1]) of ck_peer / ck_ctr, or at the latest version when ck_range[2d] == CK_LATEST
+    std::vector<u32> ck_range;
+    std::vector<u64> ck_peer;
+    std::vector<i32> ck_ctr;
+    bool ck_docset = false;                   // lb_docset_checkout: nothing was imported, the status spans stay empty
     DocInfo* d_docs = nullptr;
     u8* d_json = nullptr;
     u8* d_export = nullptr;      // phase 7 output: one FastUpdates blob per document
@@ -523,6 +530,20 @@ void pipeline(lb_batch* b) {
         d_doc_nprior = dv.alloc<u32>(D + 1);
         CK(cudaMemcpyAsync(d_doc_nprior, b->doc_nprior.data(), sizeof(u32) * D, cudaMemcpyHostToDevice, st));
     }
+    uint2* d_ck_range = nullptr;
+    u64* d_ck_peer = nullptr;
+    i32* d_ck_ctr = nullptr;
+    if (!b->ck_range.empty()) {   // the host vectors live as long as the batch: no synchronise needed
+        const size_t NF = b->ck_peer.size();
+        d_ck_range = dv.alloc<uint2>(D);
+        d_ck_peer = dv.alloc<u64>(NF);
+        d_ck_ctr = dv.alloc<i32>(NF);
+        CK(cudaMemcpyAsync(d_ck_range, b->ck_range.data(), sizeof(u32) * 2 * D, cudaMemcpyHostToDevice, st));
+        if (NF) {
+            CK(cudaMemcpyAsync(d_ck_peer, b->ck_peer.data(), sizeof(u64) * NF, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(d_ck_ctr, b->ck_ctr.data(), sizeof(i32) * NF, cudaMemcpyHostToDevice, st));
+        }
+    }
     LB_LAUNCH(k_frame_docs, nblk(D), TPB, 0, st, D, d_doc_blob0, d_blob_code, d_blob_block0, d_doc_nprior, b->d_docs);
     tm.kernel_launches += 2;
     u64 B = d2h_one(b, d_blob_block0 + Q);
@@ -626,6 +647,11 @@ void pipeline(lb_batch* b) {
     u32* d_cursor = dv.alloc<u32>(NP);
     LB_LAUNCH(k_doc_causal, nblk(D, 64), 64, 0, st, b->d_docs, D, blk, t, d_cursor, d_doc_blob0, d_pend_scratch);
     LB_LAUNCH(k_doc_frontiers, nblk(D, 64), 64, 0, st, b->d_docs, D, t);
+    if (d_ck_range) {
+        t.ck_end = dv.alloc<i32>(NP + 1);
+        LB_LAUNCH(k_doc_checkout, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, t, d_ck_range, d_ck_peer, d_ck_ctr);
+        tm.kernel_launches += 1;
+    }
     LB_LAUNCH(k_doc_sizes, nblk(D), TPB, 0, st, b->d_docs, D, d_tmp_a, d_tmp_b, d_tmp_c, 1);
     tm.kernel_launches += 3;
     run_scans(b, {ScanJob{(const u8*)d_tmp_b, (u8*)b->d_docs + offsetof(DocInfo, atom0), 4, sizeof(DocInfo), D},
@@ -869,11 +895,11 @@ void build_status(lb_batch* b) {
     for (size_t d = 0; d < D; d++) {
         DocInfo& di = b->docs[d];
         if (di.code == DOC_OK && di.has_unsupported) di.code = DOC_ERR_UNSUPPORTED;
-        if (di.code == DOC_OK || di.code == DOC_ERR_UNSUPPORTED) {
+        if (di.code == DOC_OK || di.code == DOC_ERR_UNSUPPORTED || di.code == DOC_ERR_FRONTIERS) {
             for (u32 p = 0; p < di.P; p++) {
                 const DocPeer& dp = b->dpeer[b->peer_base[d] + p];
-                if (dp.has_succ) b->spans[0].push_back(lb_id_span{dp.id, dp.succ_lo, dp.end_counter});
-                if (dp.pend_hi > dp.pend_lo) b->spans[1].push_back(lb_id_span{dp.id, dp.pend_lo, dp.pend_hi});
+                if (dp.has_succ && !b->ck_docset) b->spans[0].push_back(lb_id_span{dp.id, dp.succ_lo, dp.end_counter});
+                if (dp.pend_hi > dp.pend_lo && !b->ck_docset) b->spans[1].push_back(lb_id_span{dp.id, dp.pend_lo, dp.pend_hi});
                 if (dp.end_counter > 0) b->spans[2].push_back(lb_id_span{dp.id, 0, dp.end_counter});
                 if (dp.is_head && dp.end_counter > 0) b->spans[3].push_back(lb_id_span{dp.id, dp.end_counter - 1, dp.end_counter});
             }
@@ -1086,15 +1112,28 @@ void docset_store(lb_docset* set, lb_batch* b, const std::vector<u64>& offs, con
 
 extern "C" {
 
-// Host-buffer import, shared by lb_import_batch (fresh documents) and lb_docset_import (documents with an earlier state:
-// their stored blobs come first, already in device memory, and count as `n_prior` for the import status).
-static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_options* opt, lb_docset* set, lb_batch** out) {
-    if (!out || (!blobs && n_blobs)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
+// Host-buffer import, shared by lb_import_batch (fresh documents), lb_docset_import (documents with an earlier state:
+// their stored blobs come first, already in device memory, and count as `n_prior` for the import status) and the
+// checkout entry points: `at` names the documents built at an earlier version (k_checkout.cuh).  With `set_checkout` the
+// documents are the requests themselves, one per entry of `at`, each made of its document's stored blobs only; the
+// docset is read, never written.
+static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_version* at, size_t n_at, const lb_options* opt,
+                             lb_docset* set, bool set_checkout, lb_batch** out) {
+    if (!out || (!blobs && n_blobs) || (!at && n_at)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
     *out = nullptr;
     lb_options o2;
     memset(&o2, 0, sizeof(o2));
     if (opt) o2 = *opt;
-    if (set) { o2.device = set->device; o2.flags |= LB_FLAG_EXPORT; }   // the re-export is what a stored document keeps
+    if (at || set_checkout) {
+        if (o2.flags & (LB_FLAG_EXPORT | LB_FLAG_COMPACT)) {
+            g_last_error = "a checked-out document is not exported (LB_FLAG_EXPORT / LB_FLAG_COMPACT)";
+            return LB_ERR_INVALID_ARG;
+        }
+        for (size_t i = 0; i < n_at; i++)
+            if (!at[i].frontiers && at[i].n_frontiers) { g_last_error = "null frontiers"; return LB_ERR_INVALID_ARG; }
+    }
+    if (set) o2.device = set->device;
+    if (set && !set_checkout) o2.flags |= LB_FLAG_EXPORT;   // the re-export is what a stored document keeps
     lb_status s = check_device(&o2);
     if (s != LB_OK) return s;
     if (n_blobs >= 0x7FFFFFFFull) { g_last_error = "too many blobs"; return LB_ERR_INVALID_ARG; }
@@ -1109,8 +1148,8 @@ static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_opti
         // first appearance and their blobs laid out consecutively, in the order given
         std::vector<u32> order(n_blobs);
         std::vector<u32> host_count;
+        std::unordered_map<u64, u32> doc_of;
         {
-            std::unordered_map<u64, u32> doc_of;
             std::vector<u32> doc_idx(n_blobs);
             std::vector<u32>& count = host_count;
             for (size_t i = 0; i < n_blobs; i++) {
@@ -1142,9 +1181,31 @@ static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_opti
                 std::stable_sort(keyed.begin(), keyed.end(), [](const auto& x, const auto& y) { return x.first < y.first; });
                 for (u32 q = q0; q < q1; q++) order[q] = keyed[q - q0].second;
             }
+            if (set_checkout)   // one document per request, in request order (no new blobs)
+                for (size_t i = 0; i < n_at; i++) { b->doc_ids.push_back(at[i].doc_id); count.push_back(0); nd++; }
             b->n_docs = nd;
         }
         const size_t nd = b->n_docs;
+        if (at) {
+            b->ck_docset = set_checkout;
+            b->ck_range.assign(2 * nd, CK_LATEST);
+            for (size_t i = 0; i < n_at; i++) {
+                u32 d = (u32)i;
+                if (!set_checkout) {
+                    auto it = doc_of.find(at[i].doc_id);
+                    if (it == doc_of.end()) { g_last_error = "checkout of a doc_id no blob carries"; throw lb_status(LB_ERR_INVALID_ARG); }
+                    d = it->second;
+                    if (b->ck_range[2 * d] != CK_LATEST) { g_last_error = "doc_id requested twice"; throw lb_status(LB_ERR_INVALID_ARG); }
+                }
+                b->ck_range[2 * d] = (u32)b->ck_peer.size();
+                for (size_t k = 0; k < at[i].n_frontiers; k++) {   // one span [counter, counter + 1) per id
+                    b->ck_peer.push_back(at[i].frontiers[k].peer);
+                    b->ck_ctr.push_back(at[i].frontiers[k].start);
+                }
+                b->ck_range[2 * d + 1] = (u32)b->ck_peer.size();
+            }
+            if (b->ck_peer.size() >= CK_LATEST) { g_last_error = "too many frontier ids"; throw lb_status(LB_ERR_INVALID_ARG); }
+        }
         // the blob list of the batch: per document, its stored blobs (device) then the new ones (host)
         std::vector<DocsetDoc*> prior(nd, nullptr);
         size_t n_prior_total = 0;
@@ -1232,7 +1293,7 @@ static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_opti
         // event indices: 0 start,1 h2d,2 frame,3 decode,4 resolve,5 classify,6 integrate,7 materialise,8 d2h
         s = run_batch(b);
         CK(cudaStreamSynchronize(b->dev.stream));
-        if (s == LB_OK && set) docset_store(set, b, offs, lens);
+        if (s == LB_OK && set && !set_checkout) docset_store(set, b, offs, lens);
     } catch (lb_status e) {
         s = e;
     }
@@ -1242,7 +1303,12 @@ static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_opti
 }
 
 lb_status lb_import_batch(const lb_blob* blobs, size_t n_blobs, const lb_options* opt, lb_batch** out) {
-    return import_host(blobs, n_blobs, opt, nullptr, out);
+    return import_host(blobs, n_blobs, nullptr, 0, opt, nullptr, false, out);
+}
+
+lb_status lb_import_batch_at(const lb_blob* blobs, size_t n_blobs, const lb_version* at, size_t n_at, const lb_options* opt,
+                             lb_batch** out) {
+    return import_host(blobs, n_blobs, at, n_at, opt, nullptr, false, out);
 }
 
 lb_status lb_docset_new(const lb_options* opt, lb_docset** out) {
@@ -1265,7 +1331,13 @@ uint64_t lb_docset_stored_bytes(const lb_docset* set) { return set ? set->stored
 lb_status lb_docset_import(lb_docset* set, const lb_blob* blobs, size_t n_blobs, const lb_options* opt, lb_batch** out) {
     if (!set) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
     std::lock_guard<std::mutex> g(set->mu);
-    return import_host(blobs, n_blobs, opt, set, out);
+    return import_host(blobs, n_blobs, nullptr, 0, opt, set, false, out);
+}
+
+lb_status lb_docset_checkout(lb_docset* set, const lb_version* at, size_t n_at, const lb_options* opt, lb_batch** out) {
+    if (!set) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
+    std::lock_guard<std::mutex> g(set->mu);
+    return import_host(nullptr, 0, at, n_at, opt, set, true, out);
 }
 
 lb_status lb_import_batch_device(const uint8_t* d_bytes, const uint64_t* offsets, const uint32_t* blob_lens,

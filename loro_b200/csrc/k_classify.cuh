@@ -65,6 +65,16 @@ __global__ void k_op_classify(DocInfo* __restrict__ docs, u64 n_rows, const __gr
         if (t.op_counter[row] + (i32)t.op_len[row] <= cut) kind = OPK_SKIP;
         else if (t.op_counter[row] < cut) cut_skip = (u32)(cut - t.op_counter[row]);
     }
+    // checkout (k_checkout.cuh): the mirror at the other end -- a row wholly at or past the requested version is no part
+    // of the state, the row under the cut loses its last `cut_tail` atoms.  Both cuts can hit one row.
+    u32 cut_tail = 0;
+    bool beyond = false;
+    if (t.ck_end) {
+        const i32 end = t.ck_end[di.peer0 + t.ch_peer[ch]];
+        const i32 row_end = t.op_counter[row] + (i32)t.op_len[row];
+        if (t.op_counter[row] + (i32)cut_skip >= end) beyond = true;
+        else if (row_end > end) cut_tail = (u32)(row_end - end);
+    }
     u32 lam = t.ch_lamport[ch] + (u32)(t.op_counter[row] - t.ch_counter[ch]);
     if (kind != OPK_TREE && t.op_vtype[row] == VK_RAW_TREE_MOVE) {
         // a RawTreeMove row that is not an applied op of a Tree container: its slot of the tree tables says so (the
@@ -100,6 +110,7 @@ __global__ void k_op_classify(DocInfo* __restrict__ docs, u64 n_rows, const __gr
             ids.x = tp; ids.y = (u32)tc; ids.z = (u32)pk | (pp << 2); ids.w = (u32)pc;
             t.tr_ids[ti] = ids;
             t.tr_key[ti] = ((u64)lam << 32) | ((u64)t.dpeer[di.peer0 + t.ch_peer[ch]].rank << 16);
+            if (beyond) { t.tr_rec[ti].w = 0xFFFFFFFFu; t.tr_key[ti] = ~0ull; }
         }
     }
     {   // tracker record: everything k_seq needs about this row in one 16-byte load
@@ -116,11 +127,17 @@ __global__ void k_op_classify(DocInfo* __restrict__ docs, u64 n_rows, const __gr
             aux = tp;
             rev = dlen < 0 ? 1u : 0u;
             if (cut_skip && !rev) w += cut_skip;   // forward span: the first targets go with the dropped atoms
+            if (rev) w += cut_tail;                // reversed span: the last atoms delete the lowest targets
+                                                   // (DeleteSpanWithId::slice, container/list/list_op.rs:251-270)
         } else if (kind == OPK_SEQ_INS) w += cut_skip;   // insert position of the first kept atom
+        if (beyond) {   // unsupported ops are counted over the whole applied history, wherever they fall
+            if (kind == OPK_UNSUPPORTED) atomicAdd(&di.has_unsupported, 1u);
+            kind = OPK_SKIP;
+        }
         uint4 rec;
         rec.x = (u32)kind | (rev << 3) | (cidx << 4);
         rec.y = (u32)t.op_counter[row] + cut_skip;
-        rec.z = t.op_len[row] - cut_skip;
+        rec.z = t.op_len[row] - cut_skip - cut_tail;
         rec.w = w;
         t.op_rec[row] = rec;
         t.op_aux[row] = aux;
@@ -129,7 +146,7 @@ __global__ void k_op_classify(DocInfo* __restrict__ docs, u64 n_rows, const __gr
     t.op_cidx[row] = cidx;
     t.op_lamport[row] = lam;
     if (kind == OPK_SKIP) return;
-    u32 len = t.op_len[row] - cut_skip;
+    u32 len = t.op_len[row] - cut_skip - cut_tail;
     const DocPeer& dp = t.dpeer[di.peer0 + t.ch_peer[ch]];
     // atom -> row index (used by the tracker to resolve ids; reference: id_to_cursor.rs)
     u64 a0 = di.atom0 + dp.atom_base + (u32)t.op_counter[row] + cut_skip;

@@ -982,7 +982,8 @@ __device__ __forceinline__ void integrate_doc(DocInfo& di, SeqSmem* sm, int lane
             prev_peer = peer;
         }
     }
-    // final version = everything applied
+    // final version = everything applied, or the requested version of a checkout (k_checkout.cuh): the atoms past it were
+    // never integrated, and their atom -> row entries were never written
     for (u32 ci = 0; ci < C && !sm->err; ci++) {
         const DocContainer& dc = tables.dcont[cid0 + ci];
         if (!dc.leaf_cap || (dc.n_leaves == 0 && ci != cidx)) continue;
@@ -992,7 +993,7 @@ __device__ __forceinline__ void integrate_doc(DocInfo& di, SeqSmem* sm, int lane
             cidx = ci;
         }
         for (u32 q = 0; q < P && !sm->err; q++) {
-            i32 tgt = sm->dpeer[q].end_counter;
+            i32 tgt = tables.ck_end ? tables.ck_end[(sm->dpeer - tables.dpeer) + q] : sm->dpeer[q].end_counter;
             i32 cur = cvv_get(pools, sm, q);
             if (cur > tgt) toggle_ops(pools, tables, ch0, cidx, q, tgt, cur, -1);
             else if (cur < tgt) toggle_ops(pools, tables, ch0, cidx, q, cur, tgt, +1);

@@ -40,7 +40,7 @@ typedef int64_t i64;
 
 // per-document codes (mirror include/loro_b200.h lb_doc_code)
 enum { DOC_OK = 0, DOC_ERR_DECODE = 1, DOC_ERR_CHECKSUM = 2, DOC_ERR_MODE = 3, DOC_ERR_CORRUPT = 4,
-       DOC_ERR_UNSUPPORTED = 5, DOC_ERR_CAPACITY = 6 };
+       DOC_ERR_UNSUPPORTED = 5, DOC_ERR_CAPACITY = 6, DOC_ERR_FRONTIERS = 7 };
 
 // value kinds of the `values` stream (reference: encoding/value.rs:39-161)
 enum { VK_NULL = 0, VK_TRUE = 1, VK_FALSE = 2, VK_I64 = 3, VK_F64 = 4, VK_STR = 5, VK_BINARY = 6,

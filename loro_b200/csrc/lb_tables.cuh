@@ -118,4 +118,8 @@ struct BatchTables {
     // a copy of the batch's struct.
     u32 only_doc; const i32* from_ctr;
     XDoc* xdoc;
+    // ---- checkout (k_checkout.cuh), written after the causal scan, read by phases 4 and 5 (last, so that the layout of
+    // every other field is the same with or without it)
+    i32* ck_end;         // per doc peer: the version the state is built at: atoms at or past it are cut; end_counter for
+                         // documents without a request.  Null when the batch has no checkout request
 };
