@@ -109,6 +109,8 @@ typedef struct lb_timings { /* device time per phase in milliseconds (CUDA event
     float h2d, frame, decode, resolve, classify, integrate, materialise, d2h, total_device, reexport;
     /* algorithmic bytes of the decode phase (SURVEY.md 8d): blob bytes read + SoA bytes written */
     uint64_t decode_bytes_read, decode_bytes_written;
+    /* kernels launched for this batch so far: lb_batch_timings reads it at call time, so the launches of a later
+     * lb_doc_export_updates(from) show up in the next read */
     uint32_t kernel_launches;
     uint64_t export_bytes;             /* bytes written by the re-export phase */
     float tree;                        /* movable-tree phase (sort, apply, sibling lists) */

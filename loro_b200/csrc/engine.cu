@@ -51,22 +51,31 @@ void lb_launch_failed(const char* kernel, cudaError_t e) {
 }
 #endif
 
-// thread per doc helpers -------------------------------------------------------------------------
-__global__ void k_doc_sizes(const DocInfo* __restrict__ docs, u32 n_docs, u32* __restrict__ vvsize,
-                            u32* __restrict__ atoms, u32* __restrict__ mapslots, int which) {
+// thread per doc helpers: the per-document sizes the host scans into table offsets ------------------
+__global__ void k_doc_vv_cells(const DocInfo* __restrict__ docs, u32 n_docs, u32* __restrict__ vv_cells) {
+    u32 d = blockIdx.x * blockDim.x + threadIdx.x;
+    if (d >= n_docs) return;
+    const DocInfo& di = docs[d];
+    vv_cells[d] = di.code == DOC_OK ? di.n_changes * di.P : 0;
+}
+__global__ void k_doc_atoms_mapslots(const DocInfo* __restrict__ docs, u32 n_docs, u32* __restrict__ atoms,
+                                     u32* __restrict__ mapslots) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
     const DocInfo& di = docs[d];
     bool ok = di.code == DOC_OK;
-    if (which == 0) vvsize[d] = ok ? di.n_changes * di.P : 0;
-    else if (which == 2) {   // tree node slots (k_tree.cuh) ; atoms[n_docs] collects the largest tree document
-        vvsize[d] = ok && di.has_tree ? (u32)di.atom_total + di.C : 0;
-        if (ok && di.has_tree) atomicMax(&atoms[n_docs], (u32)di.atom_total);
-    }
-    else {
-        atoms[d] = ok ? (u32)di.atom_total : 0;
-        mapslots[d] = ok ? di.C * di.K : 0;
-    }
+    atoms[d] = ok ? (u32)di.atom_total : 0;
+    mapslots[d] = ok ? di.C * di.K : 0;
+}
+// tree node slots (k_tree.cuh) and, in *max_tree_atoms (zero on entry), the atoms of the largest tree document
+__global__ void k_doc_tree_slots(const DocInfo* __restrict__ docs, u32 n_docs, u32* __restrict__ tree_slots,
+                                 u32* __restrict__ max_tree_atoms) {
+    u32 d = blockIdx.x * blockDim.x + threadIdx.x;
+    if (d >= n_docs) return;
+    const DocInfo& di = docs[d];
+    bool tree = di.code == DOC_OK && di.has_tree;
+    tree_slots[d] = tree ? (u32)di.atom_total + di.C : 0;
+    if (tree) atomicMax(max_tree_atoms, (u32)di.atom_total);
 }
 __global__ void k_pack_peers(const DocInfo* __restrict__ docs, u32 n_docs, const DocPeer* __restrict__ dpeer,
                              const u64* __restrict__ base, DocPeer* __restrict__ out) {
@@ -133,6 +142,9 @@ __global__ void k_copy_segments(const CopySeg* __restrict__ segs, u32 n) {
 }
 
 namespace {
+
+// LB_PHASE_TRACE: diagnostics on stderr.  Read at every use, so that a process can switch it on between batches.
+inline bool phase_trace() { return getenv("LB_PHASE_TRACE") != nullptr; }
 
 // Device blocks that lived until their batch was freed are kept per device, by size class, and handed to the next batch
 // that asks for the same class: a service imports batch after batch of similar shape, and the stream-ordered pool took
@@ -252,7 +264,7 @@ struct Dev {  // owns every device allocation of a batch
         }
         double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
         alloc_ms += ms;
-        if (ms > 1.0 && getenv("LB_PHASE_TRACE")) fprintf(stderr, "[trace] slow alloc: %zu bytes took %.3f ms\n", sz, ms);
+        if (ms > 1.0 && phase_trace()) fprintf(stderr, "[trace] slow alloc: %zu bytes took %.3f ms\n", sz, ms);
         if (!carved) { ptrs.push_back({p, sz}); bytes += sz; }
         if (zero) CK(cudaMemsetAsync(p, 0, want, stream));
         return (T*)p;
@@ -302,6 +314,11 @@ struct Dev {  // owns every device allocation of a batch
 
 }  // namespace
 
+// Events on the batch stream, in pipeline order: EV_x is recorded when phase x has been enqueued (mark), and a phase's
+// device time is the interval from the event before it (timings_from_events).
+enum BatchEvent { EV_START, EV_H2D, EV_FRAME, EV_DECODE, EV_RESOLVE, EV_CLASSIFY, EV_INTEGRATE, EV_TREE, EV_MATERIALISE,
+                  EV_EXPORT, EV_D2H, EV_COUNT };
+
 struct lb_batch {
     Dev dev;
     size_t n_docs = 0;
@@ -347,8 +364,8 @@ struct lb_batch {
     lb_counters counters{};
     lb_timings timings{};
     std::chrono::steady_clock::time_point t_call = std::chrono::steady_clock::now(), t_tail = t_call;
-    cudaEvent_t ev[16];
-    int n_ev = 0;
+    cudaEvent_t ev[EV_COUNT];
+    bool ev_recorded[EV_COUNT] = {};
     bool ev_created = false;
 };
 
@@ -375,13 +392,19 @@ namespace {
 const int TPB = 128;
 inline unsigned nblk(u64 n, int tpb = TPB) { return (unsigned)((n + tpb - 1) / tpb); }
 
+// Every kernel a batch launches goes through here: on the batch's stream, and counted in lb_timings.kernel_launches.
+#define LB_BATCH_LAUNCH(b, kernel, grid, block, smem, ...)                          \
+    do {                                                                            \
+        LB_LAUNCH(kernel, grid, block, smem, (b)->dev.stream, __VA_ARGS__);         \
+        (b)->timings.kernel_launches++;                                             \
+    } while (0)
+
 // the export encoder over NOB output blocks (retry = 1: only the blocks that outgrew their staging slot, into their
 // retry slots), in the build that is faster for that many (k_export.cuh)
-void launch_exp_encode(cudaStream_t st, DocInfo* docs, u64 NOB, const BatchTables& xt, XBlock* xb, u32* xscratch, u8* out,
-                       int retry) {
+void launch_exp_encode(lb_batch* b, u64 NOB, const BatchTables& xt, XBlock* xb, u32* xscratch, u8* out, int retry) {
     if (!NOB) return;
-    if (NOB >= LB_XENC_BOUNDED_MIN_BLOCKS) LB_LAUNCH(k_exp_encode<1>, nblk(NOB, 64), 64, 0, st, docs, NOB, xt, xb, xscratch, out, retry);
-    else LB_LAUNCH(k_exp_encode<0>, nblk(NOB, 64), 64, 0, st, docs, NOB, xt, xb, xscratch, out, retry);
+    if (NOB >= LB_XENC_BOUNDED_MIN_BLOCKS) LB_BATCH_LAUNCH(b, k_exp_encode<1>, nblk(NOB, 64), 64, 0, b->d_docs, NOB, xt, xb, xscratch, out, retry);
+    else LB_BATCH_LAUNCH(b, k_exp_encode<0>, nblk(NOB, 64), 64, 0, b->d_docs, NOB, xt, xb, xscratch, out, retry);
 }
 
 // CTAs of k_seq_integrate that the device holds at once, computed once per device: a batch that needs more gets that
@@ -410,8 +433,9 @@ unsigned seq_resident_ctas(int device) {
 
 // LB_PHASE_TRACE=1: host wall clock between named points (each one synchronises the stream: diagnosis only)
 void trace_point(lb_batch* b, const char* name);
-void mark(lb_batch* b) {
-    if (b->n_ev < 16) CK(cudaEventRecord(b->ev[b->n_ev++], b->dev.stream));
+void mark(lb_batch* b, BatchEvent e) {
+    CK(cudaEventRecord(b->ev[e], b->dev.stream));
+    b->ev_recorded[e] = true;
 }
 
 template <class T>
@@ -423,8 +447,7 @@ T d2h_one(lb_batch* b, const T* src) {
 }
 
 void trace_point(lb_batch* b, const char* name) {
-    static const bool on = getenv("LB_PHASE_TRACE") != nullptr;
-    if (!on) return;
+    if (!phase_trace()) return;
     static std::chrono::steady_clock::time_point last = std::chrono::steady_clock::now();
     cudaStreamSynchronize(b->dev.stream);
     auto now = std::chrono::steady_clock::now();
@@ -438,8 +461,7 @@ void run_scans(lb_batch* b, std::vector<ScanJob> jobs) {
         memset(&sj, 0, sizeof(sj));
         unsigned n = 0;
         for (; n < 8 && i + n < jobs.size(); n++) sj.j[n] = jobs[i + n];
-        LB_LAUNCH(k_excl_scan_multi, n, 1024, 0, b->dev.stream, sj);
-        b->timings.kernel_launches++;
+        LB_BATCH_LAUNCH(b, k_excl_scan_multi, n, 1024, 0, sj);
     }
 }
 #define FIELD_JOB(base, type, in_field, out_field, count)                                              \
@@ -454,13 +476,10 @@ void run_scans(lb_batch* b, std::vector<ScanJob> jobs) {
 // Returns the export buffer (*total bytes, document d's blob at xt.xdoc[d].exp_off).
 u8* export_encode(lb_batch* b, const BatchTables& xt, u64* total) {
     Dev& dv = b->dev;
-    cudaStream_t st = dv.stream;
     const u32 D = (u32)b->n_docs;
-    lb_timings& tm = b->timings;
     u32* cnt = dv.alloc<u32>(3 * (u64)(D + 1));
     u32 *n_a = cnt, *n_b = cnt + (D + 1), *n_c = cnt + 2 * (D + 1);
-    LB_LAUNCH(k_exp_sizes, nblk(D), TPB, 0, st, b->d_docs, D, xt, n_a, n_b, n_c);
-    tm.kernel_launches += 1;
+    LB_BATCH_LAUNCH(b, k_exp_sizes, nblk(D), TPB, 0, b->d_docs, D, xt, n_a, n_b, n_c);
     run_scans(b, {ScanJob{(const u8*)n_a, (u8*)xt.xdoc + offsetof(XDoc, ob0), 4, sizeof(XDoc), D},
                   ScanJob{(const u8*)n_b, (u8*)xt.xdoc + offsetof(XDoc, scratch0), 4, sizeof(XDoc), D},
                   ScanJob{(const u8*)n_c, (u8*)xt.xdoc + offsetof(XDoc, stage0), 4, sizeof(XDoc), D}});
@@ -472,17 +491,16 @@ u8* export_encode(lb_batch* b, const BatchTables& xt, u64* total) {
     const char* cap_env = getenv("LB_EXPORT_STAGE_CAP");   // testing hook: smaller slots send blocks through the retry
     const u32 stage_max = cap_env ? (u32)strtoul(cap_env, nullptr, 10) : 0xFFFFFFFFu;
     trace_point(b, "store+sizes");
-    LB_LAUNCH(k_exp_list, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb, stage_max);
-    launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, xstage, 0);
-    LB_LAUNCH(k_exp_layout, nblk(D), TPB, 0, st, b->d_docs, D, xt, xb, n_a, n_b, n_c);
-    tm.kernel_launches += 3;
+    LB_BATCH_LAUNCH(b, k_exp_list, nblk(D), TPB, 0, b->d_docs, D, xt, xb, stage_max);
+    launch_exp_encode(b, NOB, xt, xb, xscratch, xstage, 0);
+    LB_BATCH_LAUNCH(b, k_exp_layout, nblk(D), TPB, 0, b->d_docs, D, xt, xb, n_a, n_b, n_c);
     trace_point(b, "encode");
     run_scans(b, {ScanJob{(const u8*)n_a, (u8*)xt.xdoc + offsetof(XDoc, exp_off), 4, sizeof(XDoc), D},
                   ScanJob{(const u8*)n_b, (u8*)xt.xdoc + offsetof(XDoc, ovf0), 4, sizeof(XDoc), D},
                   ScanJob{(const u8*)n_c, (u8*)xt.xdoc + offsetof(XDoc, restage0), 4, sizeof(XDoc), D}});
     xtot = d2h_one(b, xt.xdoc + D);
     const u64 XT = xtot.exp_off, NOVF = xtot.ovf0, NRST = xtot.restage0;
-    if (getenv("LB_PHASE_TRACE"))
+    if (phase_trace())
         fprintf(stderr, "[trace] export: %llu blocks, %llu outgrew their staging slot; %llu staging bytes for %llu exported\n",
                 (unsigned long long)NOB, (unsigned long long)NOVF, (unsigned long long)NSTG, (unsigned long long)XT);
     trace_point(b, "layout scan + size d2h");
@@ -491,11 +509,9 @@ u8* export_encode(lb_batch* b, const BatchTables& xt, u64* total) {
     u8* xrestage = nullptr;
     if (NOVF) {
         xrestage = dv.alloc<u8>(NRST + 16);
-        launch_exp_encode(st, b->d_docs, NOB, xt, xb, xscratch, xrestage, 1);
-        tm.kernel_launches += 1;
+        launch_exp_encode(b, NOB, xt, xb, xscratch, xrestage, 1);
     }
-    LB_LAUNCH(k_exp_finish, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, xt, xb, xstage, xrestage, out);
-    tm.kernel_launches += 1;
+    LB_BATCH_LAUNCH(b, k_exp_finish, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, xt, xb, xstage, xrestage, out);
     trace_point(b, "assemble");
     dv.release(cnt); dv.release(xb); dv.release(xscratch); dv.release(xstage); dv.release(xrestage);
     *total = XT;
@@ -508,7 +524,6 @@ void pipeline(lb_batch* b) {
     u32 D = (u32)b->n_docs;
     lb_timings& tm = b->timings;
     if (D == 0) {
-        for (int i = 0; i < 8; i++) mark(b);
         b->docs.resize(1);
         return;
     }
@@ -523,7 +538,7 @@ void pipeline(lb_batch* b) {
     u32* d_doc_blob0 = dv.alloc<u32>(D + 2);
     CK(cudaMemcpyAsync(d_blob_doc, b->blob_doc.data(), sizeof(u32) * Q, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_doc_blob0, b->doc_blob0.data(), sizeof(u32) * (D + 1), cudaMemcpyHostToDevice, st));
-    LB_LAUNCH(k_frame_count, nblk((u64)Q * 32, 128), 128, 0, st, t.bytes, b->d_offs, b->d_lens, Q, d_blob_code, d_blob_nblocks);
+    LB_BATCH_LAUNCH(b, k_frame_count, nblk((u64)Q * 32, 128), 128, 0, t.bytes, b->d_offs, b->d_lens, Q, d_blob_code, d_blob_nblocks);
     run_scans(b, {ScanJob{(const u8*)d_blob_nblocks, (u8*)d_blob_block0, 4, 8, Q}});
     u32* d_doc_nprior = nullptr;
     if (!b->doc_nprior.empty()) {
@@ -544,19 +559,16 @@ void pipeline(lb_batch* b) {
             CK(cudaMemcpyAsync(d_ck_ctr, b->ck_ctr.data(), sizeof(i32) * NF, cudaMemcpyHostToDevice, st));
         }
     }
-    LB_LAUNCH(k_frame_docs, nblk(D), TPB, 0, st, D, d_doc_blob0, d_blob_code, d_blob_block0, d_doc_nprior, b->d_docs);
-    tm.kernel_launches += 2;
+    LB_BATCH_LAUNCH(b, k_frame_docs, nblk(D), TPB, 0, D, d_doc_blob0, d_blob_code, d_blob_block0, d_doc_nprior, b->d_docs);
     u64 B = d2h_one(b, d_blob_block0 + Q);
     b->n_blocks = B;
     t.blocks = dv.alloc<BlockInfo>(B + 1, true);
-    LB_LAUNCH(k_frame_fill, nblk(Q), TPB, 0, st, t.bytes, b->d_offs, b->d_lens, Q, d_blob_doc, d_blob_code, d_blob_block0, d_doc_blob0, t.blocks);
-    tm.kernel_launches += 1;
-    mark(b);  // [1] frame done
+    LB_BATCH_LAUNCH(b, k_frame_fill, nblk(Q), TPB, 0, t.bytes, b->d_offs, b->d_lens, Q, d_blob_doc, d_blob_code, d_blob_block0, d_doc_blob0, t.blocks);
+    mark(b, EV_FRAME);
     // ------------------------------------------------------------ phase 2: decode
     BlockInfo* blk = t.blocks;
     if (B) {
-        LB_LAUNCH(k_block_count, nblk(B, 64), 64, 0, st, t.bytes, blk, B);
-        tm.kernel_launches += 1;
+        LB_BATCH_LAUNCH(b, k_block_count, nblk(B, 64), 64, 0, t.bytes, blk, B);
     }
     run_scans(b, {FIELD_JOB(blk, BlockInfo, n_peers, peer0, B), FIELD_JOB(blk, BlockInfo, n_keys, key0, B),
                   FIELD_JOB(blk, BlockInfo, n_cids, cid0, B), FIELD_JOB(blk, BlockInfo, n_changes, ch0, B),
@@ -600,18 +612,17 @@ void pipeline(lb_batch* b) {
         // (k_decode_warp.cuh); anything else, or nothing, a thread per block one column at a time (k_decode.cuh)
         static const char* mode_env = getenv("LB_DECODE");
         static const bool warp = mode_env && !strcmp(mode_env, "warp");
-        if (!warp) LB_LAUNCH(k_block_decode_cols, nblk(B, 64), 64, 0, st, t.bytes, blk, B, t);
+        if (!warp) LB_BATCH_LAUNCH(b, k_block_decode_cols, nblk(B, 64), 64, 0, t.bytes, blk, B, t);
         else {
             const size_t smem = sizeof(DwWarp) * DW_WARPS;
 #ifndef LB_SIMT_EMU
             static bool attr_set = false;
             if (!attr_set) { CK(cudaFuncSetAttribute(k_block_decode_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr_set = true; }
 #endif
-            LB_LAUNCH(k_block_decode_warp, nblk(B, DW_WARPS), 32 * DW_WARPS, smem, st, t.bytes, blk, B, t);
+            LB_BATCH_LAUNCH(b, k_block_decode_warp, nblk(B, DW_WARPS), 32 * DW_WARPS, smem, t.bytes, blk, B, t);
         }
-        tm.kernel_launches += 1;
     }
-    mark(b);  // [2] decode done
+    mark(b, EV_DECODE);
     // SURVEY 8d algorithmic bytes of decode: blob bytes read + SoA written
     tm.decode_bytes_written = NR * 13 + NCH * (4 + 4 + 8 + 4) + ND * 12;
     // ------------------------------------------------------------ phase 3: resolve
@@ -635,30 +646,27 @@ void pipeline(lb_batch* b) {
         t.head_lamport = dv.alloc<u32>(NP);
         d_pend_scratch = dv.alloc<i32>(2 * (u64)Q + 2);
     }
-    LB_LAUNCH(k_doc_tables, nblk(D, 64), 64, 0, st, t.bytes, b->d_docs, D, blk, t);
-    u32* d_tmp_a = dv.alloc<u32>(D + 1, true);
-    u32* d_tmp_b = dv.alloc<u32>(D + 1, true);
-    u32* d_tmp_c = dv.alloc<u32>(D + 1, true);
-    LB_LAUNCH(k_doc_sizes, nblk(D), TPB, 0, st, b->d_docs, D, d_tmp_a, d_tmp_b, d_tmp_c, 0);
-    tm.kernel_launches += 2;
-    run_scans(b, {ScanJob{(const u8*)d_tmp_a, (u8*)b->d_docs + offsetof(DocInfo, vv0), 4, sizeof(DocInfo), D}});
+    LB_BATCH_LAUNCH(b, k_doc_tables, nblk(D, 64), 64, 0, t.bytes, b->d_docs, D, blk, t);
+    u32* d_vv_cells = dv.alloc<u32>(D + 1);
+    LB_BATCH_LAUNCH(b, k_doc_vv_cells, nblk(D), TPB, 0, b->d_docs, D, d_vv_cells);
+    run_scans(b, {ScanJob{(const u8*)d_vv_cells, (u8*)b->d_docs + offsetof(DocInfo, vv0), 4, sizeof(DocInfo), D}});
     u64 VV = d2h_one(b, &b->d_docs[D].vv0);
     t.ch_vv = dv.alloc<i32>(VV);
     u32* d_cursor = dv.alloc<u32>(NP);
-    LB_LAUNCH(k_doc_causal, nblk(D, 64), 64, 0, st, b->d_docs, D, blk, t, d_cursor, d_doc_blob0, d_pend_scratch);
-    LB_LAUNCH(k_doc_frontiers, nblk(D, 64), 64, 0, st, b->d_docs, D, t);
+    LB_BATCH_LAUNCH(b, k_doc_causal, nblk(D, 64), 64, 0, b->d_docs, D, blk, t, d_cursor, d_doc_blob0, d_pend_scratch);
+    LB_BATCH_LAUNCH(b, k_doc_frontiers, nblk(D, 64), 64, 0, b->d_docs, D, t);
     if (d_ck_range) {
         t.ck_end = dv.alloc<i32>(NP + 1);
-        LB_LAUNCH(k_doc_checkout, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, t, d_ck_range, d_ck_peer, d_ck_ctr);
-        tm.kernel_launches += 1;
+        LB_BATCH_LAUNCH(b, k_doc_checkout, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t, d_ck_range, d_ck_peer, d_ck_ctr);
     }
-    LB_LAUNCH(k_doc_sizes, nblk(D), TPB, 0, st, b->d_docs, D, d_tmp_a, d_tmp_b, d_tmp_c, 1);
-    tm.kernel_launches += 3;
-    run_scans(b, {ScanJob{(const u8*)d_tmp_b, (u8*)b->d_docs + offsetof(DocInfo, atom0), 4, sizeof(DocInfo), D},
-                  ScanJob{(const u8*)d_tmp_c, (u8*)b->d_docs + offsetof(DocInfo, mapslot0), 4, sizeof(DocInfo), D}});
+    u32* d_atoms = dv.alloc<u32>(D + 1);
+    u32* d_mapslots = dv.alloc<u32>(D + 1);
+    LB_BATCH_LAUNCH(b, k_doc_atoms_mapslots, nblk(D), TPB, 0, b->d_docs, D, d_atoms, d_mapslots);
+    run_scans(b, {ScanJob{(const u8*)d_atoms, (u8*)b->d_docs + offsetof(DocInfo, atom0), 4, sizeof(DocInfo), D},
+                  ScanJob{(const u8*)d_mapslots, (u8*)b->d_docs + offsetof(DocInfo, mapslot0), 4, sizeof(DocInfo), D}});
     DocInfo dtot = d2h_one(b, &b->d_docs[D]);
     u64 NATOM = dtot.atom0, NSLOT = dtot.mapslot0;
-    mark(b);  // [3] resolve done
+    mark(b, EV_RESOLVE);
     // ------------------------------------------------------------ phase 4: classify + map LWW
     t.tr_rec = dv.alloc<uint4>(NTR); t.tr_key = dv.alloc<u64>(NTR); t.tr_ids = dv.alloc<uint4>(NTR);
     t.op_kind = dv.alloc<u8>(NR); t.op_cidx = dv.alloc<u32>(NR); t.op_lamport = dv.alloc<u32>(NR);
@@ -667,9 +675,8 @@ void pipeline(lb_batch* b) {
     t.map_best = dv.alloc<unsigned long long>(NSLOT, true);
     t.map_row = dv.alloc<u32>(NSLOT);
     if (NR) {
-        LB_LAUNCH(k_op_classify, nblk(NR, 256), 256, 0, st, b->d_docs, NR, t);
-        LB_LAUNCH(k_map_winner, nblk(NR, 256), 256, 0, st, b->d_docs, NR, t);
-        tm.kernel_launches += 2;
+        LB_BATCH_LAUNCH(b, k_op_classify, nblk(NR, 256), 256, 0, b->d_docs, NR, t);
+        LB_BATCH_LAUNCH(b, k_map_winner, nblk(NR, 256), 256, 0, b->d_docs, NR, t);
     }
     // capacities -> pools
     u32* cap_leaf = dv.alloc<u32>(NC + 1, true);
@@ -678,8 +685,7 @@ void pipeline(lb_batch* b) {
     u32* cap_cvv = dv.alloc<u32>(NC + 1, true);
     u32* span_cap = dv.alloc<u32>(D + 1, true);
     const u32 leaf_w = 32;   // slots per leaf = lanes per warp (k_seq.cuh)
-    LB_LAUNCH(k_container_caps, nblk(D), TPB, 0, st, b->d_docs, D, t.dcont, cap_leaf, cap_node, cap_out, cap_cvv, span_cap, leaf_w);
-    tm.kernel_launches += 1;
+    LB_BATCH_LAUNCH(b, k_container_caps, nblk(D), TPB, 0, b->d_docs, D, t.dcont, cap_leaf, cap_node, cap_out, cap_cvv, span_cap, leaf_w);
     run_scans(b, {ScanJob{(const u8*)cap_leaf, (u8*)t.dcont + offsetof(DocContainer, leaf0), 4, sizeof(DocContainer), NC},
                   ScanJob{(const u8*)cap_node, (u8*)t.dcont + offsetof(DocContainer, node0), 4, sizeof(DocContainer), NC},
                   ScanJob{(const u8*)cap_out, (u8*)t.dcont + offsetof(DocContainer, out0), 4, sizeof(DocContainer), NC},
@@ -687,7 +693,7 @@ void pipeline(lb_batch* b) {
                   ScanJob{(const u8*)span_cap, (u8*)b->d_docs + offsetof(DocInfo, span0), 4, sizeof(DocInfo), D}});
     DocContainer ctot = d2h_one(b, t.dcont + NC);
     u64 NLEAF = ctot.leaf0, NNODE = ctot.node0, NOUT = ctot.out0, NCVV = ctot.cvv0;
-    mark(b);  // [4] classify done
+    mark(b, EV_CLASSIFY);
     // ------------------------------------------------------------ phase 5: sequence integration
     SeqPools sp;
     memset(&sp, 0, sizeof(sp));
@@ -702,21 +708,21 @@ void pipeline(lb_batch* b) {
     sp.next_doc = dv.alloc<u32>(1, true);
     t.out_row = dv.alloc<u32>(NOUT); t.out_off = dv.alloc<u32>(NOUT); t.out_len = dv.alloc<u32>(NOUT);
     const unsigned seq_ctas = seq_resident_ctas(b->device);
-    if (nblk(D, LB_SEQ_WARPS) > seq_ctas) LB_LAUNCH(k_seq_integrate<1>, seq_ctas, 32 * LB_SEQ_WARPS, 0, st, b->d_docs, D, sp, t);
-    else LB_LAUNCH(k_seq_integrate<0>, nblk(D, LB_SEQ_WARPS), 32 * LB_SEQ_WARPS, 0, st, b->d_docs, D, sp, t);
-    tm.kernel_launches += 1;
+    if (nblk(D, LB_SEQ_WARPS) > seq_ctas) LB_BATCH_LAUNCH(b, k_seq_integrate<1>, seq_ctas, 32 * LB_SEQ_WARPS, 0, b->d_docs, D, sp, t);
+    else LB_BATCH_LAUNCH(b, k_seq_integrate<0>, nblk(D, LB_SEQ_WARPS), 32 * LB_SEQ_WARPS, 0, b->d_docs, D, sp, t);
     if (!(b->flags & LB_FLAG_KEEP_DEVICE)) {   // the tracker pools are the largest tables of the batch: free them early
         dv.release(sp.leaf); dv.release(sp.node); dv.release(sp.node_parent); dv.release(sp.atom_leaf); dv.release(sp.a_org);
         dv.release(sp.cvv); dv.release(sp.cont_epoch); dv.release(sp.next_doc); dv.release(t.atom_row); dv.release(t.op_rec);
     }
-    mark(b);  // [5] list/text integration done
+    mark(b, EV_INTEGRATE);
     // ------------------------------------------------------------ phase 5b: movable trees
     if (NTR) {
-        CK(cudaMemsetAsync(d_tmp_b + D, 0, sizeof(u32), st));
-        LB_LAUNCH(k_doc_sizes, nblk(D), TPB, 0, st, b->d_docs, D, d_tmp_a, d_tmp_b, d_tmp_c, 2);
-        run_scans(b, {ScanJob{(const u8*)d_tmp_a, (u8*)b->d_docs + offsetof(DocInfo, tree0), 4, sizeof(DocInfo), D}});
+        u32* d_tree_slots = dv.alloc<u32>(D + 1);
+        u32* d_max_tree_atoms = dv.alloc<u32>(1, true);
+        LB_BATCH_LAUNCH(b, k_doc_tree_slots, nblk(D), TPB, 0, b->d_docs, D, d_tree_slots, d_max_tree_atoms);
+        run_scans(b, {ScanJob{(const u8*)d_tree_slots, (u8*)b->d_docs + offsetof(DocInfo, tree0), 4, sizeof(DocInfo), D}});
         u64 NTS = d2h_one(b, &b->d_docs[D].tree0);
-        const u32 max_atoms = d2h_one(b, d_tmp_b + D);
+        const u32 max_atoms = d2h_one(b, d_max_tree_atoms);
         t.ts_key = dv.alloc<u64>(NTR); t.ts_val = dv.alloc<u32>(NTR); t.ts_rec = dv.alloc<uint4>(NTR);
         t.tn_parent = dv.alloc<u32>(NTS); t.tn_move = dv.alloc<u32>(NTS); t.tn_base = dv.alloc<u32>(NTS);
         t.tn_cnt = dv.alloc<u32>(NTS); t.tn_sib = dv.alloc<u32>(NTS); t.ns_key = dv.alloc<u64>(NTS);
@@ -730,35 +736,32 @@ void pipeline(lb_batch* b) {
 #ifndef LB_SIMT_EMU
         CK(cudaFuncSetAttribute(k_tree_apply, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tree_smem));
         CK(cudaFuncSetAttribute(k_tree_apply, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-        if (getenv("LB_PHASE_TRACE")) {
+        if (phase_trace()) {
             int nb = 0;
             cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_tree_apply, 32 * TREE_WARPS, tree_smem);
             fprintf(stderr, "[trace] k_tree_apply: %zu bytes of shared memory per document, %d documents resident per SM\n", tree_smem, nb);
         }
 #endif
-        LB_LAUNCH(k_tree_sort, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, t);
-        LB_LAUNCH(k_tree_apply, nblk((u64)D * 32, 32 * TREE_WARPS), 32 * TREE_WARPS, tree_smem, st, b->d_docs, D, t, s_nodes);
-        LB_LAUNCH(k_tree_layout, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, t);
-        tm.kernel_launches += 4;
+        LB_BATCH_LAUNCH(b, k_tree_sort, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t);
+        LB_BATCH_LAUNCH(b, k_tree_apply, nblk((u64)D * 32, 32 * TREE_WARPS), 32 * TREE_WARPS, tree_smem, b->d_docs, D, t, s_nodes);
+        LB_BATCH_LAUNCH(b, k_tree_layout, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t);
     }
-    mark(b);  // [5b] trees done
+    mark(b, EV_TREE);
     tm.tree_ops = NTR;
     // ------------------------------------------------------------ phase 6: JSON
     unsigned long long* d_acc = dv.alloc<unsigned long long>(4, true);
     if (!(b->flags & LB_FLAG_NO_JSON)) {
-        LB_LAUNCH(k_json, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, t, (u8*)nullptr, 0);
-        LB_LAUNCH(k_json_padlen, nblk(D), TPB, 0, st, b->d_docs, D, d_tmp_a);
-        tm.kernel_launches += 2;
-        run_scans(b, {ScanJob{(const u8*)d_tmp_a, (u8*)b->d_docs + offsetof(DocInfo, json_off), 4, sizeof(DocInfo), D}});
+        LB_BATCH_LAUNCH(b, k_json, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t, (u8*)nullptr, 0);
+        u32* d_json_padded = dv.alloc<u32>(D + 1);
+        LB_BATCH_LAUNCH(b, k_json_padlen, nblk(D), TPB, 0, b->d_docs, D, d_json_padded);
+        run_scans(b, {ScanJob{(const u8*)d_json_padded, (u8*)b->d_docs + offsetof(DocInfo, json_off), 4, sizeof(DocInfo), D}});
         u64 JT = d2h_one(b, &b->d_docs[D].json_off);
         b->json_total = JT;
         b->d_json = dv.alloc<u8>(JT + 16, true);
-        LB_LAUNCH(k_json, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, t, b->d_json, 1);
-        tm.kernel_launches += 1;
+        LB_BATCH_LAUNCH(b, k_json, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t, b->d_json, 1);
     }
-    LB_LAUNCH(k_doc_hash, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, (const u8*)b->d_json, d_acc);
-    tm.kernel_launches += 1;
-    mark(b);  // [6] materialise done
+    LB_BATCH_LAUNCH(b, k_doc_hash, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, (const u8*)b->d_json, d_acc);
+    mark(b, EV_MATERIALISE);
     if (b->eager_json && b->json_total && !(b->flags & LB_FLAG_NO_JSON)) {
         CK(cudaStreamCreate(&b->stream2));
         CK(cudaEventCreate(&b->json_ev));
@@ -792,23 +795,27 @@ void pipeline(lb_batch* b) {
         // extras are counted by pass 0, so the arrays are sized with a bound first and checked after the scan
         u64 SEGCAP = NCH + NCH / 4 + 1024;
         if (getenv("LB_EXPORT_TIGHT_SEGCAP")) SEGCAP = NCH;   // testing hook: force the growth path
-        t.sg_src = dv.alloc<u32>(SEGCAP); t.sg_r0 = dv.alloc<u32>(SEGCAP); t.sg_from = dv.alloc<u32>(SEGCAP);
-        t.sg_atoms = dv.alloc<u32>(SEGCAP); t.sg_est = dv.alloc<u32>(SEGCAP); t.sg_nmops = dv.alloc<u32>(SEGCAP);
-        t.sg_ndel = dv.alloc<u32>(SEGCAP); t.sg_nrows = dv.alloc<u32>(SEGCAP); t.sg_last_head = dv.alloc<u32>(SEGCAP);
-        t.sg_skip = dv.alloc<u32>(SEGCAP, true);
-        t.fc_src = dv.alloc<u32>(SEGCAP); t.fc_pos = dv.alloc<u32>(SEGCAP); t.fc_r0 = dv.alloc<u32>(SEGCAP);
-        t.fc_from = dv.alloc<u32>(SEGCAP); t.fc_atoms = dv.alloc<u32>(SEGCAP); t.fc_nrows = dv.alloc<u32>(SEGCAP);
-        t.fc_ndel = dv.alloc<u32>(SEGCAP); t.fc_block = dv.alloc<u8>(SEGCAP); t.fc_skip = dv.alloc<u32>(SEGCAP, true);
-        t.fc_est = dv.alloc<u32>(SEGCAP);
+        // the u32 tables of the two groups, in allocation order, for here and for the growth path below; the *_skip
+        // tables start zeroed, and fc_block (the one byte-wide table) has its place before fc_skip
+        static u32* BatchTables::* const SG_TABLES[] = {
+            &BatchTables::sg_src, &BatchTables::sg_r0, &BatchTables::sg_from, &BatchTables::sg_atoms, &BatchTables::sg_est,
+            &BatchTables::sg_nmops, &BatchTables::sg_ndel, &BatchTables::sg_nrows, &BatchTables::sg_last_head, &BatchTables::sg_skip};
+        static u32* BatchTables::* const FC_TABLES[] = {
+            &BatchTables::fc_src, &BatchTables::fc_pos, &BatchTables::fc_r0, &BatchTables::fc_from, &BatchTables::fc_atoms,
+            &BatchTables::fc_nrows, &BatchTables::fc_ndel, &BatchTables::fc_skip, &BatchTables::fc_est};
+        for (auto m : SG_TABLES) t.*m = dv.alloc<u32>(SEGCAP, m == &BatchTables::sg_skip);
+        for (auto m : FC_TABLES) {
+            if (m == &BatchTables::fc_skip) t.fc_block = dv.alloc<u8>(SEGCAP);
+            t.*m = dv.alloc<u32>(SEGCAP, m == &BatchTables::fc_skip);
+        }
         t.only_doc = 0xFFFFFFFFu; t.from_ctr = nullptr;
         trace_point(b, "export allocs");
-        LB_LAUNCH(k_exp_init, nblk(D), TPB, 0, st, b->d_docs, D, t);
-        if (NTR) { LB_LAUNCH(k_exp_posrank, nblk((u64)D * 32, 128), 128, 0, st, b->d_docs, D, t); tm.kernel_launches += 1; }
-        if (NCH) LB_LAUNCH(k_exp_arena, nblk(NCH, 64), 64, 0, st, NCH, t, b->d_docs);
+        LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, t);
+        if (NTR) LB_BATCH_LAUNCH(b, k_exp_posrank, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t);
+        if (NCH) LB_BATCH_LAUNCH(b, k_exp_arena, nblk(NCH, 64), 64, 0, NCH, t, b->d_docs);
         run_scans(b, {ScanJob{(const u8*)t.ch_aval, (u8*)t.ch_aval0, 4, 8, NCH}, ScanJob{(const u8*)t.ch_astr, (u8*)t.ch_astr0, 4, 8, NCH}});
         trace_point(b, "posrank+arena");
-        if (NCH) LB_LAUNCH(k_exp_changes, nblk(NCH, 64), 64, 0, st, b->d_docs, NCH, t, 0);
-        tm.kernel_launches += 3;
+        if (NCH) LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, t, 0);
         trace_point(b, "changes pass 0");
         run_scans(b, {ScanJob{(const u8*)t.ch_novf, (u8*)t.ch_seg0, 4, 8, NCH}, ScanJob{(const u8*)t.ch_syn, (u8*)t.ch_syn0, 4, 8, NCH}});
         u64 NOVF = d2h_one(b, t.ch_seg0 + NCH);
@@ -818,27 +825,24 @@ void pipeline(lb_batch* b) {
         t.s_flag = dv.alloc<u8>(NSYN); t.s_voff = dv.alloc<u64>(NSYN); t.s_vlen = dv.alloc<u32>(NSYN); t.s_aux = dv.alloc<u32>(NSYN);
         if (NCH + NOVF > SEGCAP) {   // unusually many split changes: grow the tables, keep what pass 0 wrote
             u64 cap = NCH + NOVF;
-            u32** sgs[10] = {&t.sg_src, &t.sg_r0, &t.sg_from, &t.sg_atoms, &t.sg_est, &t.sg_nmops, &t.sg_ndel, &t.sg_nrows, &t.sg_last_head, &t.sg_skip};
-            for (auto pp : sgs) {
+            for (auto m : SG_TABLES) {
                 u32* nw = dv.alloc<u32>(cap);
-                CK(cudaMemcpyAsync(nw, *pp, sizeof(u32) * NCH, cudaMemcpyDeviceToDevice, st));
-                dv.release(*pp);
-                *pp = nw;
+                CK(cudaMemcpyAsync(nw, t.*m, sizeof(u32) * NCH, cudaMemcpyDeviceToDevice, st));
+                dv.release(t.*m);
+                t.*m = nw;
             }
-            u32** fcs[9] = {&t.fc_src, &t.fc_pos, &t.fc_r0, &t.fc_from, &t.fc_atoms, &t.fc_nrows, &t.fc_ndel, &t.fc_skip, &t.fc_est};
-            for (auto pp : fcs) { dv.release(*pp); *pp = dv.alloc<u32>(cap, true); }
+            for (auto m : FC_TABLES) { dv.release(t.*m); t.*m = dv.alloc<u32>(cap, true); }
             dv.release(t.fc_block);
             t.fc_block = dv.alloc<u8>(cap);
         }
-        if (NOVF) { LB_LAUNCH(k_exp_changes, nblk(NCH, 64), 64, 0, st, b->d_docs, NCH, t, 1); tm.kernel_launches += 1; }
-        LB_LAUNCH(k_exp_store, nblk(D, 64), 64, 0, st, b->d_docs, D, t);
-        tm.kernel_launches += 1;
+        if (NOVF) LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, t, 1);
+        LB_BATCH_LAUNCH(b, k_exp_store, nblk(D, 64), 64, 0, b->d_docs, D, t);
         u64 XT = 0;
         b->d_export = export_encode(b, t, &XT);
         b->export_total = XT;
         tm.export_bytes = XT;
     }
-    mark(b);  // [7] export done
+    mark(b, EV_EXPORT);
     // ------------------------------------------------------------ results to host
     b->t_tail = std::chrono::steady_clock::now();
     b->docs.resize(D + 1);
@@ -863,12 +867,11 @@ void pipeline(lb_batch* b) {
             u64* d_pbase = dv.alloc<u64>(D + 1);
             DocPeer* d_packed = dv.alloc<DocPeer>(total);
             CK(cudaMemcpyAsync(d_pbase, b->peer_base.data(), sizeof(u64) * (D + 1), cudaMemcpyHostToDevice, st));
-            LB_LAUNCH(k_pack_peers, nblk(D), TPB, 0, st, b->d_docs, D, t.dpeer, d_pbase, d_packed);
-            tm.kernel_launches += 1;
+            LB_BATCH_LAUNCH(b, k_pack_peers, nblk(D), TPB, 0, b->d_docs, D, t.dpeer, d_pbase, d_packed);
             CK(cudaMemcpyAsync(b->dpeer.data(), d_packed, sizeof(DocPeer) * total, cudaMemcpyDeviceToHost, st));
         }
     }
-    mark(b);  // [8] d2h queued
+    mark(b, EV_D2H);   // the result copies are queued
     CK(cudaStreamSynchronize(st));
     lb_counters& c = b->counters;
     c.docs = D;
@@ -909,23 +912,23 @@ void build_status(lb_batch* b) {
 }
 
 void timings_from_events(lb_batch* b) {
-    auto el = [&](int a, int c) {
+    auto el = [&](BatchEvent a, BatchEvent c) {   // 0 when either end was not recorded (the empty batch)
         float ms = 0;
-        if (a < b->n_ev && c < b->n_ev) cudaEventElapsedTime(&ms, b->ev[a], b->ev[c]);
+        if (b->ev_recorded[a] && b->ev_recorded[c]) cudaEventElapsedTime(&ms, b->ev[a], b->ev[c]);
         return ms;
     };
     lb_timings& t = b->timings;
-    t.h2d = el(0, 1);
-    t.frame = el(1, 2);
-    t.decode = el(2, 3);
-    t.resolve = el(3, 4);
-    t.classify = el(4, 5);
-    t.integrate = el(5, 6);
-    t.tree = el(6, 7);
-    t.materialise = el(7, 8);
-    t.reexport = el(8, 9);
-    t.d2h = el(9, 10);
-    t.total_device = el(1, 9);
+    t.h2d = el(EV_START, EV_H2D);
+    t.frame = el(EV_H2D, EV_FRAME);
+    t.decode = el(EV_FRAME, EV_DECODE);
+    t.resolve = el(EV_DECODE, EV_RESOLVE);
+    t.classify = el(EV_RESOLVE, EV_CLASSIFY);
+    t.integrate = el(EV_CLASSIFY, EV_INTEGRATE);
+    t.tree = el(EV_INTEGRATE, EV_TREE);
+    t.materialise = el(EV_TREE, EV_MATERIALISE);
+    t.reexport = el(EV_MATERIALISE, EV_EXPORT);
+    t.d2h = el(EV_EXPORT, EV_D2H);
+    t.total_device = el(EV_H2D, EV_EXPORT);
 }
 
 lb_status run_batch(lb_batch* b) {
@@ -996,12 +999,41 @@ lb_status check_device(const lb_options* opt) {
     return LB_OK;
 }
 
-void init_batch(lb_batch* b) {
-    b->dev.device = b->device;
-    b->dev.stream = stream_take(b->device);
-    if (!b->dev.stream) { g_last_error = "cudaStreamCreate failed"; throw lb_status(LB_ERR_CUDA); }
-    for (int i = 0; i < 16; i++) CK(cudaEventCreate(&b->ev[i]));
-    b->ev_created = true;
+// What every import entry point does around its own part: the device check, a batch with its stream and events, then
+// `fill` (it builds the blob list, ends in upload_and_run and returns a status or throws one), and the one place where a
+// failed batch is freed and a good one handed out.
+template <class Fill>
+lb_status import_with_new_batch(const lb_options* opt, lb_batch** out, Fill fill) {
+    lb_status s = check_device(opt);
+    if (s != LB_OK) return s;
+    lb_batch* b = new lb_batch();
+    b->flags = opt ? opt->flags : 0;
+    b->device = b->dev.device = opt ? opt->device : 0;
+    try {
+        b->dev.stream = stream_take(b->device);
+        if (!b->dev.stream) { g_last_error = "cudaStreamCreate failed"; throw lb_status(LB_ERR_CUDA); }
+        for (cudaEvent_t& e : b->ev) CK(cudaEventCreate(&e));
+        b->ev_created = true;
+        s = fill(b);
+    } catch (lb_status e) {
+        s = e;
+    }
+    if (s != LB_OK) { lb_batch_free(b); return s; }
+    *out = b;
+    return LB_OK;
+}
+
+// The blob table (offsets and lengths into `d_bytes`, already on the device) goes up, then the pipeline runs.
+lb_status upload_and_run(lb_batch* b, const std::vector<u64>& offs, const std::vector<u32>& lens, const u8* d_bytes) {
+    const size_t Q = b->n_blobs;
+    b->d_offs = b->dev.alloc<u64>(Q + 1);
+    b->d_lens = b->dev.alloc<u32>(Q + 1);
+    CK(cudaMemcpyAsync(b->d_offs, offs.data(), sizeof(u64) * (Q + 1), cudaMemcpyHostToDevice, b->dev.stream));
+    CK(cudaMemcpyAsync(b->d_lens, lens.data(), sizeof(u32) * (Q + 1), cudaMemcpyHostToDevice, b->dev.stream));
+    b->tb.bytes = d_bytes;
+    b->timings.decode_bytes_read = b->counters.blob_bytes;
+    mark(b, EV_H2D);
+    return run_batch(b);
 }
 
 // export(ExportMode::updates(from)) of one document (encoding.rs:79-83 ; change_store.rs:494-528 export_blocks_from):
@@ -1028,12 +1060,12 @@ lb_status export_from(lb_batch* b, size_t doc, const lb_id_span* from, size_t n_
         xt.only_doc = (u32)doc;
         XDoc* xdoc = dv.alloc<XDoc>(D + 1, true);
         xt.xdoc = xdoc;
-        LB_LAUNCH(k_exp_init, nblk(D), TPB, 0, st, b->d_docs, D, xt);
+        LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, xt);
         if (NCH) {
-            LB_LAUNCH(k_exp_changes, nblk(NCH, 64), 64, 0, st, b->d_docs, NCH, xt, 0);
-            LB_LAUNCH(k_exp_changes, nblk(NCH, 64), 64, 0, st, b->d_docs, NCH, xt, 1);
+            LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 0);
+            LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 1);
         }
-        LB_LAUNCH(k_exp_store, nblk(D, 64), 64, 0, st, b->d_docs, D, xt);
+        LB_BATCH_LAUNCH(b, k_exp_store, nblk(D, 64), 64, 0, b->d_docs, D, xt);
         u64 XT = 0;
         u8* d_out = export_encode(b, xt, &XT);
         XDoc x = d2h_one(b, xdoc + doc);
@@ -1100,7 +1132,7 @@ void docset_store(lb_docset* set, lb_batch* b, const std::vector<u64>& offs, con
     }
     CopySeg* d_segs = b->dev.alloc<CopySeg>(segs.size());
     CK(cudaMemcpyAsync(d_segs, segs.data(), sizeof(CopySeg) * segs.size(), cudaMemcpyHostToDevice, b->dev.stream));
-    LB_LAUNCH(k_copy_segments, nblk((u64)segs.size() * 32, 128), 128, 0, b->dev.stream, d_segs, (u32)segs.size());
+    LB_BATCH_LAUNCH(b, k_copy_segments, nblk((u64)segs.size() * 32, 128), 128, 0, d_segs, (u32)segs.size());
     CK(cudaStreamSynchronize(b->dev.stream));
     for (auto& kv : fresh) {
         DocsetDoc& slot = set->docs[kv.first];
@@ -1134,16 +1166,9 @@ static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_vers
     }
     if (set) o2.device = set->device;
     if (set && !set_checkout) o2.flags |= LB_FLAG_EXPORT;   // the re-export is what a stored document keeps
-    lb_status s = check_device(&o2);
-    if (s != LB_OK) return s;
-    if (n_blobs >= 0x7FFFFFFFull) { g_last_error = "too many blobs"; return LB_ERR_INVALID_ARG; }
-    lb_batch* b = new lb_batch();
-    b->n_docs = n_blobs;
-    b->flags = o2.flags;
-    b->device = o2.device;
-    b->eager_json = true;   // host buffers in, host results expected
-    try {
-        init_batch(b);
+    return import_with_new_batch(&o2, out, [&](lb_batch* b) {
+        if (n_blobs >= 0x7FFFFFFFull) { g_last_error = "too many blobs"; throw lb_status(LB_ERR_INVALID_ARG); }
+        b->eager_json = true;   // host buffers in, host results expected
         // blobs with the same doc_id form one document (LoroDoc::import_batch); documents are numbered in order of
         // first appearance and their blobs laid out consecutively, in the order given
         std::vector<u32> order(n_blobs);
@@ -1270,36 +1295,24 @@ static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_vers
         view_offs.push_back(total);
         total = ptotal;
         // stage through the pinned ring: host gather of slot k overlaps the DMA of slot k-1 (host_stage.hpp)
-        CK(cudaEventRecord(b->ev[b->n_ev++], b->dev.stream));  // [0]
+        mark(b, EV_START);
         u8* d_bytes = b->dev.alloc<u8>(total + 64);
-        b->d_offs = b->dev.alloc<u64>(Q + 1);
-        b->d_lens = b->dev.alloc<u32>(Q + 1);
         if (!segs.empty()) {
             for (size_t k = 0; k < segs.size(); k++) segs[k].dst = d_bytes + seg_offs[k];
             CopySeg* d_segs = b->dev.alloc<CopySeg>(segs.size());
             CK(cudaMemcpyAsync(d_segs, segs.data(), sizeof(CopySeg) * segs.size(), cudaMemcpyHostToDevice, b->dev.stream));
-            LB_LAUNCH(k_copy_segments, nblk((u64)segs.size() * 32, 128), 128, 0, b->dev.stream, d_segs, (u32)segs.size());
+            LB_BATCH_LAUNCH(b, k_copy_segments, nblk((u64)segs.size() * 32, 128), 128, 0, d_segs, (u32)segs.size());
             CK(cudaStreamSynchronize(b->dev.stream));   // `segs` is pageable host memory
         }
         if (!views.empty() && !lbstage::upload_blobs(views.data(), view_offs.data(), views.size(), d_bytes, b->dev.stream)) {
             g_last_error = "h2d staging failed";
             throw lb_status(LB_ERR_CUDA);
         }
-        CK(cudaMemcpyAsync(b->d_offs, offs.data(), sizeof(u64) * (Q + 1), cudaMemcpyHostToDevice, b->dev.stream));
-        CK(cudaMemcpyAsync(b->d_lens, lens.data(), sizeof(u32) * (Q + 1), cudaMemcpyHostToDevice, b->dev.stream));
-        b->tb.bytes = d_bytes;
-        b->timings.decode_bytes_read = b->counters.blob_bytes;
-        mark(b);  // [1] h2d done (index 0 = start)
-        // event indices: 0 start,1 h2d,2 frame,3 decode,4 resolve,5 classify,6 integrate,7 materialise,8 d2h
-        s = run_batch(b);
+        lb_status s = upload_and_run(b, offs, lens, d_bytes);
         CK(cudaStreamSynchronize(b->dev.stream));
         if (s == LB_OK && set && !set_checkout) docset_store(set, b, offs, lens);
-    } catch (lb_status e) {
-        s = e;
-    }
-    if (s != LB_OK) { lb_batch_free(b); return s; }
-    *out = b;
-    return LB_OK;
+        return s;
+    });
 }
 
 lb_status lb_import_batch(const lb_blob* blobs, size_t n_blobs, const lb_options* opt, lb_batch** out) {
@@ -1344,14 +1357,8 @@ lb_status lb_import_batch_device(const uint8_t* d_bytes, const uint64_t* offsets
                                  size_t n_docs, const lb_options* opt, lb_batch** out) {
     if (!out || ((!offsets || !blob_lens || !d_bytes) && n_docs)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
     *out = nullptr;
-    lb_status s = check_device(opt);
-    if (s != LB_OK) return s;
-    lb_batch* b = new lb_batch();
-    b->n_docs = n_docs;
-    b->flags = opt ? opt->flags : 0;
-    b->device = opt ? opt->device : 0;
-    try {
-        init_batch(b);
+    return import_with_new_batch(opt, out, [&](lb_batch* b) {
+        b->n_docs = n_docs;
         std::vector<u64> offs(n_docs + 1);
         std::vector<u32> lens(n_docs + 1, 0);
         for (size_t i = 0; i < n_docs; i++) {
@@ -1366,21 +1373,9 @@ lb_status lb_import_batch_device(const uint8_t* d_bytes, const uint64_t* offsets
         offs[n_docs] = n_docs ? offsets[n_docs - 1] + lens[n_docs - 1] : 0;
         b->doc_blob0.push_back((u32)n_docs);
         b->n_blobs = n_docs;
-        CK(cudaEventRecord(b->ev[b->n_ev++], b->dev.stream));  // [0]
-        b->d_offs = b->dev.alloc<u64>(n_docs + 1);
-        b->d_lens = b->dev.alloc<u32>(n_docs + 1);
-        CK(cudaMemcpyAsync(b->d_offs, offs.data(), sizeof(u64) * (n_docs + 1), cudaMemcpyHostToDevice, b->dev.stream));
-        CK(cudaMemcpyAsync(b->d_lens, lens.data(), sizeof(u32) * (n_docs + 1), cudaMemcpyHostToDevice, b->dev.stream));
-        b->tb.bytes = d_bytes;
-        b->timings.decode_bytes_read = b->counters.blob_bytes;
-        mark(b);  // [1]
-        s = run_batch(b);
-    } catch (lb_status e) {
-        s = e;
-    }
-    if (s != LB_OK) { lb_batch_free(b); return s; }
-    *out = b;
-    return LB_OK;
+        mark(b, EV_START);
+        return upload_and_run(b, offs, lens, d_bytes);
+    });
 }
 
 size_t lb_doc_count(const lb_batch* b) { return b ? b->n_docs : 0; }
@@ -1524,7 +1519,7 @@ void lb_batch_free(lb_batch* b) {
     b->dev.free_all();
     if (b->ev_created) {   // the stream exists whenever the events do (init_batch)
         cudaStreamSynchronize(b->dev.stream);
-        for (int i = 0; i < 16; i++) cudaEventDestroy(b->ev[i]);
+        for (cudaEvent_t e : b->ev) cudaEventDestroy(e);
         stream_give(b->device, b->dev.stream);
     }
     lbstage::host_cache().give(b->json);

@@ -111,6 +111,18 @@ def test_export_inserts_larger_than_a_block():
     check_export_against_oracle(big_insert_documents(), lib_path=EMU)
 
 
+def test_export_regrows_the_segment_tables(monkeypatch, golden_dir):
+    """LB_EXPORT_TIGHT_SEGCAP sizes the segment / final-change tables for one segment per change: every workload whose
+    changes enter the store in several segments then takes the path that grows them after pass 0."""
+    import gzip
+    from loro_b200.workload import C3Batch
+    monkeypatch.setenv("LB_EXPORT_TIGHT_SEGCAP", "1")
+    check_export_against_oracle(big_insert_documents(), lib_path=EMU)
+    blobs = C3Batch(2, n_ops=10000, threads=2).blobs()
+    blobs.append(gzip.open(os.path.join(golden_dir, "automerge_trace_blob.bin.gz"), "rb").read())
+    check_export_against_oracle(blobs, lib_path=EMU, reimport=False)
+
+
 def test_export_with_pending_changes_and_after_import_batch():
     """Pending changes stay out of the export but their payloads still moved the arenas; a document built from
     several blobs is exported as the reference would after import_batch (blobs sorted by change count first)."""
