@@ -17,11 +17,13 @@
  *   lb_doc_frontiers         crates/loro/src/lib.rs:881  LoroDoc::oplog_frontiers()
  *   lb_doc_export_updates    crates/loro/src/lib.rs:1235 LoroDoc::export(ExportMode::all_updates() / updates(from))
  *                            crates/loro-internal/src/encoding.rs:79-83, 350-416, oplog/change_store.rs:494-576
+ *   lb_batch_export_updates  the same export for many (document, from) requests in one call
  *   lb_docset_import         crates/loro/src/lib.rs:639, :425 on a document that already holds history
  *                            (crates/loro-internal/src/loro.rs:562-643, 1183-1290, oplog.rs:130-196)
  *   lb_batch_counters        crates/loro-internal/src/loro.rs:1458 len_ops / len_changes (summed over the batch)
  *   lb_import_batch_at       crates/loro-internal/src/loro.rs:1353-1433 LoroDoc::checkout(&frontiers) after the import,
  *   lb_docset_checkout       then get_deep_value() (the state at an earlier version: time travel)
+ *   lb_docset_read           a stored document's get_deep_value / oplog_vv / oplog_frontiers / export, nothing imported
  *
  * Conventions (mirroring the reference): input buffers are borrowed for the duration of the call only;
  * outputs are owned by the batch handle until lb_batch_free; a bad blob never aborts the batch -- it yields a
@@ -154,9 +156,32 @@ lb_status lb_doc_frontiers(const lb_batch* b, size_t doc, const lb_id_span** spa
  * otherwise `from` is a version vector (one span per peer, `end` = the first counter the receiver lacks; peers not
  * listed start at 0) and the stored changes are cut there (Change::slice) -- computed on demand, the returned buffer
  * stays valid until the next from-export of the same document or lb_batch_free.  Needs LB_FLAG_EXPORT at import time.
- * LB_ERR_UNSUPPORTED: the document uses something the export phase does not cover (lb_last_error). */
+ * LB_ERR_UNSUPPORTED: the document uses something the export phase does not cover (lb_last_error), which includes every
+ * document with code LB_DOC_ERR_UNSUPPORTED; LB_ERR_INVALID_ARG: the document failed to import (any other code). */
 lb_status lb_doc_export_updates(const lb_batch* b, size_t doc, const lb_id_span* from, size_t n_from,
                                 const uint8_t** bytes, size_t* len);
+/* Many LoroDoc::export(ExportMode::updates(from)) in one call (crates/loro/src/lib.rs:1235, encoding.rs:79-83): what a
+ * sync server answers each client with, computed for all requested documents in the same device passes.  Request i
+ * answers exactly what lb_doc_export_updates(b, reqs[i].doc, reqs[i].from, reqs[i].n_from, ...) answers: lb_exports_get
+ * returns its status and bytes -- LB_ERR_INVALID_ARG for a document that failed to import, LB_ERR_UNSUPPORTED for one the
+ * export phase does not cover -- without failing the other requests.  Requests may come in any order and name a document
+ * several times.  Equal versions of one document are computed once; a version that asks for everything (n_from = 0, or
+ * only peers the document lacks or counters <= 0) is the import-time all_updates blob and launches nothing; the others
+ * run in rounds, round r holding the r-th distinct version of every document, so the work grows with the largest number
+ * of distinct versions asked of one document, not with the number of documents.  The whole call fails with
+ * LB_ERR_INVALID_ARG, and launches nothing, when a `doc` is out of range, `from` is NULL with n_from > 0, or the batch was
+ * imported without LB_FLAG_EXPORT (checkout batches included).  n_reqs = 0 gives an empty result.  The bytes are host
+ * memory owned by the lb_exports and stay valid until lb_exports_free, also after lb_batch_free.  Export calls on one
+ * batch run one at a time. */
+typedef struct lb_export_request {
+    size_t doc;               /* document index in the batch */
+    const lb_id_span* from;   /* version vector exactly as for lb_doc_export_updates; n_from = 0: all_updates */
+    size_t n_from;
+} lb_export_request;
+typedef struct lb_exports lb_exports;
+lb_status lb_batch_export_updates(const lb_batch* b, const lb_export_request* reqs, size_t n_reqs, lb_exports** out);
+lb_status lb_exports_get(const lb_exports* e, size_t i, const uint8_t** bytes, size_t* len);
+void lb_exports_free(lb_exports* e);
 lb_status lb_batch_counters(const lb_batch* b, lb_counters* out);
 lb_status lb_batch_timings(const lb_batch* b, lb_timings* out);
 const char* lb_last_error(void); /* thread-local, human readable */
@@ -229,6 +254,16 @@ lb_status lb_import_batch_at(const lb_blob* blobs, size_t n_blobs, const lb_vers
  * versions; one the set has never seen is an empty document).  The status spans are empty: nothing is imported.  The
  * docset is not modified.  LB_ERR_INVALID_ARG: null frontiers with n_frontiers > 0, LB_FLAG_EXPORT or LB_FLAG_COMPACT. */
 lb_status lb_docset_checkout(lb_docset* set, const lb_version* at, size_t n_at, const lb_options* opt, lb_batch** out);
+
+/* ---- reading stored documents ---------------------------------------------------------------------------------------
+ * The stored documents as they are, without importing anything (a sync server answering a client that connects with
+ * nothing to send): one document per doc_id, in the order given, each holding its stored blobs laid out exactly as
+ * lb_docset_import lays them and no new blob; an id the set has never seen is an empty document.  The batch is imported
+ * with LB_FLAG_EXPORT: lb_doc_json (get_deep_value, crates/loro/src/lib.rs:866), lb_doc_vv, lb_doc_frontiers,
+ * lb_doc_export_updates and lb_batch_export_updates (crates/loro/src/lib.rs:1235, encoding.rs:79-83) answer for the
+ * stored document; lb_doc_status gives the document's code with empty spans (nothing was imported).  LB_FLAG_NO_JSON is
+ * honoured.  The docset is not modified.  LB_ERR_INVALID_ARG: a doc_id listed twice, LB_FLAG_COMPACT. */
+lb_status lb_docset_read(lb_docset* set, const uint64_t* doc_ids, size_t n, const lb_options* opt, lb_batch** out);
 
 /* test hooks (need LB_FLAG_KEEP_DEVICE): copy one decoded SoA table to the host.
  * name in {"op_cid","op_prop","op_vtype","op_len","op_counter","ch_counter","ch_len","ch_lamport",

@@ -44,6 +44,10 @@ class _Version(ctypes.Structure):
     _fields_ = [("doc_id", ctypes.c_uint64), ("frontiers", ctypes.POINTER(_IdSpan)), ("n_frontiers", ctypes.c_size_t)]
 
 
+class _ExportRequest(ctypes.Structure):
+    _fields_ = [("doc", ctypes.c_size_t), ("from_", ctypes.POINTER(_IdSpan)), ("n_from", ctypes.c_size_t)]
+
+
 class _Status(ctypes.Structure):
     _fields_ = [("code", ctypes.c_int), ("n_success", ctypes.c_size_t), ("success", ctypes.POINTER(_IdSpan)),
                 ("n_pending", ctypes.c_size_t), ("pending", ctypes.POINTER(_IdSpan))]
@@ -92,6 +96,9 @@ def load_library(path=None):
     L.lb_doc_json.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_size_t)]
     L.lb_doc_export_updates.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(_IdSpan), ctypes.c_size_t,
                                         ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_size_t)]
+    L.lb_batch_export_updates.argtypes = [vp, ctypes.POINTER(_ExportRequest), ctypes.c_size_t, ctypes.POINTER(vp)]
+    L.lb_exports_get.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_size_t)]
+    L.lb_exports_free.argtypes = [vp]
     L.lb_doc_vv.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(ctypes.POINTER(_IdSpan)), ctypes.POINTER(ctypes.c_size_t)]
     L.lb_doc_frontiers.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(ctypes.POINTER(_IdSpan)), ctypes.POINTER(ctypes.c_size_t)]
     L.lb_batch_counters.argtypes = [vp, ctypes.POINTER(_Counters)]
@@ -106,6 +113,8 @@ def load_library(path=None):
                                      ctypes.POINTER(_Options), ctypes.POINTER(vp)]
     L.lb_docset_checkout.argtypes = [vp, ctypes.POINTER(_Version), ctypes.c_size_t, ctypes.POINTER(_Options),
                                      ctypes.POINTER(vp)]
+    L.lb_docset_read.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64), ctypes.c_size_t, ctypes.POINTER(_Options),
+                                 ctypes.POINTER(vp)]
     L.lb_docset_doc_count.restype = ctypes.c_size_t
     L.lb_docset_doc_count.argtypes = [vp]
     L.lb_docset_stored_bytes.restype = ctypes.c_uint64
@@ -170,17 +179,41 @@ class Batch:
         (needs flags=LB_FLAG_EXPORT at import).  from_vv: {peer: first counter the receiver lacks}."""
         p = ctypes.c_void_p()
         n = ctypes.c_size_t()
-        spans, k = None, 0
-        if from_vv:
-            k = len(from_vv)
-            spans = (_IdSpan * k)()
-            for j, (peer, ctr) in enumerate(from_vv.items()):
-                spans[j].peer = peer
-                spans[j].start = 0
-                spans[j].end = ctr
+        spans, k = _vv_spans(from_vv)
         _check(self._L, self._L.lb_doc_export_updates(self._h, i, spans, k, ctypes.byref(p), ctypes.byref(n)),
                "lb_doc_export_updates")
         return ctypes.string_at(p.value, n.value)
+
+    def export_updates_many(self, requests):
+        """export_updates for many documents in one call (lb_batch_export_updates): `requests` = [(doc, from_vv or
+        None), ...].  Returns one entry per request: the bytes, or the EngineError of a request that failed (returned,
+        not raised).  A bad document index or a batch without LB_FLAG_EXPORT raises."""
+        requests = list(requests)
+        arr = (_ExportRequest * max(len(requests), 1))()
+        keep = []
+        for j, (doc, from_vv) in enumerate(requests):
+            spans, k = _vv_spans(from_vv)
+            keep.append(spans)
+            arr[j].doc = doc
+            arr[j].from_ = spans
+            arr[j].n_from = k
+        h = ctypes.c_void_p()
+        _check(self._L, self._L.lb_batch_export_updates(self._h, arr, len(requests), ctypes.byref(h)),
+               "lb_batch_export_updates")
+        out = []
+        try:
+            for j in range(len(requests)):
+                p = ctypes.c_void_p()
+                n = ctypes.c_size_t()
+                rc = self._L.lb_exports_get(h, j, ctypes.byref(p), ctypes.byref(n))
+                if rc == 0:
+                    out.append(ctypes.string_at(p.value, n.value))
+                else:
+                    msg = self._L.lb_last_error().decode(errors="replace")
+                    out.append(EngineError(f"export request {j} failed (lb_status={rc}): {msg}", rc))
+        finally:
+            self._L.lb_exports_free(h)
+        return out
 
     def json_bytes(self, i):
         p = ctypes.c_char_p()
@@ -266,6 +299,19 @@ class MultiBatch:
     def oplog_vv(self, i): p, j = self._loc(i); return p.oplog_vv(j)
     def oplog_frontiers(self, i): p, j = self._loc(i); return p.oplog_frontiers(j)
     def export_updates(self, i, from_vv=None): p, j = self._loc(i); return p.export_updates(j, from_vv)
+
+    def export_updates_many(self, requests):
+        """Batch.export_updates_many with every request sent to its sub-batch: one C call per sub-batch."""
+        requests = list(requests)
+        per_part = {}
+        for k, (i, from_vv) in enumerate(requests):
+            p, j = self._loc(i)
+            per_part.setdefault(id(p), (p, []))[1].append((k, j, from_vv))
+        out = [None] * len(requests)
+        for p, reqs in per_part.values():
+            for (k, _, _), r in zip(reqs, p.export_updates_many([(j, f) for _, j, f in reqs])):
+                out[k] = r
+        return out
 
     def fetch_json(self):
         for p in self._parts:
@@ -399,6 +445,18 @@ def import_batch_at(blobs, versions, doc_ids=None, device=0, flags=0, lib_path=N
     return Batch(L, h.value)
 
 
+def _vv_spans(from_vv):
+    """{peer: counter} -> (lb_id_span array or None, count) in the form lb_doc_export_updates takes"""
+    if not from_vv:
+        return None, 0
+    spans = (_IdSpan * len(from_vv))()
+    for j, (peer, ctr) in enumerate(from_vv.items()):
+        spans[j].peer = peer
+        spans[j].start = 0
+        spans[j].end = ctr
+    return spans, len(from_vv)
+
+
 def _version_array(requests):
     """[(doc_id, [(peer, counter), ...]), ...] -> lb_version array (+ the span arrays it points into)"""
     arr = (_Version * max(len(requests), 1))()
@@ -462,6 +520,18 @@ class DocSet:
         h = ctypes.c_void_p()
         _check(self._L, self._L.lb_docset_checkout(self._h, ver, len(requests), ctypes.byref(opt), ctypes.byref(h)),
                "lb_docset_checkout")
+        return Batch(self._L, h.value)
+
+    def read(self, doc_ids, flags=0):
+        """The stored documents as they are, nothing imported (lb_docset_read): document i of the returned Batch is
+        doc_ids[i] (an id the set has never seen is an empty document), imported with LB_FLAG_EXPORT so that
+        export_updates / export_updates_many answer for it.  The set is not modified."""
+        doc_ids = [int(d) for d in doc_ids]
+        ids = (ctypes.c_uint64 * max(len(doc_ids), 1))(*doc_ids)
+        opt = _Options(device=self._device, flags=flags)
+        h = ctypes.c_void_p()
+        _check(self._L, self._L.lb_docset_read(self._h, ids, len(doc_ids), ctypes.byref(opt), ctypes.byref(h)),
+               "lb_docset_read")
         return Batch(self._L, h.value)
 
     @property

@@ -336,13 +336,15 @@ struct lb_batch {
     std::vector<u32> ck_range;
     std::vector<u64> ck_peer;
     std::vector<i32> ck_ctr;
-    bool ck_docset = false;                   // lb_docset_checkout: nothing was imported, the status spans stay empty
+    bool stored_only = false;                 // lb_docset_checkout / lb_docset_read: nothing was imported, the status spans
+                                              // stay empty
     DocInfo* d_docs = nullptr;
     u8* d_json = nullptr;
     u8* d_export = nullptr;      // phase 7 output: one FastUpdates blob per document
     u64 export_total = 0;
     std::vector<XDoc> xdocs;
-    std::unordered_map<size_t, std::vector<uint8_t>> from_exports;   // last on-demand export per document
+    std::unordered_map<size_t, std::vector<uint8_t>> from_exports;   // last lb_doc_export_updates(from) per document
+    std::mutex export_mu;                     // on-demand exports of one batch run one at a time
     uint8_t* exported = nullptr;  // malloc'ed host copy (lbstage::download)
     bool export_fetched = false;
     u64 n_blocks = 0, n_changes = 0, n_rows = 0, n_peers_tot = 0, json_total = 0, n_deps = 0;
@@ -385,6 +387,13 @@ struct lb_docset {
     std::mutex mu;
     std::unordered_map<u64, DocsetDoc> docs;
     u64 stored_bytes = 0;
+};
+
+// The answers of one lb_batch_export_updates call, in host memory that outlives the batch.
+struct lb_exports {
+    struct Answer { lb_status status; const char* error; const uint8_t* bytes; size_t len; };
+    std::vector<Answer> answers;                        // one per request
+    std::vector<std::unique_ptr<uint8_t[]>> bufs;       // the packed blobs of each round, and the all_updates copies
 };
 
 namespace {
@@ -808,7 +817,7 @@ void pipeline(lb_batch* b) {
             if (m == &BatchTables::fc_skip) t.fc_block = dv.alloc<u8>(SEGCAP);
             t.*m = dv.alloc<u32>(SEGCAP, m == &BatchTables::fc_skip);
         }
-        t.only_doc = 0xFFFFFFFFu; t.from_ctr = nullptr;
+        t.x_req = nullptr; t.from_ctr = nullptr;
         trace_point(b, "export allocs");
         LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, t);
         if (NTR) LB_BATCH_LAUNCH(b, k_exp_posrank, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t);
@@ -901,8 +910,8 @@ void build_status(lb_batch* b) {
         if (di.code == DOC_OK || di.code == DOC_ERR_UNSUPPORTED || di.code == DOC_ERR_FRONTIERS) {
             for (u32 p = 0; p < di.P; p++) {
                 const DocPeer& dp = b->dpeer[b->peer_base[d] + p];
-                if (dp.has_succ && !b->ck_docset) b->spans[0].push_back(lb_id_span{dp.id, dp.succ_lo, dp.end_counter});
-                if (dp.pend_hi > dp.pend_lo && !b->ck_docset) b->spans[1].push_back(lb_id_span{dp.id, dp.pend_lo, dp.pend_hi});
+                if (dp.has_succ && !b->stored_only) b->spans[0].push_back(lb_id_span{dp.id, dp.succ_lo, dp.end_counter});
+                if (dp.pend_hi > dp.pend_lo && !b->stored_only) b->spans[1].push_back(lb_id_span{dp.id, dp.pend_lo, dp.pend_hi});
                 if (dp.end_counter > 0) b->spans[2].push_back(lb_id_span{dp.id, 0, dp.end_counter});
                 if (dp.is_head && dp.end_counter > 0) b->spans[3].push_back(lb_id_span{dp.id, dp.end_counter - 1, dp.end_counter});
             }
@@ -1036,50 +1045,120 @@ lb_status upload_and_run(lb_batch* b, const std::vector<u64>& offs, const std::v
     return run_batch(b);
 }
 
-// export(ExportMode::updates(from)) of one document (encoding.rs:79-83 ; change_store.rs:494-528 export_blocks_from):
-// the import store is rebuilt for that document only, its changes are cut at `from` (Change::slice) on their way into
-// the fresh export store, and the result is encoded like the import-time export.  The phase-7 tables of the batch are
-// reused; only the per-call pieces (cut positions, block list, scratch, output) are allocated.
-lb_status export_from(lb_batch* b, size_t doc, const lb_id_span* from, size_t n_from, std::vector<uint8_t>& out) {
-    try {
-        Dev& dv = b->dev;
-        cudaStream_t st = dv.stream;
-        const u32 D = (u32)b->n_docs;
-        const u64 NCH = b->n_changes;
+const char* const ERR_FAILED_DOC = "document failed to import";
+const char* const ERR_NOT_COVERED = "document uses features the export phase does not cover";
+// the answer for a document whose code is not OK: one with ops the engine does not merge (LB_DOC_ERR_UNSUPPORTED) is not
+// covered by the export phase either; any other code means the import failed
+lb_exports::Answer doc_error(const DocInfo& di) {
+    if (di.code == DOC_ERR_UNSUPPORTED) return lb_exports::Answer{LB_ERR_UNSUPPORTED, ERR_NOT_COVERED, nullptr, 0};
+    return lb_exports::Answer{LB_ERR_INVALID_ARG, ERR_FAILED_DOC, nullptr, 0};
+}
+
+// One pass of export(ExportMode::updates(from)) (encoding.rs:79-83 ; change_store.rs:494-528 export_blocks_from) over
+// the documents of a round, at most one version each: the import store of each marked document is rebuilt, its changes
+// are cut at the document's `from` (Change::slice) on their way into a fresh export store, and the result is encoded
+// like the import-time export.  The phase-7 tables of the batch are reused; only the per-pass pieces (cut positions,
+// request mask, block list, scratch, output) are allocated.  The stores rewrite the rows' flags (k_exp_store merges ops
+// across changes), which is why a document can be in one request per pass only.
+// h_from: first counter to export per batch peer slot; h_req: the request mask.  Returns the round's packed blobs in
+// host memory, with the XDoc table that places them (exp_off / exp_len of every marked document).
+std::unique_ptr<uint8_t[]> export_round(lb_batch* b, const std::vector<i32>& h_from, const std::vector<u8>& h_req,
+                                        std::vector<XDoc>& xd) {
+    Dev& dv = b->dev;
+    cudaStream_t st = dv.stream;
+    const u32 D = (u32)b->n_docs;
+    const u64 NCH = b->n_changes;
+    BatchTables xt = b->tb;
+    i32* d_from = dv.alloc<i32>(h_from.size());
+    u8* d_req = dv.alloc<u8>(D);
+    CK(cudaMemcpyAsync(d_from, h_from.data(), sizeof(i32) * h_from.size(), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_req, h_req.data(), D, cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));   // pageable host memory
+    xt.from_ctr = d_from;
+    xt.x_req = d_req;
+    xt.xdoc = dv.alloc<XDoc>(D + 1, true);
+    LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, xt);
+    if (NCH) {
+        LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 0);
+        LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 1);
+    }
+    LB_BATCH_LAUNCH(b, k_exp_store, nblk(D, 64), 64, 0, b->d_docs, D, xt);
+    u64 XT = 0;
+    u8* d_out = export_encode(b, xt, &XT);
+    xd.resize(D);
+    CK(cudaMemcpyAsync(xd.data(), xt.xdoc, sizeof(XDoc) * D, cudaMemcpyDeviceToHost, st));
+    std::unique_ptr<uint8_t[]> out(new uint8_t[XT + 1]);
+    if (!lbstage::download(d_out, out.get(), XT, st)) { g_last_error = "export d2h failed"; throw lb_status(LB_ERR_CUDA); }
+    CK(cudaStreamSynchronize(st));
+    dv.release(d_from); dv.release(d_req); dv.release(xt.xdoc); dv.release(d_out);
+    return out;
+}
+
+// Answers every request of lb_batch_export_updates (the arguments are checked).  Each `from` becomes its document's
+// vector over the document's peer slots; equal vectors of one document are answered once, the all-zero vector from the
+// import-time export, and the rest in rounds: round r holds the r-th distinct vector of every document, so the number of
+// passes is the largest number of distinct versions asked of one document, whatever the number of documents.
+void export_requests(lb_batch* b, const lb_export_request* reqs, size_t n, lb_exports& e) {
+    struct Version { size_t doc; u32 round; std::vector<i32> from; };
+    std::vector<Version> versions;                          // distinct (document, vector) pairs, round by round below
+    std::unordered_map<size_t, std::vector<u32>> of_doc;    // document -> its versions, in order of first request
+    std::vector<u32> version_of(n, ~0u);                    // request -> version; ~0: all_updates or failed document
+    e.answers.assign(n, lb_exports::Answer{LB_OK, nullptr, nullptr, 0});
+    std::vector<size_t> all_updates;                        // requests answered by the import-time export
+    for (size_t i = 0; i < n; i++) {
+        const size_t doc = reqs[i].doc;
         const DocInfo& di = b->docs[doc];
-        BatchTables xt = b->tb;
-        // only the document's own peer slots are read (every kernel is restricted to `only_doc`)
-        std::vector<i32> h_from(di.P + 1, 0);
-        for (size_t k = 0; k < n_from; k++)
+        if (di.code != DOC_OK) { e.answers[i] = doc_error(di); continue; }
+        // the last span for a peer wins; peers the document lacks are ignored
+        std::vector<i32> h(di.P, 0);
+        for (size_t k = 0; k < reqs[i].n_from; k++)
             for (u32 p = 0; p < di.P; p++)
-                if (b->dpeer[b->peer_base[doc] + p].id == from[k].peer) h_from[p] = from[k].end;
-        i32* d_from = dv.alloc<i32>(b->n_peers_tot + 1);
-        CK(cudaMemcpyAsync(d_from + di.peer0, h_from.data(), sizeof(i32) * di.P, cudaMemcpyHostToDevice, st));
-        CK(cudaStreamSynchronize(st));   // h_from is pageable host memory
-        xt.from_ctr = d_from;
-        xt.only_doc = (u32)doc;
-        XDoc* xdoc = dv.alloc<XDoc>(D + 1, true);
-        xt.xdoc = xdoc;
-        LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, xt);
-        if (NCH) {
-            LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 0);
-            LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 1);
+                if (b->dpeer[b->peer_base[doc] + p].id == reqs[i].from[k].peer) h[p] = reqs[i].from[k].end;
+        if (std::all_of(h.begin(), h.end(), [](i32 c) { return c <= 0; })) { all_updates.push_back(i); continue; }
+        std::vector<u32>& mine = of_doc[doc];
+        for (u32 v : mine) if (versions[v].from == h) version_of[i] = v;
+        if (version_of[i] == ~0u) {
+            version_of[i] = (u32)versions.size();
+            versions.push_back(Version{doc, (u32)mine.size(), std::move(h)});
+            mine.push_back(version_of[i]);
         }
-        LB_BATCH_LAUNCH(b, k_exp_store, nblk(D, 64), 64, 0, b->d_docs, D, xt);
-        u64 XT = 0;
-        u8* d_out = export_encode(b, xt, &XT);
-        XDoc x = d2h_one(b, xdoc + doc);
-        lb_status rc = LB_OK;
-        if ((x.flags & 1) || x.exp_len == 0) { g_last_error = "document uses features the export phase does not cover"; rc = LB_ERR_UNSUPPORTED; }
-        else {
-            out.resize(x.exp_len);
-            CK(cudaMemcpyAsync(out.data(), d_out + x.exp_off, x.exp_len, cudaMemcpyDeviceToHost, st));
-            CK(cudaStreamSynchronize(st));
+    }
+    // all_updates: the document's blob of the import-time export, copied out of the batch's export buffer
+    if (!all_updates.empty()) {
+        u64 total = 0;
+        for (size_t i : all_updates) total += b->xdocs[reqs[i].doc].exp_len;
+        e.bufs.emplace_back(new uint8_t[total + 1]);
+        uint8_t* w = e.bufs.back().get();
+        for (size_t i : all_updates) {
+            const XDoc& x = b->xdocs[reqs[i].doc];
+            if ((x.flags & 1) || x.exp_len == 0) { e.answers[i] = lb_exports::Answer{LB_ERR_UNSUPPORTED, ERR_NOT_COVERED, nullptr, 0}; continue; }
+            CK(cudaMemcpyAsync(w, b->d_export + x.exp_off, x.exp_len, cudaMemcpyDeviceToHost, b->dev.stream));
+            e.answers[i].bytes = w;
+            e.answers[i].len = x.exp_len;
+            w += x.exp_len;
         }
-        dv.release(d_from); dv.release(xdoc); dv.release(d_out);
-        return rc;
-    } catch (lb_status s) {
-        return s;
+        CK(cudaStreamSynchronize(b->dev.stream));
+    }
+    size_t rounds = 0;
+    for (const auto& kv : of_doc) rounds = std::max(rounds, kv.second.size());
+    std::vector<XDoc> xd;
+    for (size_t r = 0; r < rounds; r++) {
+        std::vector<i32> h_from(b->n_peers_tot + 1, 0);
+        std::vector<u8> h_req(b->n_docs, 0);
+        for (const auto& kv : of_doc) {
+            if (r >= kv.second.size()) continue;
+            const Version& v = versions[kv.second[r]];
+            std::copy(v.from.begin(), v.from.end(), h_from.begin() + b->docs[v.doc].peer0);
+            h_req[v.doc] = 1;
+        }
+        e.bufs.push_back(export_round(b, h_from, h_req, xd));
+        const uint8_t* blobs = e.bufs.back().get();
+        for (size_t i = 0; i < n; i++) {
+            if (version_of[i] == ~0u || versions[version_of[i]].round != r) continue;
+            const XDoc& x = xd[reqs[i].doc];
+            if ((x.flags & 1) || x.exp_len == 0) e.answers[i] = lb_exports::Answer{LB_ERR_UNSUPPORTED, ERR_NOT_COVERED, nullptr, 0};
+            else e.answers[i] = lb_exports::Answer{LB_OK, nullptr, blobs + x.exp_off, x.exp_len};
+        }
     }
 }
 
@@ -1147,11 +1226,12 @@ extern "C" {
 // Host-buffer import, shared by lb_import_batch (fresh documents), lb_docset_import (documents with an earlier state:
 // their stored blobs come first, already in device memory, and count as `n_prior` for the import status) and the
 // checkout entry points: `at` names the documents built at an earlier version (k_checkout.cuh).  With `set_checkout` the
-// documents are the requests themselves, one per entry of `at`, each made of its document's stored blobs only; the
-// docset is read, never written.
+// documents are the requests themselves, one per entry of `at`, each made of its document's stored blobs only; with
+// `read_ids` (lb_docset_read) they are the listed ids, each made of its stored blobs, at the latest version and exported.
+// In both the docset is read, never written.
 static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_version* at, size_t n_at, const lb_options* opt,
-                             lb_docset* set, bool set_checkout, lb_batch** out) {
-    if (!out || (!blobs && n_blobs) || (!at && n_at)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
+                             lb_docset* set, bool set_checkout, const uint64_t* read_ids, size_t n_read, lb_batch** out) {
+    if (!out || (!blobs && n_blobs) || (!at && n_at) || (!read_ids && n_read)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
     *out = nullptr;
     lb_options o2;
     memset(&o2, 0, sizeof(o2));
@@ -1164,8 +1244,9 @@ static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_vers
         for (size_t i = 0; i < n_at; i++)
             if (!at[i].frontiers && at[i].n_frontiers) { g_last_error = "null frontiers"; return LB_ERR_INVALID_ARG; }
     }
+    if (read_ids && (o2.flags & LB_FLAG_COMPACT)) { g_last_error = "LB_FLAG_COMPACT on a read: the docset is not written"; return LB_ERR_INVALID_ARG; }
     if (set) o2.device = set->device;
-    if (set && !set_checkout) o2.flags |= LB_FLAG_EXPORT;   // the re-export is what a stored document keeps
+    if (set && !set_checkout) o2.flags |= LB_FLAG_EXPORT;   // the re-export is what a stored document keeps (or is read for)
     return import_with_new_batch(&o2, out, [&](lb_batch* b) {
         if (n_blobs >= 0x7FFFFFFFull) { g_last_error = "too many blobs"; throw lb_status(LB_ERR_INVALID_ARG); }
         b->eager_json = true;   // host buffers in, host results expected
@@ -1208,11 +1289,17 @@ static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_vers
             }
             if (set_checkout)   // one document per request, in request order (no new blobs)
                 for (size_t i = 0; i < n_at; i++) { b->doc_ids.push_back(at[i].doc_id); count.push_back(0); nd++; }
+            for (size_t i = 0; i < n_read; i++) {   // one document per listed id, in list order (no new blobs)
+                if (!doc_of.emplace(read_ids[i], (u32)nd).second) { g_last_error = "doc_id listed twice"; throw lb_status(LB_ERR_INVALID_ARG); }
+                b->doc_ids.push_back(read_ids[i]);
+                count.push_back(0);
+                nd++;
+            }
+            b->stored_only = set_checkout || read_ids;
             b->n_docs = nd;
         }
         const size_t nd = b->n_docs;
         if (at) {
-            b->ck_docset = set_checkout;
             b->ck_range.assign(2 * nd, CK_LATEST);
             for (size_t i = 0; i < n_at; i++) {
                 u32 d = (u32)i;
@@ -1310,18 +1397,18 @@ static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_vers
         }
         lb_status s = upload_and_run(b, offs, lens, d_bytes);
         CK(cudaStreamSynchronize(b->dev.stream));
-        if (s == LB_OK && set && !set_checkout) docset_store(set, b, offs, lens);
+        if (s == LB_OK && set && !b->stored_only) docset_store(set, b, offs, lens);
         return s;
     });
 }
 
 lb_status lb_import_batch(const lb_blob* blobs, size_t n_blobs, const lb_options* opt, lb_batch** out) {
-    return import_host(blobs, n_blobs, nullptr, 0, opt, nullptr, false, out);
+    return import_host(blobs, n_blobs, nullptr, 0, opt, nullptr, false, nullptr, 0, out);
 }
 
 lb_status lb_import_batch_at(const lb_blob* blobs, size_t n_blobs, const lb_version* at, size_t n_at, const lb_options* opt,
                              lb_batch** out) {
-    return import_host(blobs, n_blobs, at, n_at, opt, nullptr, false, out);
+    return import_host(blobs, n_blobs, at, n_at, opt, nullptr, false, nullptr, 0, out);
 }
 
 lb_status lb_docset_new(const lb_options* opt, lb_docset** out) {
@@ -1344,13 +1431,19 @@ uint64_t lb_docset_stored_bytes(const lb_docset* set) { return set ? set->stored
 lb_status lb_docset_import(lb_docset* set, const lb_blob* blobs, size_t n_blobs, const lb_options* opt, lb_batch** out) {
     if (!set) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
     std::lock_guard<std::mutex> g(set->mu);
-    return import_host(blobs, n_blobs, nullptr, 0, opt, set, false, out);
+    return import_host(blobs, n_blobs, nullptr, 0, opt, set, false, nullptr, 0, out);
 }
 
 lb_status lb_docset_checkout(lb_docset* set, const lb_version* at, size_t n_at, const lb_options* opt, lb_batch** out) {
     if (!set) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
     std::lock_guard<std::mutex> g(set->mu);
-    return import_host(nullptr, 0, at, n_at, opt, set, true, out);
+    return import_host(nullptr, 0, at, n_at, opt, set, true, nullptr, 0, out);
+}
+
+lb_status lb_docset_read(lb_docset* set, const uint64_t* doc_ids, size_t n, const lb_options* opt, lb_batch** out) {
+    if (!set) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
+    std::lock_guard<std::mutex> g(set->mu);
+    return import_host(nullptr, 0, nullptr, 0, opt, set, false, doc_ids, n, out);
 }
 
 lb_status lb_import_batch_device(const uint8_t* d_bytes, const uint64_t* offsets, const uint32_t* blob_lens,
@@ -1435,18 +1528,30 @@ lb_status lb_doc_export_updates(const lb_batch* cb, size_t doc, const lb_id_span
     lb_batch* b = const_cast<lb_batch*>(cb);
     if (!b || !bytes || !len || doc >= b->n_docs) { g_last_error = "bad argument"; return LB_ERR_INVALID_ARG; }
     if (!(b->flags & LB_FLAG_EXPORT)) { g_last_error = "batch was imported without LB_FLAG_EXPORT"; return LB_ERR_INVALID_ARG; }
-    if (b->docs[doc].code != DOC_OK) { g_last_error = "document failed to import"; return LB_ERR_INVALID_ARG; }
-    if (from && n_from) {   // export(ExportMode::updates(from)): computed on demand for this document
-        if (!b->tb.xdoc) { g_last_error = "batch holds no export tables"; return LB_ERR_INVALID_ARG; }
+    if (b->docs[doc].code != DOC_OK) {
+        lb_exports::Answer a = doc_error(b->docs[doc]);
+        g_last_error = a.error;
+        return a.status;
+    }
+    std::lock_guard<std::mutex> g(b->export_mu);
+    if (from && n_from) {   // export(ExportMode::updates(from)): a one-request lb_batch_export_updates
+        lb_export_request rq{doc, from, n_from};
+        lb_exports e;
+        try {
+            export_requests(b, &rq, 1, e);
+        } catch (lb_status s) {
+            return s;
+        }
+        const lb_exports::Answer& a = e.answers[0];
+        if (a.status != LB_OK) { g_last_error = a.error; return a.status; }
         std::vector<uint8_t>& buf = b->from_exports[doc];
-        lb_status rc = export_from(b, doc, from, n_from, buf);
-        if (rc != LB_OK) return rc;
+        buf.assign(a.bytes, a.bytes + a.len);
         *bytes = buf.data();
         *len = buf.size();
         return LB_OK;
     }
     const XDoc& x = b->xdocs[doc];
-    if ((x.flags & 1) || x.exp_len == 0) { g_last_error = "document uses features the export phase does not cover"; return LB_ERR_UNSUPPORTED; }
+    if ((x.flags & 1) || x.exp_len == 0) { g_last_error = ERR_NOT_COVERED; return LB_ERR_UNSUPPORTED; }
     if (!b->export_fetched) {
         b->exported = (uint8_t*)lbstage::host_cache().take(b->export_total + 1);
         if (!b->exported) { g_last_error = "out of host memory"; return LB_ERR_OOM; }
@@ -1460,6 +1565,37 @@ lb_status lb_doc_export_updates(const lb_batch* cb, size_t doc, const lb_id_span
     *len = x.exp_len;
     return LB_OK;
 }
+
+lb_status lb_batch_export_updates(const lb_batch* cb, const lb_export_request* reqs, size_t n_reqs, lb_exports** out) {
+    lb_batch* b = const_cast<lb_batch*>(cb);
+    if (!b || !out || (!reqs && n_reqs)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
+    *out = nullptr;
+    if (!(b->flags & LB_FLAG_EXPORT)) { g_last_error = "batch was imported without LB_FLAG_EXPORT"; return LB_ERR_INVALID_ARG; }
+    for (size_t i = 0; i < n_reqs; i++) {
+        if (reqs[i].doc >= b->n_docs) { g_last_error = "document index out of range"; return LB_ERR_INVALID_ARG; }
+        if (!reqs[i].from && reqs[i].n_from) { g_last_error = "null from with n_from > 0"; return LB_ERR_INVALID_ARG; }
+    }
+    std::unique_ptr<lb_exports> e(new lb_exports());
+    std::lock_guard<std::mutex> g(b->export_mu);
+    try {
+        export_requests(b, reqs, n_reqs, *e);
+    } catch (lb_status s) {
+        return s;
+    }
+    *out = e.release();
+    return LB_OK;
+}
+
+lb_status lb_exports_get(const lb_exports* e, size_t i, const uint8_t** bytes, size_t* len) {
+    if (!e || !bytes || !len || i >= e->answers.size()) { g_last_error = "bad argument"; return LB_ERR_INVALID_ARG; }
+    const lb_exports::Answer& a = e->answers[i];
+    if (a.status != LB_OK) { g_last_error = a.error; return a.status; }
+    *bytes = a.bytes;
+    *len = a.len;
+    return LB_OK;
+}
+
+void lb_exports_free(lb_exports* e) { delete e; }
 
 lb_status lb_batch_counters(const lb_batch* b, lb_counters* out) {
     if (!b || !out) return LB_ERR_INVALID_ARG;

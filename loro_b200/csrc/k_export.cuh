@@ -464,7 +464,7 @@ __device__ inline void segment_summaries(const BatchTables& t, const DocInfo& di
 __global__ void k_exp_changes(DocInfo* __restrict__ docs, u64 n_changes, const __grid_constant__ BatchTables t, int pass) {
     u64 ch = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (ch >= n_changes) return;
-    if (t.only_doc != 0xFFFFFFFFu && t.blocks[t.ch_block[ch]].doc != t.only_doc) return;
+    if (t.x_req && !t.x_req[t.blocks[t.ch_block[ch]].doc]) return;
     if (!t.ch_applied[ch]) { if (!pass) { t.ch_nseg[ch] = 0; t.ch_syn[ch] = 0; } return; }
     u32 doc = t.blocks[t.ch_block[ch]].doc;
     const DocInfo& di = docs[doc];
@@ -759,7 +759,7 @@ __global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, const 
     const DocInfo& di = docs[d];
     if (di.code != DOC_OK) return;
     XDoc x = t.xdoc[d];
-    if (t.only_doc != 0xFFFFFFFFu && d != t.only_doc) { x.n_fc = x.n_mb = 0; t.xdoc[d] = x; return; }
+    if (t.x_req && !t.x_req[d]) { x.n_fc = x.n_mb = 0; t.xdoc[d] = x; return; }
     if (x.flags & 1) { t.xdoc[d] = x; return; }
     u64 w = di.ch0 + t.ch_seg0[di.ch0];   // as many slots as the document has segments
     u64 w0 = w;
@@ -1450,14 +1450,15 @@ template <> __global__ void __launch_bounds__(64, 5) k_exp_encode<1>(const DocIn
 }
 
 // thread per document, after the encode: block offsets inside the blob, blob length, and the blocks that outgrew their
-// slot, each given a retry slot of its block length (an upper bound on its pieces) at a document-relative offset
+// slot, each given a retry slot of its block length (an upper bound on its pieces) at a document-relative offset.  A
+// document outside the request mask gets no blob (exp_len 0), so the buffer holds the requested blobs only.
 __global__ void k_exp_layout(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t, XBlock* __restrict__ xb,
                              u32* __restrict__ padded_len, u32* __restrict__ n_ovf, u32* __restrict__ n_restage) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
     XDoc& x = t.xdoc[d];
     u32 len = 0, ovf = 0, restage = 0;
-    if (docs[d].code == DOC_OK && !(x.flags & 1)) {
+    if (docs[d].code == DOC_OK && !(x.flags & 1) && (!t.x_req || t.x_req[d])) {
         len = 22;
         for (u32 i = 0; i < x.n_mb; i++) {
             XBlock& b = xb[x.ob0 + i];

@@ -112,11 +112,11 @@ struct BatchTables {
     u32* fc_src; u32* fc_pos; u32* fc_r0; u32* fc_from; u32* fc_atoms; u32* fc_nrows; u32* fc_ndel; u8* fc_block;
     u32* fc_skip;      // atoms of the change's first row that lie before the `from` version (Op::slice)
     u32* fc_est;       // the store's size estimate of the change's ops (sizes the staging slot of its block)
-    // export(ExportMode::updates(from)) of ONE document on demand (lb_doc_export_updates): only_doc != ~0 restricts
-    // every kernel to that document; from_ctr[doc peer slot] = first counter to export (encoding.rs:79-83,
-    // change_store.rs:494-528 export_blocks_from, change.rs:203-258 Change::slice).  export_from sets these three on
-    // a copy of the batch's struct.
-    u32 only_doc; const i32* from_ctr;
+    // export(ExportMode::updates(from)) on demand (lb_batch_export_updates): x_req[d] != 0 marks the documents of one
+    // round (null: every document, the import-time export); from_ctr[doc peer slot] = first counter to export
+    // (encoding.rs:79-83, change_store.rs:494-528 export_blocks_from, change.rs:203-258 Change::slice).  export_round
+    // sets these three on a copy of the batch's struct.
+    const u8* x_req; const i32* from_ctr;
     XDoc* xdoc;
     // ---- checkout (k_checkout.cuh), written after the causal scan, read by phases 4 and 5 (last, so that the layout of
     // every other field is the same with or without it)
