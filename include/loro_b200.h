@@ -18,6 +18,8 @@
  *   lb_doc_export_updates    crates/loro/src/lib.rs:1235 LoroDoc::export(ExportMode::all_updates() / updates(from))
  *                            crates/loro-internal/src/encoding.rs:79-83, 350-416, oplog/change_store.rs:494-576
  *   lb_batch_export_updates  the same export for many (document, from) requests in one call
+ *   lb_batch_export_json_updates  crates/loro/src/lib.rs:687-720 LoroDoc::export_json_updates(start_vv, end_vv)
+ *                            (crates/loro-internal/src/loro.rs:715-751, encoding/json_schema.rs), many requests per call
  *   lb_docset_import         crates/loro/src/lib.rs:639, :425 on a document that already holds history
  *                            (crates/loro-internal/src/loro.rs:562-643, 1183-1290, oplog.rs:130-196)
  *   lb_batch_counters        crates/loro-internal/src/loro.rs:1458 len_ops / len_changes (summed over the batch)
@@ -182,6 +184,27 @@ typedef struct lb_exports lb_exports;
 lb_status lb_batch_export_updates(const lb_batch* b, const lb_export_request* reqs, size_t n_reqs, lb_exports** out);
 lb_status lb_exports_get(const lb_exports* e, size_t i, const uint8_t** bytes, size_t* len);
 void lb_exports_free(lb_exports* e);
+/* LoroDoc::export_json_updates(start_vv, end_vv) (crates/loro/src/lib.rs:687-720, crates/loro-internal/src/loro.rs:715-751,
+ * encoding/json_schema.rs): the changes of document `doc` between two versions in the JSON schema of docs/JsonSchema.md,
+ * as serde_json::to_string prints it -- UTF-8 without a terminator, returned through lb_exports_get.  Both versions are
+ * refined like the reference's (a counter is clamped to the oplog vv; a peer not listed is 0, so an empty `end` exports
+ * nothing); every stored change of a peer that overlaps [start, end) is listed, cut at both ends (Change::slice).  Changes
+ * are ordered by lamport, equal lamports by ascending peer id (the reference leaves those in hash order); object keys of
+ * nested map values are ascending.  With peer compression (the default) ids carry indices into `peers`, registered in
+ * first-use order; LB_JSON_NO_PEER_COMPRESSION gives real peer ids and "peers": null.  All requests of a call run in one
+ * device pass whatever their number; their text is written in chunks of bounded device size.  Errors follow
+ * lb_batch_export_updates: LB_ERR_INVALID_ARG for a document that failed to import and LB_ERR_UNSUPPORTED for one the export
+ * phase does not cover, per request; the whole call fails with LB_ERR_INVALID_ARG, launching nothing, for a `doc` out of
+ * range, a null span pointer with a count > 0, or a batch imported without LB_FLAG_EXPORT.  n_reqs = 0 gives an empty
+ * result. */
+#define LB_JSON_NO_PEER_COMPRESSION 1u
+typedef struct lb_json_request {
+    size_t doc;
+    const lb_id_span* start; size_t n_start;   /* start_vv, spans as for lb_export_request.from */
+    const lb_id_span* end;   size_t n_end;     /* end_vv: a peer not listed ends at 0 */
+    uint32_t flags;                            /* LB_JSON_NO_PEER_COMPRESSION */
+} lb_json_request;
+lb_status lb_batch_export_json_updates(const lb_batch* b, const lb_json_request* reqs, size_t n_reqs, lb_exports** out);
 lb_status lb_batch_counters(const lb_batch* b, lb_counters* out);
 lb_status lb_batch_timings(const lb_batch* b, lb_timings* out);
 const char* lb_last_error(void); /* thread-local, human readable */

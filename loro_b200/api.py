@@ -48,6 +48,14 @@ class _ExportRequest(ctypes.Structure):
     _fields_ = [("doc", ctypes.c_size_t), ("from_", ctypes.POINTER(_IdSpan)), ("n_from", ctypes.c_size_t)]
 
 
+class _JsonRequest(ctypes.Structure):
+    _fields_ = [("doc", ctypes.c_size_t), ("start", ctypes.POINTER(_IdSpan)), ("n_start", ctypes.c_size_t),
+                ("end", ctypes.POINTER(_IdSpan)), ("n_end", ctypes.c_size_t), ("flags", ctypes.c_uint32)]
+
+
+LB_JSON_NO_PEER_COMPRESSION = 1
+
+
 class _Status(ctypes.Structure):
     _fields_ = [("code", ctypes.c_int), ("n_success", ctypes.c_size_t), ("success", ctypes.POINTER(_IdSpan)),
                 ("n_pending", ctypes.c_size_t), ("pending", ctypes.POINTER(_IdSpan))]
@@ -97,6 +105,7 @@ def load_library(path=None):
     L.lb_doc_export_updates.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(_IdSpan), ctypes.c_size_t,
                                         ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_size_t)]
     L.lb_batch_export_updates.argtypes = [vp, ctypes.POINTER(_ExportRequest), ctypes.c_size_t, ctypes.POINTER(vp)]
+    L.lb_batch_export_json_updates.argtypes = [vp, ctypes.POINTER(_JsonRequest), ctypes.c_size_t, ctypes.POINTER(vp)]
     L.lb_exports_get.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_size_t)]
     L.lb_exports_free.argtypes = [vp]
     L.lb_doc_vv.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(ctypes.POINTER(_IdSpan)), ctypes.POINTER(ctypes.c_size_t)]
@@ -215,6 +224,53 @@ class Batch:
             self._L.lb_exports_free(h)
         return out
 
+    def export_json_updates(self, i, start_vv=None, end_vv=None, peer_compression=True):
+        """LoroDoc::export_json_updates(start_vv, end_vv) of document i as JSON text (needs flags=LB_FLAG_EXPORT at
+        import).  start_vv=None is the empty version; end_vv=None is the document's oplog vv.  Versions are
+        {peer: counter}; peer_compression=False gives real peer ids and "peers": null."""
+        r = self.export_json_updates_many([(i, start_vv, end_vv, peer_compression)])[0]
+        if isinstance(r, EngineError):
+            raise r
+        return r
+
+    def export_json_updates_many(self, requests):
+        """export_json_updates for many (document, version range) requests in one call (lb_batch_export_json_updates):
+        `requests` = [(doc, start_vv, end_vv[, peer_compression]), ...], None versions as in export_json_updates.
+        Returns one entry per request: the JSON text, or the EngineError of a request that failed (returned, not raised).
+        A bad document index or a batch without LB_FLAG_EXPORT raises."""
+        requests = [tuple(r) for r in requests]
+        arr = (_JsonRequest * max(len(requests), 1))()
+        keep = []
+        for j, r in enumerate(requests):
+            doc, start_vv, end_vv = r[:3]
+            compress = r[3] if len(r) > 3 else True
+            if end_vv is None and 0 <= doc < self.n_docs:
+                end_vv = self.oplog_vv(doc)
+            s_spans, s_n = _vv_spans(start_vv)
+            e_spans, e_n = _vv_spans(end_vv)
+            keep.append((s_spans, e_spans))
+            arr[j].doc = doc
+            arr[j].start, arr[j].n_start = s_spans, s_n
+            arr[j].end, arr[j].n_end = e_spans, e_n
+            arr[j].flags = 0 if compress else LB_JSON_NO_PEER_COMPRESSION
+        h = ctypes.c_void_p()
+        _check(self._L, self._L.lb_batch_export_json_updates(self._h, arr, len(requests), ctypes.byref(h)),
+               "lb_batch_export_json_updates")
+        out = []
+        try:
+            for j in range(len(requests)):
+                p = ctypes.c_void_p()
+                n = ctypes.c_size_t()
+                rc = self._L.lb_exports_get(h, j, ctypes.byref(p), ctypes.byref(n))
+                if rc == 0:
+                    out.append(ctypes.string_at(p.value, n.value).decode("utf-8"))
+                else:
+                    msg = self._L.lb_last_error().decode(errors="replace")
+                    out.append(EngineError(f"json request {j} failed (lb_status={rc}): {msg}", rc))
+        finally:
+            self._L.lb_exports_free(h)
+        return out
+
     def json_bytes(self, i):
         p = ctypes.c_char_p()
         n = ctypes.c_size_t()
@@ -311,6 +367,23 @@ class MultiBatch:
         for p, reqs in per_part.values():
             for (k, _, _), r in zip(reqs, p.export_updates_many([(j, f) for _, j, f in reqs])):
                 out[k] = r
+        return out
+
+    def export_json_updates(self, i, start_vv=None, end_vv=None, peer_compression=True):
+        p, j = self._loc(i)
+        return p.export_json_updates(j, start_vv, end_vv, peer_compression)
+
+    def export_json_updates_many(self, requests):
+        """Batch.export_json_updates_many with every request sent to its sub-batch: one C call per sub-batch."""
+        requests = [tuple(r) for r in requests]
+        per_part = {}
+        for k, r in enumerate(requests):
+            p, j = self._loc(r[0])
+            per_part.setdefault(id(p), (p, []))[1].append((k, (j,) + r[1:]))
+        out = [None] * len(requests)
+        for p, reqs in per_part.values():
+            for (k, _), res in zip(reqs, p.export_json_updates_many([r for _, r in reqs])):
+                out[k] = res
         return out
 
     def fetch_json(self):

@@ -30,6 +30,7 @@
 #include "k_tree.cuh"
 #include "k_state.cuh"
 #include "k_export.cuh"
+#include "k_json_updates.cuh"
 #include "host_stage.hpp"
 
 static thread_local std::string g_last_error;
@@ -1162,6 +1163,154 @@ void export_requests(lb_batch* b, const lb_export_request* reqs, size_t n, lb_ex
     }
 }
 
+
+// Device bytes of JSON one writing pass produces at most (LB_JSON_STAGE_CAP overrides it, for testing: small chunks).
+// A request larger than this is written alone, in a chunk of its own size.
+u64 json_stage_cap() {
+    const char* e = getenv("LB_JSON_STAGE_CAP");
+    return e ? std::max<u64>(strtoull(e, nullptr, 10), 1) : (256ull << 20);
+}
+
+// Answers every request of lb_batch_export_json_updates (the arguments are checked) in one device pass: the import
+// store of every named document is rebuilt once (k_jx_store; it does not depend on any version), a thread per request
+// orders and lists its output changes (k_jx_order), a thread per output change counts its bytes (k_jx_changes), the host
+// scans the sizes and places the requests, and the changes and envelopes are written chunk by chunk, each chunk at most
+// json_stage_cap() bytes.  Each version becomes the request's refined vectors over the document's peer slots
+// (json_schema.rs:31-45: a peer the document lacks contributes nothing, counters are clamped to the oplog vv).
+void json_requests(lb_batch* b, const lb_json_request* reqs, size_t n, lb_exports& e) {
+    e.answers.assign(n, lb_exports::Answer{LB_OK, nullptr, nullptr, 0});
+    const u32 D = (u32)b->n_docs;
+    std::vector<JxReq> jr;
+    std::vector<size_t> of;            // device request -> request
+    std::vector<i32> h_start, h_end;
+    std::vector<u8> h_req(D, 0);
+    for (size_t i = 0; i < n; i++) {
+        const size_t doc = reqs[i].doc;
+        const DocInfo& di = b->docs[doc];
+        if (di.code != DOC_OK) { e.answers[i] = doc_error(di); continue; }
+        const DocPeer* dp = &b->dpeer[b->peer_base[doc]];
+        auto refine = [&](const lb_id_span* v, size_t nv, std::vector<i32>& out) {
+            const size_t base = out.size();
+            out.resize(base + di.P, 0);
+            for (size_t k = 0; k < nv; k++)   // the last span for a peer wins
+                for (u32 p = 0; p < di.P; p++)
+                    if (dp[p].id == v[k].peer) out[base + p] = std::max(0, std::min(v[k].end, dp[p].end_counter));
+        };
+        refine(reqs[i].start, reqs[i].n_start, h_start);
+        refine(reqs[i].end, reqs[i].n_end, h_end);
+        JxReq r{};
+        r.doc = (u32)doc;
+        r.flags = reqs[i].flags & JX_NO_PEER_COMPRESSION;
+        r.slot0 = h_start.size() - di.P;
+        jr.push_back(r);
+        of.push_back(i);
+        h_req[doc] = 1;
+    }
+    if (jr.empty()) return;
+    Dev& dv = b->dev;
+    cudaStream_t st = dv.stream;
+    const u64 NCH = b->n_changes, NR = jr.size(), S = std::max<size_t>(h_start.size(), 1);
+    BatchTables xt = b->tb;
+    u8* d_req = dv.alloc<u8>(D);
+    JxReq* d_jr = dv.alloc<JxReq>(NR);
+    JxScratch s{dv.alloc<i32>(S), dv.alloc<i32>(S), dv.alloc<u32>(S), dv.alloc<u32>(S), dv.alloc<u32>(S)};
+    u32* d_pf0 = dv.alloc<u32>(b->n_peers_tot + 1);
+    u32* d_pfn = dv.alloc<u32>(b->n_peers_tot + 1);
+    CK(cudaMemcpyAsync(d_req, h_req.data(), D, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(s.start, h_start.data(), sizeof(i32) * h_start.size(), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(s.end, h_end.data(), sizeof(i32) * h_end.size(), cudaMemcpyHostToDevice, st));
+    xt.x_req = d_req;
+    xt.from_ctr = nullptr;
+    xt.xdoc = dv.alloc<XDoc>(D + 1, true);
+    LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, xt);
+    if (NCH) {
+        LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 0);
+        LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 1);
+    }
+    LB_BATCH_LAUNCH(b, k_jx_store, nblk(D, 64), 64, 0, b->d_docs, D, xt, d_pf0, d_pfn);
+    // every request gets as many output slots as its document has stored changes
+    std::vector<XDoc> xd(D);
+    CK(cudaMemcpyAsync(xd.data(), xt.xdoc, sizeof(XDoc) * D, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    trace_point(b, "json: import store");
+    u64 slots = 0;
+    for (JxReq& r : jr) { r.ch0 = slots; slots += (xd[r.doc].flags & 1) ? 0 : xd[r.doc].n_fc; }
+    u32* d_och = dv.alloc<u32>(std::max<u64>(slots, 1));
+    CK(cudaMemcpyAsync(d_jr, jr.data(), sizeof(JxReq) * NR, cudaMemcpyHostToDevice, st));
+    LB_BATCH_LAUNCH(b, k_jx_order, nblk(NR, 64), 64, 0, b->d_docs, xt, d_jr, (u32)NR, s, d_pf0, d_pfn, d_och);
+    CK(cudaMemcpyAsync(jr.data(), d_jr, sizeof(JxReq) * NR, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    trace_point(b, "json: order");
+    // the output changes of all requests, numbered consecutively; a thread per change counts its bytes
+    u64 NOUT = 0;
+    for (JxReq& r : jr) { r.c0 = NOUT; NOUT += r.n_out; }
+    std::vector<u32> h_oreq(std::max<u64>(NOUT, 1));
+    for (u64 r = 0; r < NR; r++) std::fill(h_oreq.begin() + jr[r].c0, h_oreq.begin() + jr[r].c0 + jr[r].n_out, (u32)r);
+    u32* d_oreq = dv.alloc<u32>(h_oreq.size());
+    u32* d_olen = dv.alloc<u32>(h_oreq.size());
+    u64* d_ooff = dv.alloc<u64>(h_oreq.size());
+    CK(cudaMemcpyAsync(d_jr, jr.data(), sizeof(JxReq) * NR, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_oreq, h_oreq.data(), sizeof(u32) * h_oreq.size(), cudaMemcpyHostToDevice, st));
+    std::vector<u32> h_olen(h_oreq.size(), 0);
+    if (NOUT) {
+        LB_BATCH_LAUNCH(b, k_jx_changes, nblk(NOUT, 64), 64, 0, b->d_docs, xt, d_jr, s, d_pf0, d_pfn, d_och, d_oreq, 0ull, NOUT,
+                        d_olen, (const u64*)nullptr, (u8*)nullptr, 0ull);
+        CK(cudaMemcpyAsync(h_olen.data(), d_olen, sizeof(u32) * NOUT, cudaMemcpyDeviceToHost, st));
+    }
+    CK(cudaStreamSynchronize(st));
+    trace_point(b, "json: count");
+    // place the requests and their changes: envelope head, the changes, "]}"
+    std::vector<u64> h_ooff(h_oreq.size(), 0);
+    u64 total = 0;
+    for (JxReq& r : jr) {
+        r.off = total;
+        if (r.len == JX_UNSUPPORTED) continue;
+        u64 w = total + r.pre_len;
+        for (u64 k = r.c0; k < r.c0 + r.n_out; k++) { h_ooff[k] = w; w += h_olen[k]; }
+        r.len = w + 2 - total;
+        total += r.len;
+    }
+    CK(cudaMemcpyAsync(d_jr, jr.data(), sizeof(JxReq) * NR, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_ooff, h_ooff.data(), sizeof(u64) * h_ooff.size(), cudaMemcpyHostToDevice, st));
+    e.bufs.emplace_back(new uint8_t[total + 1]);
+    uint8_t* host = e.bufs.back().get();
+    const u64 cap = json_stage_cap();
+    u8* d_out = nullptr;
+    u64 d_out_cap = 0;
+    for (u64 r0 = 0; r0 < NR;) {
+        u64 r1 = r0, bytes = 0;
+        while (r1 < NR) {
+            const u64 len = jr[r1].len == JX_UNSUPPORTED ? 0 : jr[r1].len;
+            if (r1 > r0 && bytes + len > cap) break;
+            bytes += len;
+            r1++;
+        }
+        if (bytes > d_out_cap) {
+            if (d_out) dv.release(d_out);
+            d_out = dv.alloc<u8>(bytes);
+            d_out_cap = bytes;
+        }
+        const u64 base = jr[r0].off, k0 = jr[r0].c0, k1 = jr[r1 - 1].c0 + jr[r1 - 1].n_out;
+        if (k1 > k0)
+            LB_BATCH_LAUNCH(b, k_jx_changes, nblk(k1 - k0, 64), 64, 0, b->d_docs, xt, d_jr, s, d_pf0, d_pfn, d_och, d_oreq, k0, k1,
+                            (u32*)nullptr, d_ooff, d_out, base);
+        LB_BATCH_LAUNCH(b, k_jx_envelope, nblk(r1 - r0, 64), 64, 0, b->d_docs, xt, d_jr, (u32)r0, (u32)r1, s, d_pf0, d_pfn,
+                        d_out, base);
+        if (bytes && !lbstage::download(d_out, host + base, bytes, st)) { g_last_error = "json d2h failed"; throw lb_status(LB_ERR_CUDA); }
+        CK(cudaStreamSynchronize(st));
+        r0 = r1;
+    }
+    trace_point(b, "json: write");
+    for (u64 k = 0; k < NR; k++) {
+        if (jr[k].len == JX_UNSUPPORTED) e.answers[of[k]] = lb_exports::Answer{LB_ERR_UNSUPPORTED, ERR_NOT_COVERED, nullptr, 0};
+        else e.answers[of[k]] = lb_exports::Answer{LB_OK, nullptr, host + jr[k].off, (size_t)jr[k].len};
+    }
+    if (d_out) dv.release(d_out);
+    dv.release(d_req); dv.release(d_jr); dv.release(s.start); dv.release(s.end); dv.release(s.reg); dv.release(s.ord);
+    dv.release(s.cur); dv.release(d_pf0); dv.release(d_pfn); dv.release(xt.xdoc); dv.release(d_och); dv.release(d_oreq);
+    dv.release(d_olen); dv.release(d_ooff);
+}
+
 }  // namespace
 
 // After an import into a docset: every document of the batch whose import succeeded gets its new stored form -- the
@@ -1579,6 +1728,29 @@ lb_status lb_batch_export_updates(const lb_batch* cb, const lb_export_request* r
     std::lock_guard<std::mutex> g(b->export_mu);
     try {
         export_requests(b, reqs, n_reqs, *e);
+    } catch (lb_status s) {
+        return s;
+    }
+    *out = e.release();
+    return LB_OK;
+}
+
+lb_status lb_batch_export_json_updates(const lb_batch* cb, const lb_json_request* reqs, size_t n_reqs, lb_exports** out) {
+    lb_batch* b = const_cast<lb_batch*>(cb);
+    if (!b || !out || (!reqs && n_reqs)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
+    *out = nullptr;
+    if (!(b->flags & LB_FLAG_EXPORT)) { g_last_error = "batch was imported without LB_FLAG_EXPORT"; return LB_ERR_INVALID_ARG; }
+    for (size_t i = 0; i < n_reqs; i++) {
+        if (reqs[i].doc >= b->n_docs) { g_last_error = "document index out of range"; return LB_ERR_INVALID_ARG; }
+        if ((!reqs[i].start && reqs[i].n_start) || (!reqs[i].end && reqs[i].n_end)) {
+            g_last_error = "null version with a count > 0";
+            return LB_ERR_INVALID_ARG;
+        }
+    }
+    std::unique_ptr<lb_exports> e(new lb_exports());
+    std::lock_guard<std::mutex> g(b->export_mu);
+    try {
+        json_requests(b, reqs, n_reqs, *e);
     } catch (lb_status s) {
         return s;
     }
