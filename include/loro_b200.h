@@ -18,6 +18,8 @@
  *   lb_doc_export_updates    crates/loro/src/lib.rs:1235 LoroDoc::export(ExportMode::all_updates() / updates(from))
  *                            crates/loro-internal/src/encoding.rs:79-83, 350-416, oplog/change_store.rs:494-576
  *   lb_batch_export_updates  the same export for many (document, from) requests in one call
+ *   lb_batch_export_updates_in_range  crates/loro-internal/src/encoding.rs:52-151 ExportMode::UpdatesInRange / updates_till
+ *                            (oplog/change_store.rs:179-199), many (document, spans) requests per call
  *   lb_batch_export_json_updates  crates/loro/src/lib.rs:687-720 LoroDoc::export_json_updates(start_vv, end_vv)
  *                            (crates/loro-internal/src/loro.rs:715-751, encoding/json_schema.rs), many requests per call
  *   lb_docset_import         crates/loro/src/lib.rs:639, :425 on a document that already holds history
@@ -184,6 +186,28 @@ typedef struct lb_exports lb_exports;
 lb_status lb_batch_export_updates(const lb_batch* b, const lb_export_request* reqs, size_t n_reqs, lb_exports** out);
 lb_status lb_exports_get(const lb_exports* e, size_t i, const uint8_t** bytes, size_t* len);
 void lb_exports_free(lb_exports* e);
+/* Many LoroDoc::export(ExportMode::UpdatesInRange { spans }) in one call (crates/loro-internal/src/encoding.rs:52-151,
+ * oplog/change_store.rs:179-199 export_blocks_in_range): the FastUpdates blob of exactly the changes in the named id
+ * spans, each stored change cut at both ends (Change::slice).  ExportMode::updates_till(vv) is one span [0, vv[p]) per
+ * peer.  Spans are taken in request order.  A reversed span (start > end) covers end+1 .. start+1 (IdSpan::normalize_);
+ * a span that is empty, starts below 0, or names a peer the document lacks selects nothing; one past the oplog vv is cut
+ * there; a request that selects nothing gets a header-only blob.  Request order decides block boundaries: a span
+ * continues the block of an earlier-listed span of its peer that ends exactly at its start, and otherwise starts a new
+ * block.  The reference panics ("counter should be continuous") or stores changes twice when a peer's spans overlap, or
+ * when an earlier-listed span of the peer lies below a span's start without ending there: the engine answers such a
+ * request with LB_ERR_INVALID_ARG (lb_exports_get, with the reason in lb_last_error) and still answers the others.
+ * Everything else follows lb_batch_export_updates: per request, LB_ERR_INVALID_ARG for a document that failed to import
+ * and LB_ERR_UNSUPPORTED for one the export phase does not cover; equal span sets of one document are computed once, one
+ * that selects [0, vv[p]) of every peer is the import-time blob and launches nothing, the rest run in rounds whose number
+ * is the largest number of distinct span sets asked of one document; the whole call fails with LB_ERR_INVALID_ARG,
+ * launching nothing, for a `doc` out of range, `spans` NULL with n_spans > 0, or a batch imported without
+ * LB_FLAG_EXPORT. */
+typedef struct lb_range_request {
+    size_t doc;               /* document index in the batch */
+    const lb_id_span* spans;  /* (peer, start, end): counters [start, end) of the peer */
+    size_t n_spans;
+} lb_range_request;
+lb_status lb_batch_export_updates_in_range(const lb_batch* b, const lb_range_request* reqs, size_t n_reqs, lb_exports** out);
 /* LoroDoc::export_json_updates(start_vv, end_vv) (crates/loro/src/lib.rs:687-720, crates/loro-internal/src/loro.rs:715-751,
  * encoding/json_schema.rs): the changes of document `doc` between two versions in the JSON schema of docs/JsonSchema.md,
  * as serde_json::to_string prints it -- UTF-8 without a terminator, returned through lb_exports_get.  Both versions are

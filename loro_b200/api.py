@@ -48,6 +48,10 @@ class _ExportRequest(ctypes.Structure):
     _fields_ = [("doc", ctypes.c_size_t), ("from_", ctypes.POINTER(_IdSpan)), ("n_from", ctypes.c_size_t)]
 
 
+class _RangeRequest(ctypes.Structure):
+    _fields_ = [("doc", ctypes.c_size_t), ("spans", ctypes.POINTER(_IdSpan)), ("n_spans", ctypes.c_size_t)]
+
+
 class _JsonRequest(ctypes.Structure):
     _fields_ = [("doc", ctypes.c_size_t), ("start", ctypes.POINTER(_IdSpan)), ("n_start", ctypes.c_size_t),
                 ("end", ctypes.POINTER(_IdSpan)), ("n_end", ctypes.c_size_t), ("flags", ctypes.c_uint32)]
@@ -106,6 +110,7 @@ def load_library(path=None):
                                         ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_size_t)]
     L.lb_batch_export_updates.argtypes = [vp, ctypes.POINTER(_ExportRequest), ctypes.c_size_t, ctypes.POINTER(vp)]
     L.lb_batch_export_json_updates.argtypes = [vp, ctypes.POINTER(_JsonRequest), ctypes.c_size_t, ctypes.POINTER(vp)]
+    L.lb_batch_export_updates_in_range.argtypes = [vp, ctypes.POINTER(_RangeRequest), ctypes.c_size_t, ctypes.POINTER(vp)]
     L.lb_exports_get.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_size_t)]
     L.lb_exports_free.argtypes = [vp]
     L.lb_doc_vv.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(ctypes.POINTER(_IdSpan)), ctypes.POINTER(ctypes.c_size_t)]
@@ -209,17 +214,56 @@ class Batch:
         h = ctypes.c_void_p()
         _check(self._L, self._L.lb_batch_export_updates(self._h, arr, len(requests), ctypes.byref(h)),
                "lb_batch_export_updates")
+        return self._exports(h, len(requests), "export request")
+
+    def export_updates_in_range(self, i, spans):
+        """LoroDoc::export(ExportMode::UpdatesInRange { spans }) of document i (needs flags=LB_FLAG_EXPORT at import):
+        the changes in `spans` = [(peer, start, end), ...], counters [start, end), taken in the order given."""
+        r = self.export_updates_in_range_many([(i, spans)])[0]
+        if isinstance(r, EngineError):
+            raise r
+        return r
+
+    def export_updates_till(self, i, vv):
+        """LoroDoc::export(ExportMode::updates_till(vv)) of document i: one span [0, vv[peer]) per peer
+        (encoding.rs:140-151)."""
+        return self.export_updates_in_range(i, _till_spans(vv))
+
+    def export_updates_in_range_many(self, requests):
+        """export_updates_in_range for many (document, spans) requests in one call (lb_batch_export_updates_in_range).
+        Returns one entry per request: the bytes, or the EngineError of a request that failed or was refused (returned,
+        not raised).  A bad document index or a batch without LB_FLAG_EXPORT raises."""
+        requests = list(requests)
+        arr = (_RangeRequest * max(len(requests), 1))()
+        keep = []
+        for j, (doc, spans) in enumerate(requests):
+            spans = list(spans)
+            sp = (_IdSpan * max(len(spans), 1))()
+            for k, (peer, start, end) in enumerate(spans):
+                sp[k].peer, sp[k].start, sp[k].end = int(peer), int(start), int(end)
+            keep.append(sp)
+            arr[j].doc = doc
+            arr[j].spans = sp
+            arr[j].n_spans = len(spans)
+        h = ctypes.c_void_p()
+        _check(self._L, self._L.lb_batch_export_updates_in_range(self._h, arr, len(requests), ctypes.byref(h)),
+               "lb_batch_export_updates_in_range")
+        return self._exports(h, len(requests), "range request")
+
+    def _exports(self, h, n, what, text=False):
+        """the n answers of an lb_exports (freed here): bytes (text: str), or the EngineError of a failed request"""
         out = []
         try:
-            for j in range(len(requests)):
+            for j in range(n):
                 p = ctypes.c_void_p()
-                n = ctypes.c_size_t()
-                rc = self._L.lb_exports_get(h, j, ctypes.byref(p), ctypes.byref(n))
+                ln = ctypes.c_size_t()
+                rc = self._L.lb_exports_get(h, j, ctypes.byref(p), ctypes.byref(ln))
                 if rc == 0:
-                    out.append(ctypes.string_at(p.value, n.value))
+                    b = ctypes.string_at(p.value, ln.value)
+                    out.append(b.decode("utf-8") if text else b)
                 else:
                     msg = self._L.lb_last_error().decode(errors="replace")
-                    out.append(EngineError(f"export request {j} failed (lb_status={rc}): {msg}", rc))
+                    out.append(EngineError(f"{what} {j} failed (lb_status={rc}): {msg}", rc))
         finally:
             self._L.lb_exports_free(h)
         return out
@@ -256,20 +300,7 @@ class Batch:
         h = ctypes.c_void_p()
         _check(self._L, self._L.lb_batch_export_json_updates(self._h, arr, len(requests), ctypes.byref(h)),
                "lb_batch_export_json_updates")
-        out = []
-        try:
-            for j in range(len(requests)):
-                p = ctypes.c_void_p()
-                n = ctypes.c_size_t()
-                rc = self._L.lb_exports_get(h, j, ctypes.byref(p), ctypes.byref(n))
-                if rc == 0:
-                    out.append(ctypes.string_at(p.value, n.value).decode("utf-8"))
-                else:
-                    msg = self._L.lb_last_error().decode(errors="replace")
-                    out.append(EngineError(f"json request {j} failed (lb_status={rc}): {msg}", rc))
-        finally:
-            self._L.lb_exports_free(h)
-        return out
+        return self._exports(h, len(requests), "json request", text=True)
 
     def json_bytes(self, i):
         p = ctypes.c_char_p()
@@ -366,6 +397,22 @@ class MultiBatch:
         out = [None] * len(requests)
         for p, reqs in per_part.values():
             for (k, _, _), r in zip(reqs, p.export_updates_many([(j, f) for _, j, f in reqs])):
+                out[k] = r
+        return out
+
+    def export_updates_in_range(self, i, spans): p, j = self._loc(i); return p.export_updates_in_range(j, spans)
+    def export_updates_till(self, i, vv): p, j = self._loc(i); return p.export_updates_till(j, vv)
+
+    def export_updates_in_range_many(self, requests):
+        """Batch.export_updates_in_range_many with every request sent to its sub-batch: one C call per sub-batch."""
+        requests = list(requests)
+        per_part = {}
+        for k, (i, spans) in enumerate(requests):
+            p, j = self._loc(i)
+            per_part.setdefault(id(p), (p, []))[1].append((k, j, spans))
+        out = [None] * len(requests)
+        for p, reqs in per_part.values():
+            for (k, _, _), r in zip(reqs, p.export_updates_in_range_many([(j, s) for _, j, s in reqs])):
                 out[k] = r
         return out
 
@@ -516,6 +563,11 @@ def import_batch_at(blobs, versions, doc_ids=None, device=0, flags=0, lib_path=N
     _check(L, L.lb_import_batch_at(arr, len(blobs), ver, len(versions), ctypes.byref(opt), ctypes.byref(h)),
            "lb_import_batch_at")
     return Batch(L, h.value)
+
+
+def _till_spans(vv):
+    """ExportMode::updates_till(vv) as spans (encoding.rs:140-151): [0, vv[peer]) for every peer of vv"""
+    return [(p, 0, c) for p, c in dict(vv or {}).items()]
 
 
 def _vv_spans(from_vv):

@@ -349,6 +349,7 @@ struct lb_batch {
     uint8_t* exported = nullptr;  // malloc'ed host copy (lbstage::download)
     bool export_fetched = false;
     u64 n_blocks = 0, n_changes = 0, n_rows = 0, n_peers_tot = 0, json_total = 0, n_deps = 0;
+    u64 n_segs = 0, fc_cap = 0;   // phase 7: segments (changes + extra segments of split ones), fc_* table capacity
     // host results
     std::vector<DocInfo> docs;
     std::vector<DocPeer> dpeer;          // packed: document d owns [peer_base[d], peer_base[d] + P)
@@ -409,11 +410,22 @@ inline unsigned nblk(u64 n, int tpb = TPB) { return (unsigned)((n + tpb - 1) / t
         (b)->timings.kernel_launches++;                                             \
     } while (0)
 
+// the u32 segment and final-change tables of phase 7, for its allocation and the growth paths
+u32* BatchTables::* const SG_TABLES[] = {
+    &BatchTables::sg_src, &BatchTables::sg_r0, &BatchTables::sg_from, &BatchTables::sg_atoms, &BatchTables::sg_est,
+    &BatchTables::sg_nmops, &BatchTables::sg_ndel, &BatchTables::sg_nrows, &BatchTables::sg_last_head, &BatchTables::sg_skip};
+u32* BatchTables::* const FC_TABLES[] = {
+    &BatchTables::fc_src, &BatchTables::fc_pos, &BatchTables::fc_r0, &BatchTables::fc_from, &BatchTables::fc_atoms,
+    &BatchTables::fc_nrows, &BatchTables::fc_ndel, &BatchTables::fc_skip, &BatchTables::fc_tail, &BatchTables::fc_est};
+
 // the export encoder over NOB output blocks (retry = 1: only the blocks that outgrew their staging slot, into their
-// retry slots), in the build that is faster for that many (k_export.cuh)
-void launch_exp_encode(lb_batch* b, u64 NOB, const BatchTables& xt, XBlock* xb, u32* xscratch, u8* out, int retry) {
+// retry slots), in the build that is faster for that many (k_export.cuh); cuts: some change is cut at the end of its span
+void launch_exp_encode(lb_batch* b, u64 NOB, const BatchTables& xt, XBlock* xb, u32* xscratch, u8* out, int retry, bool cuts) {
     if (!NOB) return;
-    if (NOB >= LB_XENC_BOUNDED_MIN_BLOCKS) LB_BATCH_LAUNCH(b, k_exp_encode<1>, nblk(NOB, 64), 64, 0, b->d_docs, NOB, xt, xb, xscratch, out, retry);
+    const bool capped = NOB >= LB_XENC_BOUNDED_MIN_BLOCKS;
+    if (cuts && capped) LB_BATCH_LAUNCH(b, k_exp_encode_cut<1>, nblk(NOB, 64), 64, 0, b->d_docs, NOB, xt, xb, xscratch, out, retry);
+    else if (cuts) LB_BATCH_LAUNCH(b, k_exp_encode_cut<0>, nblk(NOB, 64), 64, 0, b->d_docs, NOB, xt, xb, xscratch, out, retry);
+    else if (capped) LB_BATCH_LAUNCH(b, k_exp_encode<1>, nblk(NOB, 64), 64, 0, b->d_docs, NOB, xt, xb, xscratch, out, retry);
     else LB_BATCH_LAUNCH(b, k_exp_encode<0>, nblk(NOB, 64), 64, 0, b->d_docs, NOB, xt, xb, xscratch, out, retry);
 }
 
@@ -483,8 +495,9 @@ void run_scans(lb_batch* b, std::vector<ScanJob> jobs) {
 // layout (the lengths are exact, so are the offsets and the retry slots), the encode again of the blocks that outgrew
 // their slot, into retry slots of their exact size (only when there are any: the retry bytes come back with the blob
 // sizes), then the blobs assembled per document.
+// cuts: some span of the pass ends inside a change (the encoder build that honours fc_tail).
 // Returns the export buffer (*total bytes, document d's blob at xt.xdoc[d].exp_off).
-u8* export_encode(lb_batch* b, const BatchTables& xt, u64* total) {
+u8* export_encode(lb_batch* b, const BatchTables& xt, u64* total, bool cuts) {
     Dev& dv = b->dev;
     const u32 D = (u32)b->n_docs;
     u32* cnt = dv.alloc<u32>(3 * (u64)(D + 1));
@@ -502,7 +515,7 @@ u8* export_encode(lb_batch* b, const BatchTables& xt, u64* total) {
     const u32 stage_max = cap_env ? (u32)strtoul(cap_env, nullptr, 10) : 0xFFFFFFFFu;
     trace_point(b, "store+sizes");
     LB_BATCH_LAUNCH(b, k_exp_list, nblk(D), TPB, 0, b->d_docs, D, xt, xb, stage_max);
-    launch_exp_encode(b, NOB, xt, xb, xscratch, xstage, 0);
+    launch_exp_encode(b, NOB, xt, xb, xscratch, xstage, 0, cuts);
     LB_BATCH_LAUNCH(b, k_exp_layout, nblk(D), TPB, 0, b->d_docs, D, xt, xb, n_a, n_b, n_c);
     trace_point(b, "encode");
     run_scans(b, {ScanJob{(const u8*)n_a, (u8*)xt.xdoc + offsetof(XDoc, exp_off), 4, sizeof(XDoc), D},
@@ -519,7 +532,7 @@ u8* export_encode(lb_batch* b, const BatchTables& xt, u64* total) {
     u8* xrestage = nullptr;
     if (NOVF) {
         xrestage = dv.alloc<u8>(NRST + 16);
-        launch_exp_encode(b, NOB, xt, xb, xscratch, xrestage, 1);
+        launch_exp_encode(b, NOB, xt, xb, xscratch, xrestage, 1, cuts);
     }
     LB_BATCH_LAUNCH(b, k_exp_finish, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, xt, xb, xstage, xrestage, out);
     trace_point(b, "assemble");
@@ -805,20 +818,14 @@ void pipeline(lb_batch* b) {
         // extras are counted by pass 0, so the arrays are sized with a bound first and checked after the scan
         u64 SEGCAP = NCH + NCH / 4 + 1024;
         if (getenv("LB_EXPORT_TIGHT_SEGCAP")) SEGCAP = NCH;   // testing hook: force the growth path
-        // the u32 tables of the two groups, in allocation order, for here and for the growth path below; the *_skip
-        // tables start zeroed, and fc_block (the one byte-wide table) has its place before fc_skip
-        static u32* BatchTables::* const SG_TABLES[] = {
-            &BatchTables::sg_src, &BatchTables::sg_r0, &BatchTables::sg_from, &BatchTables::sg_atoms, &BatchTables::sg_est,
-            &BatchTables::sg_nmops, &BatchTables::sg_ndel, &BatchTables::sg_nrows, &BatchTables::sg_last_head, &BatchTables::sg_skip};
-        static u32* BatchTables::* const FC_TABLES[] = {
-            &BatchTables::fc_src, &BatchTables::fc_pos, &BatchTables::fc_r0, &BatchTables::fc_from, &BatchTables::fc_atoms,
-            &BatchTables::fc_nrows, &BatchTables::fc_ndel, &BatchTables::fc_skip, &BatchTables::fc_est};
+        // the u32 tables of the two groups (SG_TABLES, FC_TABLES) in allocation order; the *_skip and fc_tail tables
+        // start zeroed, and fc_block (the one byte-wide table) has its place before fc_skip
         for (auto m : SG_TABLES) t.*m = dv.alloc<u32>(SEGCAP, m == &BatchTables::sg_skip);
         for (auto m : FC_TABLES) {
             if (m == &BatchTables::fc_skip) t.fc_block = dv.alloc<u8>(SEGCAP);
-            t.*m = dv.alloc<u32>(SEGCAP, m == &BatchTables::fc_skip);
+            t.*m = dv.alloc<u32>(SEGCAP, m == &BatchTables::fc_skip || m == &BatchTables::fc_tail);
         }
-        t.x_req = nullptr; t.from_ctr = nullptr;
+        t.x_req = nullptr; t.x_span0 = nullptr; t.x_spans = nullptr;
         trace_point(b, "export allocs");
         LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, t);
         if (NTR) LB_BATCH_LAUNCH(b, k_exp_posrank, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t);
@@ -845,10 +852,12 @@ void pipeline(lb_batch* b) {
             dv.release(t.fc_block);
             t.fc_block = dv.alloc<u8>(cap);
         }
+        b->n_segs = NCH + NOVF;
+        b->fc_cap = std::max(SEGCAP, NCH + NOVF);
         if (NOVF) LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, t, 1);
         LB_BATCH_LAUNCH(b, k_exp_store, nblk(D, 64), 64, 0, b->d_docs, D, t);
         u64 XT = 0;
-        b->d_export = export_encode(b, t, &XT);
+        b->d_export = export_encode(b, t, &XT, false);
         b->export_total = XT;
         tm.export_bytes = XT;
     }
@@ -1055,27 +1064,39 @@ lb_exports::Answer doc_error(const DocInfo& di) {
     return lb_exports::Answer{LB_ERR_INVALID_ARG, ERR_FAILED_DOC, nullptr, 0};
 }
 
-// One pass of export(ExportMode::updates(from)) (encoding.rs:79-83 ; change_store.rs:494-528 export_blocks_from) over
-// the documents of a round, at most one version each: the import store of each marked document is rebuilt, its changes
-// are cut at the document's `from` (Change::slice) on their way into a fresh export store, and the result is encoded
-// like the import-time export.  The phase-7 tables of the batch are reused; only the per-pass pieces (cut positions,
-// request mask, block list, scratch, output) are allocated.  The stores rewrite the rows' flags (k_exp_store merges ops
-// across changes), which is why a document can be in one request per pass only.
-// h_from: first counter to export per batch peer slot; h_req: the request mask.  Returns the round's packed blobs in
-// host memory, with the XDoc table that places them (exp_off / exp_len of every marked document).
-std::unique_ptr<uint8_t[]> export_round(lb_batch* b, const std::vector<i32>& h_from, const std::vector<u8>& h_req,
-                                        std::vector<XDoc>& xd) {
+// One pass of the export of chosen id spans (change_store.rs:179-199 export_blocks_in_range, :494-528
+// export_blocks_from) over the documents of a round, one span set each: the import store of each marked document is
+// rebuilt, its changes are cut to the document's spans (Change::slice at both ends) on their way into a fresh export
+// store, and the result is encoded like the import-time export.  The phase-7 tables of the batch are reused; only the
+// per-pass pieces (span table, request mask, block list, scratch, output) are allocated.  The stores rewrite the rows'
+// flags (k_exp_store merges ops across changes), which is why a document can be in one request per pass only.
+// h_span0 / h_spans: the span table over the batch's peer slots (BatchTables::x_span0); cuts: some span ends below its
+// peer's vv; h_req: the request mask.
+// Returns the round's packed blobs in host memory, with the XDoc table that places them (exp_off / exp_len of every
+// marked document).
+std::unique_ptr<uint8_t[]> export_round(lb_batch* b, const std::vector<u32>& h_span0, const std::vector<XSpan>& h_spans,
+                                        bool cuts, const std::vector<u8>& h_req, std::vector<XDoc>& xd) {
     Dev& dv = b->dev;
     cudaStream_t st = dv.stream;
     const u32 D = (u32)b->n_docs;
     const u64 NCH = b->n_changes;
+    // a document's final changes get one slot per segment and one per span (xfc0): grow the tables when a round needs more
+    if (b->n_segs + h_spans.size() > b->fc_cap) {
+        b->fc_cap = b->n_segs + h_spans.size();
+        for (auto m : FC_TABLES) { dv.release(b->tb.*m); b->tb.*m = dv.alloc<u32>(b->fc_cap, true); }
+        dv.release(b->tb.fc_block);
+        b->tb.fc_block = dv.alloc<u8>(b->fc_cap);
+    }
     BatchTables xt = b->tb;
-    i32* d_from = dv.alloc<i32>(h_from.size());
+    u32* d_span0 = dv.alloc<u32>(h_span0.size());
+    XSpan* d_spans = dv.alloc<XSpan>(std::max<size_t>(h_spans.size(), 1));
     u8* d_req = dv.alloc<u8>(D);
-    CK(cudaMemcpyAsync(d_from, h_from.data(), sizeof(i32) * h_from.size(), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_span0, h_span0.data(), sizeof(u32) * h_span0.size(), cudaMemcpyHostToDevice, st));
+    if (!h_spans.empty()) CK(cudaMemcpyAsync(d_spans, h_spans.data(), sizeof(XSpan) * h_spans.size(), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_req, h_req.data(), D, cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));   // pageable host memory
-    xt.from_ctr = d_from;
+    xt.x_span0 = d_span0;
+    xt.x_spans = d_spans;
     xt.x_req = d_req;
     xt.xdoc = dv.alloc<XDoc>(D + 1, true);
     LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, xt);
@@ -1085,53 +1106,64 @@ std::unique_ptr<uint8_t[]> export_round(lb_batch* b, const std::vector<i32>& h_f
     }
     LB_BATCH_LAUNCH(b, k_exp_store, nblk(D, 64), 64, 0, b->d_docs, D, xt);
     u64 XT = 0;
-    u8* d_out = export_encode(b, xt, &XT);
+    u8* d_out = export_encode(b, xt, &XT, cuts);
     xd.resize(D);
     CK(cudaMemcpyAsync(xd.data(), xt.xdoc, sizeof(XDoc) * D, cudaMemcpyDeviceToHost, st));
     std::unique_ptr<uint8_t[]> out(new uint8_t[XT + 1]);
     if (!lbstage::download(d_out, out.get(), XT, st)) { g_last_error = "export d2h failed"; throw lb_status(LB_ERR_CUDA); }
     CK(cudaStreamSynchronize(st));
-    dv.release(d_from); dv.release(d_req); dv.release(xt.xdoc); dv.release(d_out);
+    dv.release(d_span0); dv.release(d_spans); dv.release(d_req); dv.release(xt.xdoc); dv.release(d_out);
     return out;
 }
 
-// Answers every request of lb_batch_export_updates (the arguments are checked).  Each `from` becomes its document's
-// vector over the document's peer slots; equal vectors of one document are answered once, the all-zero vector from the
-// import-time export, and the rest in rounds: round r holds the r-th distinct vector of every document, so the number of
-// passes is the largest number of distinct versions asked of one document, whatever the number of documents.
-void export_requests(lb_batch* b, const lb_export_request* reqs, size_t n, lb_exports& e) {
-    struct Version { size_t doc; u32 round; std::vector<i32> from; };
-    std::vector<Version> versions;                          // distinct (document, vector) pairs, round by round below
+// A document's span set in the form export_span_sets compares and lays out: per peer slot p of the document, the number
+// of its spans, then (start, end, fresh) of each, sorted by start.
+using SpanKey = std::vector<i32>;
+const char* const ERR_SPANS_OVERLAP = "two spans of one peer overlap (the reference would store their changes twice or panic)";
+const char* const ERR_SPANS_GAP = "a span starts above an earlier-listed span of its peer that does not end at its start "
+                                  "(the reference panics: counter should be continuous)";
+
+// Answers requests that each name a document and a span set.  key_of(i, di, peers, key) writes request i's key and
+// returns nullptr, or returns why the request is refused.  Equal keys of one document are answered once, the key that
+// selects [0, vv) of every peer from the import-time export (no launch), and the rest in rounds: round r holds the r-th
+// distinct key of every document, so the number of passes is the largest number of distinct span sets asked of one
+// document, whatever the number of documents or spans.
+template <class DocOf, class KeyOf>
+void export_span_sets(lb_batch* b, size_t n, DocOf doc_of, KeyOf key_of, lb_exports& e) {
+    struct Version { size_t doc; u32 round; SpanKey key; };
+    std::vector<Version> versions;                          // distinct (document, key) pairs, round by round below
     std::unordered_map<size_t, std::vector<u32>> of_doc;    // document -> its versions, in order of first request
-    std::vector<u32> version_of(n, ~0u);                    // request -> version; ~0: all_updates or failed document
+    std::vector<u32> version_of(n, ~0u);                    // request -> version; ~0: all_updates or an error
     e.answers.assign(n, lb_exports::Answer{LB_OK, nullptr, nullptr, 0});
     std::vector<size_t> all_updates;                        // requests answered by the import-time export
     for (size_t i = 0; i < n; i++) {
-        const size_t doc = reqs[i].doc;
+        const size_t doc = doc_of(i);
         const DocInfo& di = b->docs[doc];
         if (di.code != DOC_OK) { e.answers[i] = doc_error(di); continue; }
-        // the last span for a peer wins; peers the document lacks are ignored
-        std::vector<i32> h(di.P, 0);
-        for (size_t k = 0; k < reqs[i].n_from; k++)
-            for (u32 p = 0; p < di.P; p++)
-                if (b->dpeer[b->peer_base[doc] + p].id == reqs[i].from[k].peer) h[p] = reqs[i].from[k].end;
-        if (std::all_of(h.begin(), h.end(), [](i32 c) { return c <= 0; })) { all_updates.push_back(i); continue; }
+        const DocPeer* dp = &b->dpeer[b->peer_base[doc]];
+        SpanKey key, whole;
+        if (const char* err = key_of(i, di, dp, key)) { e.answers[i] = lb_exports::Answer{LB_ERR_INVALID_ARG, err, nullptr, 0}; continue; }
+        for (u32 p = 0; p < di.P; p++) {
+            if (dp[p].end_counter > 0) whole.insert(whole.end(), {1, 0, dp[p].end_counter, 1});
+            else whole.push_back(0);
+        }
+        if (key == whole) { all_updates.push_back(i); continue; }
         std::vector<u32>& mine = of_doc[doc];
-        for (u32 v : mine) if (versions[v].from == h) version_of[i] = v;
+        for (u32 v : mine) if (versions[v].key == key) version_of[i] = v;
         if (version_of[i] == ~0u) {
             version_of[i] = (u32)versions.size();
-            versions.push_back(Version{doc, (u32)mine.size(), std::move(h)});
+            versions.push_back(Version{doc, (u32)mine.size(), std::move(key)});
             mine.push_back(version_of[i]);
         }
     }
     // all_updates: the document's blob of the import-time export, copied out of the batch's export buffer
     if (!all_updates.empty()) {
         u64 total = 0;
-        for (size_t i : all_updates) total += b->xdocs[reqs[i].doc].exp_len;
+        for (size_t i : all_updates) total += b->xdocs[doc_of(i)].exp_len;
         e.bufs.emplace_back(new uint8_t[total + 1]);
         uint8_t* w = e.bufs.back().get();
         for (size_t i : all_updates) {
-            const XDoc& x = b->xdocs[reqs[i].doc];
+            const XDoc& x = b->xdocs[doc_of(i)];
             if ((x.flags & 1) || x.exp_len == 0) { e.answers[i] = lb_exports::Answer{LB_ERR_UNSUPPORTED, ERR_NOT_COVERED, nullptr, 0}; continue; }
             CK(cudaMemcpyAsync(w, b->d_export + x.exp_off, x.exp_len, cudaMemcpyDeviceToHost, b->dev.stream));
             e.answers[i].bytes = w;
@@ -1144,25 +1176,102 @@ void export_requests(lb_batch* b, const lb_export_request* reqs, size_t n, lb_ex
     for (const auto& kv : of_doc) rounds = std::max(rounds, kv.second.size());
     std::vector<XDoc> xd;
     for (size_t r = 0; r < rounds; r++) {
-        std::vector<i32> h_from(b->n_peers_tot + 1, 0);
+        std::vector<const i32*> slot_key(b->n_peers_tot, nullptr);   // peer slot -> its part of the round's key
         std::vector<u8> h_req(b->n_docs, 0);
+        bool cuts = false;
         for (const auto& kv : of_doc) {
             if (r >= kv.second.size()) continue;
             const Version& v = versions[kv.second[r]];
-            std::copy(v.from.begin(), v.from.end(), h_from.begin() + b->docs[v.doc].peer0);
+            const DocPeer* dp = &b->dpeer[b->peer_base[v.doc]];
+            const i32* k = v.key.data();
+            for (u32 p = 0; p < b->docs[v.doc].P; p++) {
+                slot_key[b->docs[v.doc].peer0 + p] = k;
+                for (i32 q = 0; q < k[0]; q++) cuts |= k[2 + 3 * q] < dp[p].end_counter;
+                k += 1 + 3 * k[0];
+            }
             h_req[v.doc] = 1;
         }
-        e.bufs.push_back(export_round(b, h_from, h_req, xd));
+        std::vector<u32> h_span0(b->n_peers_tot + 1, 0);
+        std::vector<XSpan> h_spans;
+        for (size_t slot = 0; slot < b->n_peers_tot; slot++) {
+            h_span0[slot] = (u32)h_spans.size();
+            if (const i32* k = slot_key[slot])
+                for (i32 q = 0; q < k[0]; q++) h_spans.push_back(XSpan{k[1 + 3 * q], k[2 + 3 * q], (u32)k[3 + 3 * q], 0});
+        }
+        h_span0[b->n_peers_tot] = (u32)h_spans.size();
+        e.bufs.push_back(export_round(b, h_span0, h_spans, cuts, h_req, xd));
         const uint8_t* blobs = e.bufs.back().get();
         for (size_t i = 0; i < n; i++) {
             if (version_of[i] == ~0u || versions[version_of[i]].round != r) continue;
-            const XDoc& x = xd[reqs[i].doc];
+            const XDoc& x = xd[doc_of(i)];
             if ((x.flags & 1) || x.exp_len == 0) e.answers[i] = lb_exports::Answer{LB_ERR_UNSUPPORTED, ERR_NOT_COVERED, nullptr, 0};
             else e.answers[i] = lb_exports::Answer{LB_OK, nullptr, blobs + x.exp_off, x.exp_len};
         }
     }
 }
 
+// Answers every request of lb_batch_export_updates (the arguments are checked): export(ExportMode::updates(from)) is
+// one span [from, vv) per peer (change_store.rs:494-528); the last span given for a peer wins, peers the document lacks
+// are ignored.
+void export_requests(lb_batch* b, const lb_export_request* reqs, size_t n, lb_exports& e) {
+    export_span_sets(b, n, [&](size_t i) { return reqs[i].doc; },
+                     [&](size_t i, const DocInfo& di, const DocPeer* dp, SpanKey& key) -> const char* {
+        std::vector<i32> h(di.P, 0);
+        for (size_t k = 0; k < reqs[i].n_from; k++)
+            for (u32 p = 0; p < di.P; p++)
+                if (dp[p].id == reqs[i].from[k].peer) h[p] = reqs[i].from[k].end;
+        for (u32 p = 0; p < di.P; p++) {
+            const i32 start = std::max(h[p], 0);
+            if (start < dp[p].end_counter) key.insert(key.end(), {1, start, dp[p].end_counter, 1});
+            else key.push_back(0);
+        }
+        return nullptr;
+    }, e);
+}
+
+// Answers every request of lb_batch_export_updates_in_range (the arguments are checked), as export_blocks_in_range takes
+// its spans (change_store.rs:179-199): each is normalised (span.rs:51-68: a reversed span covers end+1 .. start+1); one
+// that is empty, starts below 0 (iter_blocks then finds another peer's block), or names a peer the document lacks selects
+// nothing; the others are clamped to the oplog vv.  In request order, a span continues the block of an earlier-listed
+// span of its peer that ends exactly at its start (insert_change: the previous block by id), and starts a fresh block when
+// no earlier-listed span of its peer lies below it.  The span sets the reference panics on or stores twice are refused.
+void export_range_requests(lb_batch* b, const lb_range_request* reqs, size_t n, lb_exports& e) {
+    export_span_sets(b, n, [&](size_t i) { return reqs[i].doc; },
+                     [&](size_t i, const DocInfo& di, const DocPeer* dp, SpanKey& key) -> const char* {
+        std::vector<std::vector<XSpan>> per(di.P);   // selected spans of each peer, in request order
+        for (size_t k = 0; k < reqs[i].n_spans; k++) {
+            const lb_id_span& sp = reqs[i].spans[k];
+            u32 p = 0;
+            while (p < di.P && dp[p].id != sp.peer) p++;
+            if (p == di.P) continue;
+            i64 s = sp.start, en = sp.end;
+            if (en < s) { const i64 s2 = en + 1; en = s + 1; s = s2; }
+            if (s < 0 || s == en) continue;
+            en = std::min<i64>(en, dp[p].end_counter);
+            if (s >= en) continue;
+            per[p].push_back(XSpan{(i32)s, (i32)en, 1, (u32)per[p].size()});   // pad: the place in request order
+        }
+        for (u32 p = 0; p < di.P; p++) {
+            // sorted by start, a span's neighbour below is the only candidate for the block it continues: one listed
+            // earlier must end exactly at its start; one listed later leaves it a fresh block unless some span below it
+            // was listed earlier still (that one ends below the neighbour's start: a gap)
+            std::vector<XSpan>& v = per[p];
+            std::sort(v.begin(), v.end(), [](const XSpan& x, const XSpan& y) { return x.start < y.start; });
+            u32 first_below = ~0u;   // the earliest request place among the spans below the current one
+            for (size_t a = 0; a < v.size(); a++) {
+                if (a && v[a - 1].end > v[a].start) return ERR_SPANS_OVERLAP;
+                if (a && v[a - 1].pad < v[a].pad) {
+                    if (v[a - 1].end != v[a].start) return ERR_SPANS_GAP;
+                    v[a].fresh = 0;
+                } else if (first_below < v[a].pad) return ERR_SPANS_GAP;
+                first_below = std::min(first_below, v[a].pad);
+            }
+            key.push_back((i32)v.size());
+            for (const XSpan& x : v) key.insert(key.end(), {x.start, x.end, (i32)x.fresh});
+        }
+        return nullptr;
+    }, e);
+}
 
 // Device bytes of JSON one writing pass produces at most (LB_JSON_STAGE_CAP overrides it, for testing: small chunks).
 // A request larger than this is written alone, in a chunk of its own size.
@@ -1220,7 +1329,7 @@ void json_requests(lb_batch* b, const lb_json_request* reqs, size_t n, lb_export
     CK(cudaMemcpyAsync(s.start, h_start.data(), sizeof(i32) * h_start.size(), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(s.end, h_end.data(), sizeof(i32) * h_end.size(), cudaMemcpyHostToDevice, st));
     xt.x_req = d_req;
-    xt.from_ctr = nullptr;
+    xt.x_span0 = nullptr; xt.x_spans = nullptr;
     xt.xdoc = dv.alloc<XDoc>(D + 1, true);
     LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, xt);
     if (NCH) {
@@ -1728,6 +1837,26 @@ lb_status lb_batch_export_updates(const lb_batch* cb, const lb_export_request* r
     std::lock_guard<std::mutex> g(b->export_mu);
     try {
         export_requests(b, reqs, n_reqs, *e);
+    } catch (lb_status s) {
+        return s;
+    }
+    *out = e.release();
+    return LB_OK;
+}
+
+lb_status lb_batch_export_updates_in_range(const lb_batch* cb, const lb_range_request* reqs, size_t n_reqs, lb_exports** out) {
+    lb_batch* b = const_cast<lb_batch*>(cb);
+    if (!b || !out || (!reqs && n_reqs)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
+    *out = nullptr;
+    if (!(b->flags & LB_FLAG_EXPORT)) { g_last_error = "batch was imported without LB_FLAG_EXPORT"; return LB_ERR_INVALID_ARG; }
+    for (size_t i = 0; i < n_reqs; i++) {
+        if (reqs[i].doc >= b->n_docs) { g_last_error = "document index out of range"; return LB_ERR_INVALID_ARG; }
+        if (!reqs[i].spans && reqs[i].n_spans) { g_last_error = "null spans with n_spans > 0"; return LB_ERR_INVALID_ARG; }
+    }
+    std::unique_ptr<lb_exports> e(new lb_exports());
+    std::lock_guard<std::mutex> g(b->export_mu);
+    try {
+        export_range_requests(b, reqs, n_reqs, *e);
     } catch (lb_status s) {
         return s;
     }

@@ -279,6 +279,15 @@ __device__ inline void xr_payload_skip(const BatchTables& t, u64 row, u32 xk, u3
     *p += off;
     *n -= off;
 }
+// ... and without its last `tail` atoms too, given the payload of its `atoms` atoms after the skip
+__device__ inline void xr_payload_drop_tail(u32 xk, u32 atoms, u32 tail, const u8* p, u32* n) {
+    if (xk == XK_TEXT) *n = text_byte_index(p, *n, atoms, atoms - tail);
+    else if (xk == XK_LIST) {
+        Cur c(p, *n);
+        for (u32 k = 0; k < atoms - tail && !c.err; k++) { u8 kk = c.get(); skip_loro_value_content(c, kk, nullptr); }
+        *n = (u32)(c.p - p);
+    }
+}
 // Op::slice(skip, len) of the op made from `row` (op.rs:161-172, list_op.rs:603-658, 251-278, 436-444)
 __device__ inline void xop_slice_front(const BatchTables& t, XOp& o, u64 row, u32 skip) {
     if (!skip) return;
@@ -299,6 +308,26 @@ __device__ inline void xop_slice_front(const BatchTables& t, XOp& o, u64 row, u3
     }
     o.ctr += (i32)skip;
     o.atoms -= skip;
+}
+// Op::slice(0, atoms - tail) of an op whose last row is `row` (read for Text only): list_op.rs:251-278, 436-444
+__device__ inline void xop_slice_back(const BatchTables& t, XOp& o, u64 row, u32 tail) {
+    if (!tail) return;
+    switch (o.xk) {
+        case XK_LIST: o.f1 -= tail; break;
+        case XK_TEXT: {
+            const u8* pp; u32 pn;
+            xr_payload(t, row, XK_TEXT, &pp, &pn);
+            const u32 ra = xr_len(t, row);
+            o.f1 -= pn - text_byte_index(pp, pn, ra, ra - tail);
+            break;
+        }
+        case XK_DEL:   // a reversed span keeps its position and loses its lowest ids
+            if (o.f2 > 0) o.f2 -= (i32)tail;
+            else { o.f1 += tail; o.f2 += (i32)tail; }
+            break;
+        default: return;   // one-atom ops are never cut
+    }
+    o.atoms -= tail;
 }
 
 // ---------------------------------------------------------------------------------------------- X1: arenas
@@ -575,7 +604,8 @@ struct XEntry {        // a change on its way through a store: one segment, or a
     u32 src, from;     // metadata of its first segment: source change + atom offset (deps, lamport, timestamp, message)
     u32 pos, r0;       // where its rows start: position in ch_aorder (absolute) + row inside that change
     u32 atoms, est_ops, nmops, ndel, nrows;
-    u32 skip;          // atoms of the first row already known to the importer of this export (from-version cut)
+    u32 skip;          // atoms of the first row outside the entry (import-side trim, or the front cut of its span)
+    u32 tail;          // atoms of the last row outside the entry (the end cut of its span)
     u32 lh_ch, lh_row; // last op: source change + row (inside that change) of its first row ...
     XOp last;          // ... or, once the entry has been through a store, the accumulated op itself
     bool last_valid;
@@ -617,28 +647,21 @@ struct XRows {
         }
     }
 };
-// accumulate the merged op that starts at the cursor (consumes its rows, at most `left` of them)
-// bytes one row contributes to the values section of a (merged) op, without the op's own prefix
-__device__ __forceinline__ u32 row_value_bytes(const BatchTables& t, const XOp& o, u64 row) {
-    const u8* p;
-    u32 n;
-    xr_payload(t, row, o.xk, &p, &n);
-    return n;
-}
-__device__ inline XOp xop_gather(const BatchTables& t, const DocInfo& di, XRows& it, u32& left, u32* vbytes = nullptr, u32 skip = 0) {
+// accumulate the merged op that starts at the cursor (consumes its rows, at most `left` of them): `skip` atoms of its
+// first row are left out, and `tail` atoms of the entry's last row when the op reaches it (the cursor then stays there)
+__device__ inline XOp xop_gather(const BatchTables& t, const DocInfo& di, XRows& it, u32& left, u32 skip = 0, u32 tail = 0) {
     XOp o = xop_from_row(t, di, it.ch, it.row());
     if (skip) xop_slice_front(t, o, it.row(), skip);
-    if (vbytes) { const u8* pp; u32 pn; xr_payload_skip(t, it.row(), o.xk, skip, &pp, &pn); *vbytes += pn; }
     left--;
     if (left) it.next();
     while (left && !(xr_flag(t, it.row()) & XF_HEAD)) {
-        if (vbytes) { const u8* pp; u32 pn; xr_payload_skip(t, it.row(), o.xk, it.skip, &pp, &pn); *vbytes += pn; }
         XOp x = xop_from_row(t, di, it.ch, it.row());
         if (it.skip) xop_slice_front(t, x, it.row(), it.skip);
         xop_merge(o, x);
         left--;
         if (left) it.next();
     }
+    if (!left && tail) xop_slice_back(t, o, it.row(), tail);
     return o;
 }
 // last op of an entry that came straight from stage A: from its head row to the end of its segment
@@ -664,27 +687,38 @@ __device__ inline bool xstore_push(const BatchTables& t, const DocInfo& di, XSto
         bool is_full = est + s.blk_est > LB_MAX_BLOCK_SIZE;
         bool dep_only_self = E.from ? true : (t.ch_dep_self[E.src] && t.ch_ndeps[E.src] == 0);
         bool can = dep_only_self && t.ch_ts[E.src] <= t.ch_ts[s.open.src] && xmsg_same(t, s.open.src, E.src);
+        // the last change ends inside a row (an end cut) and E starts on that row: E can only grow the change when the
+        // two halves of the row's op merge back (for list, text and delete halves they always do), since the grown
+        // change lists the row once; otherwise E starts a change of its own
+        const bool shared = s.open.tail != 0;
+        if (can && shared) {
+            XRows it(t, E.pos, E.r0);
+            u32 left = E.nrows;
+            can = xop_mergable(s.back, xop_gather(t, di, it, left, E.skip, E.tail));
+        }
         bool single = false;
         if (can && is_full && E.nmops == 1) {
             XRows it(t, E.pos, E.r0);
             u32 left = E.nrows;
-            single = xop_mergable(s.back, xop_gather(t, di, it, left, nullptr, E.skip));
+            single = xop_mergable(s.back, xop_gather(t, di, it, left, E.skip, E.tail));
         }
         if (can && (!is_full || single)) {
-            // the ops of E are pushed onto the last change (RleVec::push): a prefix of them may merge into its last op
+            // the ops of E are pushed onto the last change (RleVec::push): a prefix of them may merge into its last op.
+            // When the last change ends inside a row (an end cut), E starts on that same row: the two halves of the row's
+            // op merge back, and the grown change lists the row once
             XRows it(t, E.pos, E.r0);
             u32 left = E.nrows;
             u32 merged = 0, merged_sz = 0, merged_del = 0;
             bool first_op = true;
             while (left) {
                 u64 head_row = it.row();
-                XOp o = xop_gather(t, di, it, left, nullptr, first_op ? E.skip : it.skip);
-                first_op = false;
+                XOp o = xop_gather(t, di, it, left, first_op ? E.skip : it.skip, E.tail);
                 if (!xop_mergable(s.back, o)) break;
                 merged_sz += xop_estimate(o);
                 merged_del += o.xk == XK_DEL;
                 xop_merge(s.back, o);
-                *xr_flagp(t, head_row) &= (u8)~XF_HEAD;
+                if (!(first_op && shared)) *xr_flagp(t, head_row) &= (u8)~XF_HEAD;
+                first_op = false;
                 merged++;
             }
             s.blk_est += E.est_ops - merged_sz;          // only ops that did not merge count (change_store.rs:1271-1279)
@@ -692,7 +726,8 @@ __device__ inline bool xstore_push(const BatchTables& t, const DocInfo& di, XSto
             s.open.est_ops += E.est_ops - 8 * merged_del; // fresh estimate of the grown change (used by the next store)
             s.open.nmops += E.nmops - merged;
             s.open.ndel += E.ndel - merged_del;
-            s.open.nrows += E.nrows;
+            s.open.nrows += E.nrows - (shared ? 1u : 0u);
+            s.open.tail = E.tail;
             if (E.nmops > merged) s.back = xentry_last_op(t, di, E);
             return false;
         }
@@ -708,13 +743,9 @@ __device__ inline bool xstore_push(const BatchTables& t, const DocInfo& di, XSto
     return closed;
 }
 
-// Change::slice at the `from` version (change_store.rs:505-521, change.rs:203-258): entry E covers counters
-// [c0, c0 + atoms) of its peer; what lies before `start` is dropped.  false = nothing left.
-__device__ inline bool xentry_cut(const BatchTables& t, const DocInfo& di, XEntry& E, i32 start) {
-    i32 c0 = t.ch_counter[E.src] + (i32)E.from;
-    if (start <= c0) return true;
-    if (start >= c0 + (i32)E.atoms) return false;
-    u32 cut = (u32)(start - c0);
+// Change::slice (change_store.rs:505-521, change.rs:203-258) in front: entry E covers counters [c0, c0 + atoms) of its
+// peer; its first `cut` atoms (0 < cut < atoms) are dropped.  The summary is left to xentry_summary.
+__device__ inline void xentry_trim_front(const BatchTables& t, XEntry& E, u32 cut) {
     XRows it(t, E.pos, E.r0);
     u32 left = E.nrows, acc = 0, lead = E.skip;   // `lead`: atoms of the current row already outside the entry
     while (left) {
@@ -730,14 +761,32 @@ __device__ inline bool xentry_cut(const BatchTables& t, const DocInfo& di, XEntr
     E.skip = lead + (cut - acc);
     E.from += cut;
     E.atoms -= cut;
-    // fresh summary of what is left: size estimate, ops, deletes, last op
-    XRows it2(t, E.pos, E.r0);
-    u32 l = left, est = 0, nm = 0, nd = 0;
+}
+// ... and at the end: only the first `keep` atoms (0 < keep < atoms) stay; the row holding the last of them ends the
+// entry, with the atoms after it counted in `tail` (E.tail is 0 before: end cuts are taken from the import store)
+__device__ inline void xentry_trim_back(const BatchTables& t, XEntry& E, u32 keep) {
+    XRows it(t, E.pos, E.r0);
+    u32 n = 1, acc = 0, lead = E.skip;
+    while (true) {
+        const u32 len = xr_len(t, it.row()) - lead;
+        if (acc + len >= keep) { E.tail = acc + len - keep; break; }
+        acc += len;
+        n++;
+        it.next();
+        lead = it.skip;
+    }
+    E.nrows = n;
+    E.atoms = keep;
+}
+// fresh summary of a cut entry: size estimate, ops, deletes, last op
+__device__ inline void xentry_summary(const BatchTables& t, const DocInfo& di, XEntry& E) {
+    XRows it(t, E.pos, E.r0);
+    u32 l = E.nrows, est = 0, nm = 0, nd = 0;
     XOp last;
     last.xk = XK_NONE;
     bool first = true;
     while (l) {
-        XOp o = xop_gather(t, di, it2, l, nullptr, first ? E.skip : it2.skip);
+        XOp o = xop_gather(t, di, it, l, first ? E.skip : it.skip, E.tail);
         first = false;
         est += xop_estimate(o);
         nm++;
@@ -749,10 +798,35 @@ __device__ inline bool xentry_cut(const BatchTables& t, const DocInfo& di, XEntr
     E.ndel = nd;
     E.last = last;
     E.last_valid = true;
+}
+// Change::slice at the `from` version: what lies before `start` is dropped.  false = nothing left.
+__device__ inline bool xentry_cut(const BatchTables& t, const DocInfo& di, XEntry& E, i32 start) {
+    i32 c0 = t.ch_counter[E.src] + (i32)E.from;
+    if (start <= c0) return true;
+    if (start >= c0 + (i32)E.atoms) return false;
+    xentry_trim_front(t, E, (u32)(start - c0));
+    xentry_summary(t, di, E);
     return true;
 }
+// Change::slice(start, end) clamped to the entry, which overlaps [start, end)
+__device__ inline void xentry_slice(const BatchTables& t, const DocInfo& di, XEntry& E, i32 start, i32 end) {
+    const i32 c0 = t.ch_counter[E.src] + (i32)E.from;
+    if (start > c0) xentry_trim_front(t, E, (u32)(start - c0));
+    const i32 c1 = t.ch_counter[E.src] + (i32)E.from;
+    if (end < c1 + (i32)E.atoms) xentry_trim_back(t, E, (u32)(end - c1));
+    xentry_summary(t, di, E);
+}
 
-// thread per document
+// first final-change slot of a document: one slot per segment, and in an export of chosen spans one more per span of
+// the documents before it (a stored change that k spans cut leaves k pieces, so a document can need that many more)
+__device__ __forceinline__ u64 xfc0(const BatchTables& t, const DocInfo& di) {
+    return di.ch0 + t.ch_seg0[di.ch0] + (t.x_span0 ? t.x_span0[di.peer0] : 0u);
+}
+// thread per document: per peer, the import store (s1) is rebuilt once; every change it completes is cut to each of the
+// peer's spans it overlaps (one change can give several pieces, each cut at both ends) and the pieces enter the export
+// store (s2) in counter order.  A span with the fresh bit starts a new block there (its first change found no block of
+// the peer ending at its start: change_store.rs:711-764); the others continue the block of the span that ends at their
+// start.
 __global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
@@ -761,13 +835,13 @@ __global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, const 
     XDoc x = t.xdoc[d];
     if (t.x_req && !t.x_req[d]) { x.n_fc = x.n_mb = 0; t.xdoc[d] = x; return; }
     if (x.flags & 1) { t.xdoc[d] = x; return; }
-    u64 w = di.ch0 + t.ch_seg0[di.ch0];   // as many slots as the document has segments
+    u64 w = xfc0(t, di);
     u64 w0 = w;
     u32 n_mb = 0;
     auto emit = [&](const XEntry& e, bool starts_block) {
         t.fc_src[w] = e.src; t.fc_pos[w] = e.pos; t.fc_r0[w] = e.r0; t.fc_from[w] = e.from; t.fc_atoms[w] = e.atoms;
         t.fc_nrows[w] = e.nrows; t.fc_ndel[w] = e.ndel; t.fc_block[w] = starts_block ? 1 : 0; t.fc_skip[w] = e.skip;
-        t.fc_est[w] = e.est_ops;
+        t.fc_tail[w] = e.tail; t.fc_est[w] = e.est_ops;
         n_mb += starts_block;
         w++;
     };
@@ -776,14 +850,38 @@ __global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, const 
         while (p < di.P && t.dpeer[di.peer0 + p].rank != rank) p++;
         if (p == di.P) break;
         const DocPeer& dp = t.dpeer[di.peer0 + p];
-        const i32 start = t.from_ctr ? t.from_ctr[di.peer0 + p] : 0;
-        if (start >= dp.end_counter) continue;   // the importer of this export already has the whole peer
+        const u32 sp0 = t.x_spans ? t.x_span0[di.peer0 + p] : 0u;
+        const u32 nsp = t.x_spans ? t.x_span0[di.peer0 + p + 1] - sp0 : 1u;
+        u32 j = 0;   // the first span not yet finished
         XStore s1, s2;   // import store, export store
         s1.have_block = s1.open_valid = s1.open_starts_block = false; s1.blk_est = 0;
         s2 = s1;
+        // a change the import store completed: its pieces inside the spans go to the export store
+        auto take = [&](const XEntry& c) {
+            const i32 c0 = t.ch_counter[c.src] + (i32)c.from, c1 = c0 + (i32)c.atoms;
+            while (j < nsp) {
+                XSpan s;
+                if (t.x_spans) s = t.x_spans[sp0 + j];
+                else { s.start = 0; s.end = dp.end_counter; s.fresh = 1; }
+                if (s.start >= c1) break;
+                if (s.end > c0) {
+                    if (s.fresh && s.start >= c0) {
+                        if (s2.open_valid) emit(s2.open, s2.open_starts_block);
+                        s2.have_block = s2.open_valid = false;
+                    }
+                    XEntry piece = c;
+                    if (s.start > c0 || s.end < c1) xentry_slice(t, di, piece, s.start, s.end);
+                    XEntry d2;
+                    bool d2_blk = false;
+                    if (xstore_push(t, di, s2, piece, d2, d2_blk)) emit(d2, d2_blk);
+                }
+                if (s.end > c1) break;
+                j++;
+            }
+        };
         XEntry done;
         bool done_blk = false;
-        for (u32 k = 0; k < dp.ch_count; k++) {
+        for (u32 k = 0; k < dp.ch_count && j < nsp; k++) {
             u32 pos = (u32)di.ch0 + dp.ch_first + k;
             u32 ch = t.ch_aorder[pos];
             u32 nseg = t.ch_nseg[ch];
@@ -792,20 +890,14 @@ __global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, const 
                 XEntry E;
                 E.src = ch; E.from = t.sg_from[sg]; E.pos = pos; E.r0 = t.sg_r0[sg]; E.atoms = t.sg_atoms[sg];
                 E.est_ops = t.sg_est[sg]; E.nmops = t.sg_nmops[sg]; E.ndel = t.sg_ndel[sg]; E.nrows = t.sg_nrows[sg];
-                E.lh_ch = ch; E.lh_row = t.sg_last_head[sg]; E.last_valid = false; E.skip = t.sg_skip[sg];
-                if (xstore_push(t, di, s1, E, done, done_blk)) {
-                    XEntry d2;
-                    bool d2_blk = false;
-                    if ((start <= 0 || xentry_cut(t, di, done, start)) && xstore_push(t, di, s2, done, d2, d2_blk)) emit(d2, d2_blk);
-                }
+                E.lh_ch = ch; E.lh_row = t.sg_last_head[sg]; E.last_valid = false; E.skip = t.sg_skip[sg]; E.tail = 0;
+                if (xstore_push(t, di, s1, E, done, done_blk)) take(done);
             }
         }
-        if (s1.open_valid) {
-            XEntry d2;
-            bool d2_blk = false;
+        if (s1.open_valid && j < nsp) {
             s1.open.last = s1.back;
             s1.open.last_valid = true;
-            if ((start <= 0 || xentry_cut(t, di, s1.open, start)) && xstore_push(t, di, s2, s1.open, d2, d2_blk)) emit(d2, d2_blk);
+            take(s1.open);
         }
         if (s2.open_valid) emit(s2.open, s2.open_starts_block);
     }
@@ -838,7 +930,7 @@ __global__ void k_exp_list(const DocInfo* __restrict__ docs, u32 n_docs, const _
     const DocInfo& di = docs[d];
     const XDoc& x = t.xdoc[d];
     if (di.code != DOC_OK || x.n_mb == 0) return;
-    u64 f0 = di.ch0 + t.ch_seg0[di.ch0];
+    u64 f0 = xfc0(t, di);
     u64 scr = x.scratch0, stg = x.stage0, words = 0, slot = 0;
     int idx = -1;
     XBlock b;
@@ -875,7 +967,7 @@ __global__ void k_exp_sizes(const DocInfo* __restrict__ docs, u32 n_docs, const 
     u32 nb = di.code == DOC_OK ? x.n_mb : 0;
     u64 words = 0, bytes = 0;
     if (nb) {
-        u64 f0 = di.ch0 + t.ch_seg0[di.ch0];
+        u64 f0 = xfc0(t, di);
         words = nb * xscratch_block(di);
         bytes = nb * xstage_block(di);
         for (u64 k = f0; k < f0 + x.n_fc; k++) {
@@ -1147,7 +1239,11 @@ __global__ void k_exp_posrank(const DocInfo* __restrict__ docs, u32 n_docs, cons
 // exact, and is flagged (XBlock::ovf).  retry = 1, flagged blocks only: the same encode once more, into the slot
 // k_exp_layout gave the block in the retry buffer (`out`, from the document's restage0 on), which its lengths fill.
 // Two builds of the same code: <1> is compiled with __launch_bounds__(64, 5) (the compiler then schedules for 64-thread
-// CTAs: 132 registers against 128 without bounds, other load / store placement), <0> without bounds.  Registers decide
+// CTAs: 132 registers against 128 without bounds, other load / store placement), <0> without bounds.  Each has a twin,
+// k_exp_encode_cut<CAPPED>, that also honours end cuts (fc_tail: an export of spans that end inside a change); the
+// end-cut code costs the encoder registers (sm_90a: 136 against 128 unbounded, 136 against 132 bounded), which would
+// take the unbounded build from 8 CTAs to 7, so the exports without end cuts (import time, updates(from)) keep builds
+// without it.  Registers decide
 // the CTAs an SM holds: up to 128 give 8, up to 136 give 7, and each build is faster at its own count.  On one H100
 // 80GB HBM3 (700 W power limit), the bounded build at 127 registers (8 CTAs) took C5's re-export from 107 to 120 ms,
 // and the unbounded one at 132 (7 CTAs) took C3's at 4 k documents from 38.6 to 45.9 ms.
@@ -1156,6 +1252,7 @@ __global__ void k_exp_posrank(const DocInfo* __restrict__ docs, u32 n_docs, cons
 // against 106.4 ms; C3 at 40 k documents (~550 k blocks) 346.4 against 325.3 / 323.4 ms.  So batches of at least
 // LB_XENC_BOUNDED_MIN_BLOCKS output blocks take the bounded build.
 #define LB_XENC_BOUNDED_MIN_BLOCKS 100000ull
+template <int CUT>
 __device__ __forceinline__ void exp_encode_body(
     const DocInfo* __restrict__ docs, u64 n_blocks, const BatchTables& t, XBlock* __restrict__ xb,
                              u32* __restrict__ scratch, u8* __restrict__ out, int retry) {
@@ -1251,12 +1348,15 @@ __device__ __forceinline__ void exp_encode_body(
     for (u32 j = 0; j < N; j++) {
         XRows it(t, t.fc_pos[fc0 + j], t.fc_r0[fc0 + j]);
         u32 left = t.fc_nrows[fc0 + j];
-        u32 skip = t.fc_skip[fc0 + j];   // only the first op of a change cut at the `from` version
+        u32 skip = t.fc_skip[fc0 + j];   // the first op of a change cut in front
         while (left) {
             XRows it0 = it;
             const u32 left0 = left;
             const u32 skip0 = skip;
-            XOp o = xop_gather(t, di, it, left, nullptr, skip);
+            XOp o = xop_gather(t, di, it, left, skip);
+            // the last op of a change cut at the end (fc_tail is loaded here only: a value held across the loop would
+            // cost the encoder registers)
+            if (CUT && !left) xop_slice_back(t, o, it.row(), t.fc_tail[fc0 + j]);
             skip = left ? it.skip : 0u;   // (the next op may start on the first kept row of a trimmed change)
             if (o.xk == XK_LIST) { vs.put(7); vs.varint(o.atoms); }
             else if (o.xk == XK_TEXT) vs.varint(o.f1 - o.f0);
@@ -1269,7 +1369,9 @@ __device__ __forceinline__ void exp_encode_body(
                 while (k) {
                     const u8* pp;
                     u32 pn;
-                    xr_payload_skip(t, it0.row(), o.xk, k == left0 - left ? skip0 : it0.skip, &pp, &pn);
+                    const u32 sk = k == left0 - left ? skip0 : it0.skip;
+                    xr_payload_skip(t, it0.row(), o.xk, sk, &pp, &pn);
+                    if (CUT && k == 1 && !left && t.fc_tail[fc0 + j]) xr_payload_drop_tail(o.xk, xr_len(t, it0.row()) - sk, t.fc_tail[fc0 + j], pp, &pn);
                     if (has_maps && o.xk != XK_TEXT) xvalue_copy(vs, pp, pn, t, t.blocks[t.ch_block[it0.ch]].key0, keys);
                     else vs.copy(pp, pn);
                     k--;
@@ -1441,12 +1543,23 @@ template <int CAPPED> __global__ void k_exp_encode(const DocInfo* __restrict__ d
                                                  u32* __restrict__ scratch, u8* __restrict__ out, int retry);
 template <> __global__ void k_exp_encode<0>(const DocInfo* __restrict__ docs, u64 n_blocks, const __grid_constant__ BatchTables t, XBlock* __restrict__ xb,
                                             u32* __restrict__ scratch, u8* __restrict__ out, int retry) {
-    exp_encode_body(docs, n_blocks, t, xb, scratch, out, retry);
+    exp_encode_body<0>(docs, n_blocks, t, xb, scratch, out, retry);
 }
 template <> __global__ void __launch_bounds__(64, 5) k_exp_encode<1>(const DocInfo* __restrict__ docs, u64 n_blocks, const __grid_constant__ BatchTables t,
                                                                      XBlock* __restrict__ xb, u32* __restrict__ scratch,
                                                                      u8* __restrict__ out, int retry) {
-    exp_encode_body(docs, n_blocks, t, xb, scratch, out, retry);
+    exp_encode_body<0>(docs, n_blocks, t, xb, scratch, out, retry);
+}
+template <int CAPPED> __global__ void k_exp_encode_cut(const DocInfo* __restrict__ docs, u64 n_blocks, const __grid_constant__ BatchTables t, XBlock* __restrict__ xb,
+                                                     u32* __restrict__ scratch, u8* __restrict__ out, int retry);
+template <> __global__ void k_exp_encode_cut<0>(const DocInfo* __restrict__ docs, u64 n_blocks, const __grid_constant__ BatchTables t, XBlock* __restrict__ xb,
+                                                u32* __restrict__ scratch, u8* __restrict__ out, int retry) {
+    exp_encode_body<1>(docs, n_blocks, t, xb, scratch, out, retry);
+}
+template <> __global__ void __launch_bounds__(64, 5) k_exp_encode_cut<1>(const DocInfo* __restrict__ docs, u64 n_blocks, const __grid_constant__ BatchTables t,
+                                                                         XBlock* __restrict__ xb, u32* __restrict__ scratch,
+                                                                         u8* __restrict__ out, int retry) {
+    exp_encode_body<1>(docs, n_blocks, t, xb, scratch, out, retry);
 }
 
 // thread per document, after the encode: block offsets inside the blob, blob length, and the blocks that outgrew their

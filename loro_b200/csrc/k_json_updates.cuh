@@ -78,7 +78,7 @@ __global__ void k_jx_store(const DocInfo* __restrict__ docs, u32 n_docs, const _
                 XEntry E;
                 E.src = ch; E.from = t.sg_from[sg]; E.pos = pos; E.r0 = t.sg_r0[sg]; E.atoms = t.sg_atoms[sg];
                 E.est_ops = t.sg_est[sg]; E.nmops = t.sg_nmops[sg]; E.ndel = t.sg_ndel[sg]; E.nrows = t.sg_nrows[sg];
-                E.lh_ch = ch; E.lh_row = t.sg_last_head[sg]; E.last_valid = false; E.skip = t.sg_skip[sg];
+                E.lh_ch = ch; E.lh_row = t.sg_last_head[sg]; E.last_valid = false; E.skip = t.sg_skip[sg]; E.tail = 0;
                 if (xstore_push(t, di, s1, E, done, done_blk)) emit(done);
             }
         }
@@ -225,7 +225,7 @@ struct JxWriter {
     __device__ bool entry(u32 p, u32 k, XEntry& E, u32& keep) {
         const u64 f = fc_base + pf0[di.peer0 + p] + k;
         E.src = t.fc_src[f]; E.from = t.fc_from[f]; E.pos = t.fc_pos[f]; E.r0 = t.fc_r0[f]; E.atoms = t.fc_atoms[f];
-        E.nrows = t.fc_nrows[f]; E.skip = t.fc_skip[f]; E.last_valid = false;
+        E.nrows = t.fc_nrows[f]; E.skip = t.fc_skip[f]; E.tail = 0; E.last_valid = false;
         const i32 st = s.start[rq.slot0 + p], en = s.end[rq.slot0 + p];
         if (st >= en) return false;   // from.diff_iter(to) holds nothing of the peer
         const i32 c0 = t.ch_counter[E.src] + (i32)E.from;
@@ -246,7 +246,7 @@ struct JxWriter {
             XRows at = it;
             const u32 skip = first ? E.skip : it.skip;
             first = false;
-            XOp op = xop_gather(t, di, it, left, nullptr, skip);
+            XOp op = xop_gather(t, di, it, left, skip);
             const u32 take = op.atoms < keep ? op.atoms : keep;
             f(op, take, at, skip);
             keep -= take;
@@ -359,10 +359,7 @@ struct JxWriter {
                     break;
                 }
                 case XK_DEL: {
-                    if (take < op.atoms) {   // Op::slice(0, take) (list_op.rs:436-444)
-                        if (op.f2 > 0) op.f2 = (i32)take;
-                        else { op.f1 += op.atoms - take; op.f2 = -(i32)take; }
-                    }
+                    xop_slice_back(t, op, at.row(), op.atoms - take);
                     o.puts_("\"delete\",\"pos\":");
                     o.put_i64(op.prop);
                     o.puts_(",\"len\":");

@@ -9,6 +9,10 @@
 #include "lb_defs.h"
 
 struct XDoc;   // k_export.cuh
+struct XSpan {   // counters [start, end) of one peer to export; fresh = 1: the span starts a new block in the export store
+    i32 start, end;
+    u32 fresh, pad;
+};
 
 struct BatchTables {
     // ---- input and phase 1 (frame)
@@ -110,13 +114,15 @@ struct BatchTables {
     u32* sg_skip;      // atoms of the segment's first row the document already had (import-side trim, k_doc_causal)
     // final changes (same index space: a document never ends up with more changes than segments)
     u32* fc_src; u32* fc_pos; u32* fc_r0; u32* fc_from; u32* fc_atoms; u32* fc_nrows; u32* fc_ndel; u8* fc_block;
-    u32* fc_skip;      // atoms of the change's first row that lie before the `from` version (Op::slice)
+    u32* fc_skip;      // atoms of the change's first row that lie before its span (Change::slice at the front)
+    u32* fc_tail;      // atoms of the change's last row that lie at or past the end of its span (Change::slice at the end)
     u32* fc_est;       // the store's size estimate of the change's ops (sizes the staging slot of its block)
-    // export(ExportMode::updates(from)) on demand (lb_batch_export_updates): x_req[d] != 0 marks the documents of one
-    // round (null: every document, the import-time export); from_ctr[doc peer slot] = first counter to export
-    // (encoding.rs:79-83, change_store.rs:494-528 export_blocks_from, change.rs:203-258 Change::slice).  export_round
-    // sets these three on a copy of the batch's struct.
-    const u8* x_req; const i32* from_ctr;
+    // export of chosen id spans on demand (lb_batch_export_updates, lb_batch_export_updates_in_range): x_req[d] != 0
+    // marks the documents of one round (null: every document, the import-time export); the spans of doc peer slot s are
+    // x_spans[x_span0[s] .. x_span0[s + 1]), disjoint and sorted by start (null: [0, vv) for every peer).  updates(from)
+    // is one span [from, vv) per peer (encoding.rs:79-83, change_store.rs:494-528); UpdatesInRange is the caller's spans
+    // (change_store.rs:179-199).  export_round sets these on a copy of the batch's struct.
+    const u8* x_req; const u32* x_span0; const XSpan* x_spans;
     XDoc* xdoc;
     // ---- checkout (k_checkout.cuh), written after the causal scan, read by phases 4 and 5 (last, so that the layout of
     // every other field is the same with or without it)
