@@ -219,10 +219,7 @@ class Batch:
     def export_updates_in_range(self, i, spans):
         """LoroDoc::export(ExportMode::UpdatesInRange { spans }) of document i (needs flags=LB_FLAG_EXPORT at import):
         the changes in `spans` = [(peer, start, end), ...], counters [start, end), taken in the order given."""
-        r = self.export_updates_in_range_many([(i, spans)])[0]
-        if isinstance(r, EngineError):
-            raise r
-        return r
+        return self._one(self.export_updates_in_range_many([(i, spans)]))
 
     def export_updates_till(self, i, vv):
         """LoroDoc::export(ExportMode::updates_till(vv)) of document i: one span [0, vv[peer]) per peer
@@ -250,6 +247,13 @@ class Batch:
                "lb_batch_export_updates_in_range")
         return self._exports(h, len(requests), "range request")
 
+    @staticmethod
+    def _one(answers):
+        """the answer of a one-request *_many call: its value, or its EngineError raised"""
+        if isinstance(answers[0], EngineError):
+            raise answers[0]
+        return answers[0]
+
     def _exports(self, h, n, what, text=False):
         """the n answers of an lb_exports (freed here): bytes (text: str), or the EngineError of a failed request"""
         out = []
@@ -272,10 +276,7 @@ class Batch:
         """LoroDoc::export_json_updates(start_vv, end_vv) of document i as JSON text (needs flags=LB_FLAG_EXPORT at
         import).  start_vv=None is the empty version; end_vv=None is the document's oplog vv.  Versions are
         {peer: counter}; peer_compression=False gives real peer ids and "peers": null."""
-        r = self.export_json_updates_many([(i, start_vv, end_vv, peer_compression)])[0]
-        if isinstance(r, EngineError):
-            raise r
-        return r
+        return self._one(self.export_json_updates_many([(i, start_vv, end_vv, peer_compression)]))
 
     def export_json_updates_many(self, requests):
         """export_json_updates for many (document, version range) requests in one call (lb_batch_export_json_updates):
@@ -387,41 +388,9 @@ class MultiBatch:
     def oplog_frontiers(self, i): p, j = self._loc(i); return p.oplog_frontiers(j)
     def export_updates(self, i, from_vv=None): p, j = self._loc(i); return p.export_updates(j, from_vv)
 
-    def export_updates_many(self, requests):
-        """Batch.export_updates_many with every request sent to its sub-batch: one C call per sub-batch."""
-        requests = list(requests)
-        per_part = {}
-        for k, (i, from_vv) in enumerate(requests):
-            p, j = self._loc(i)
-            per_part.setdefault(id(p), (p, []))[1].append((k, j, from_vv))
-        out = [None] * len(requests)
-        for p, reqs in per_part.values():
-            for (k, _, _), r in zip(reqs, p.export_updates_many([(j, f) for _, j, f in reqs])):
-                out[k] = r
-        return out
-
-    def export_updates_in_range(self, i, spans): p, j = self._loc(i); return p.export_updates_in_range(j, spans)
-    def export_updates_till(self, i, vv): p, j = self._loc(i); return p.export_updates_till(j, vv)
-
-    def export_updates_in_range_many(self, requests):
-        """Batch.export_updates_in_range_many with every request sent to its sub-batch: one C call per sub-batch."""
-        requests = list(requests)
-        per_part = {}
-        for k, (i, spans) in enumerate(requests):
-            p, j = self._loc(i)
-            per_part.setdefault(id(p), (p, []))[1].append((k, j, spans))
-        out = [None] * len(requests)
-        for p, reqs in per_part.values():
-            for (k, _, _), r in zip(reqs, p.export_updates_in_range_many([(j, s) for _, j, s in reqs])):
-                out[k] = r
-        return out
-
-    def export_json_updates(self, i, start_vv=None, end_vv=None, peer_compression=True):
-        p, j = self._loc(i)
-        return p.export_json_updates(j, start_vv, end_vv, peer_compression)
-
-    def export_json_updates_many(self, requests):
-        """Batch.export_json_updates_many with every request sent to its sub-batch: one C call per sub-batch."""
+    def _many(self, method, requests):
+        """Batch.<method> for requests (doc, ...) with every request sent to its sub-batch: one call per sub-batch, the
+        answers in request order"""
         requests = [tuple(r) for r in requests]
         per_part = {}
         for k, r in enumerate(requests):
@@ -429,9 +398,28 @@ class MultiBatch:
             per_part.setdefault(id(p), (p, []))[1].append((k, (j,) + r[1:]))
         out = [None] * len(requests)
         for p, reqs in per_part.values():
-            for (k, _), res in zip(reqs, p.export_json_updates_many([r for _, r in reqs])):
+            for (k, _), res in zip(reqs, getattr(p, method)([r for _, r in reqs])):
                 out[k] = res
         return out
+
+    def export_updates_many(self, requests):
+        """Batch.export_updates_many with every request sent to its sub-batch: one C call per sub-batch."""
+        return self._many("export_updates_many", requests)
+
+    def export_updates_in_range(self, i, spans): p, j = self._loc(i); return p.export_updates_in_range(j, spans)
+    def export_updates_till(self, i, vv): p, j = self._loc(i); return p.export_updates_till(j, vv)
+
+    def export_updates_in_range_many(self, requests):
+        """Batch.export_updates_in_range_many with every request sent to its sub-batch: one C call per sub-batch."""
+        return self._many("export_updates_in_range_many", requests)
+
+    def export_json_updates(self, i, start_vv=None, end_vv=None, peer_compression=True):
+        p, j = self._loc(i)
+        return p.export_json_updates(j, start_vv, end_vv, peer_compression)
+
+    def export_json_updates_many(self, requests):
+        """Batch.export_json_updates_many with every request sent to its sub-batch: one C call per sub-batch."""
+        return self._many("export_json_updates_many", requests)
 
     def fetch_json(self):
         for p in self._parts:

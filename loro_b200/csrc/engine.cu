@@ -1064,6 +1064,26 @@ lb_exports::Answer doc_error(const DocInfo& di) {
     return lb_exports::Answer{LB_ERR_INVALID_ARG, ERR_FAILED_DOC, nullptr, 0};
 }
 
+// The start of an on-demand export pass over the documents h_req marks: a copy of the batch's tables with the request
+// mask (x_req) and a fresh XDoc table, and the marked documents' changes prepared for the stores (k_exp_init, both passes
+// of k_exp_changes).  The caller releases xt.x_req and xt.xdoc.
+BatchTables export_pass(lb_batch* b, const std::vector<u8>& h_req) {
+    Dev& dv = b->dev;
+    const u32 D = (u32)b->n_docs;
+    const u64 NCH = b->n_changes;
+    BatchTables xt = b->tb;
+    u8* d_req = dv.alloc<u8>(D);
+    CK(cudaMemcpyAsync(d_req, h_req.data(), D, cudaMemcpyHostToDevice, dv.stream));
+    xt.x_req = d_req;
+    xt.xdoc = dv.alloc<XDoc>(D + 1, true);
+    LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, xt);
+    if (NCH) {
+        LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 0);
+        LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 1);
+    }
+    return xt;
+}
+
 // One pass of the export of chosen id spans (change_store.rs:179-199 export_blocks_in_range, :494-528
 // export_blocks_from) over the documents of a round, one span set each: the import store of each marked document is
 // rebuilt, its changes are cut to the document's spans (Change::slice at both ends) on their way into a fresh export
@@ -1079,7 +1099,6 @@ std::unique_ptr<uint8_t[]> export_round(lb_batch* b, const std::vector<u32>& h_s
     Dev& dv = b->dev;
     cudaStream_t st = dv.stream;
     const u32 D = (u32)b->n_docs;
-    const u64 NCH = b->n_changes;
     // a document's final changes get one slot per segment and one per span (xfc0): grow the tables when a round needs more
     if (b->n_segs + h_spans.size() > b->fc_cap) {
         b->fc_cap = b->n_segs + h_spans.size();
@@ -1087,23 +1106,14 @@ std::unique_ptr<uint8_t[]> export_round(lb_batch* b, const std::vector<u32>& h_s
         dv.release(b->tb.fc_block);
         b->tb.fc_block = dv.alloc<u8>(b->fc_cap);
     }
-    BatchTables xt = b->tb;
     u32* d_span0 = dv.alloc<u32>(h_span0.size());
     XSpan* d_spans = dv.alloc<XSpan>(std::max<size_t>(h_spans.size(), 1));
-    u8* d_req = dv.alloc<u8>(D);
     CK(cudaMemcpyAsync(d_span0, h_span0.data(), sizeof(u32) * h_span0.size(), cudaMemcpyHostToDevice, st));
     if (!h_spans.empty()) CK(cudaMemcpyAsync(d_spans, h_spans.data(), sizeof(XSpan) * h_spans.size(), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_req, h_req.data(), D, cudaMemcpyHostToDevice, st));
+    BatchTables xt = export_pass(b, h_req);
     CK(cudaStreamSynchronize(st));   // pageable host memory
     xt.x_span0 = d_span0;
     xt.x_spans = d_spans;
-    xt.x_req = d_req;
-    xt.xdoc = dv.alloc<XDoc>(D + 1, true);
-    LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, xt);
-    if (NCH) {
-        LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 0);
-        LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 1);
-    }
     LB_BATCH_LAUNCH(b, k_exp_store, nblk(D, 64), 64, 0, b->d_docs, D, xt);
     u64 XT = 0;
     u8* d_out = export_encode(b, xt, &XT, cuts);
@@ -1112,7 +1122,7 @@ std::unique_ptr<uint8_t[]> export_round(lb_batch* b, const std::vector<u32>& h_s
     std::unique_ptr<uint8_t[]> out(new uint8_t[XT + 1]);
     if (!lbstage::download(d_out, out.get(), XT, st)) { g_last_error = "export d2h failed"; throw lb_status(LB_ERR_CUDA); }
     CK(cudaStreamSynchronize(st));
-    dv.release(d_span0); dv.release(d_spans); dv.release(d_req); dv.release(xt.xdoc); dv.release(d_out);
+    dv.release(d_span0); dv.release(d_spans); dv.release(xt.x_req); dv.release(xt.xdoc); dv.release(d_out);
     return out;
 }
 
@@ -1318,24 +1328,14 @@ void json_requests(lb_batch* b, const lb_json_request* reqs, size_t n, lb_export
     if (jr.empty()) return;
     Dev& dv = b->dev;
     cudaStream_t st = dv.stream;
-    const u64 NCH = b->n_changes, NR = jr.size(), S = std::max<size_t>(h_start.size(), 1);
-    BatchTables xt = b->tb;
-    u8* d_req = dv.alloc<u8>(D);
+    const u64 NR = jr.size(), S = std::max<size_t>(h_start.size(), 1);
     JxReq* d_jr = dv.alloc<JxReq>(NR);
     JxScratch s{dv.alloc<i32>(S), dv.alloc<i32>(S), dv.alloc<u32>(S), dv.alloc<u32>(S), dv.alloc<u32>(S)};
     u32* d_pf0 = dv.alloc<u32>(b->n_peers_tot + 1);
     u32* d_pfn = dv.alloc<u32>(b->n_peers_tot + 1);
-    CK(cudaMemcpyAsync(d_req, h_req.data(), D, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(s.start, h_start.data(), sizeof(i32) * h_start.size(), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(s.end, h_end.data(), sizeof(i32) * h_end.size(), cudaMemcpyHostToDevice, st));
-    xt.x_req = d_req;
-    xt.x_span0 = nullptr; xt.x_spans = nullptr;
-    xt.xdoc = dv.alloc<XDoc>(D + 1, true);
-    LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, xt);
-    if (NCH) {
-        LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 0);
-        LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 1);
-    }
+    BatchTables xt = export_pass(b, h_req);
     LB_BATCH_LAUNCH(b, k_jx_store, nblk(D, 64), 64, 0, b->d_docs, D, xt, d_pf0, d_pfn);
     // every request gets as many output slots as its document has stored changes
     std::vector<XDoc> xd(D);
@@ -1415,9 +1415,34 @@ void json_requests(lb_batch* b, const lb_json_request* reqs, size_t n, lb_export
         else e.answers[of[k]] = lb_exports::Answer{LB_OK, nullptr, host + jr[k].off, (size_t)jr[k].len};
     }
     if (d_out) dv.release(d_out);
-    dv.release(d_req); dv.release(d_jr); dv.release(s.start); dv.release(s.end); dv.release(s.reg); dv.release(s.ord);
+    dv.release(xt.x_req); dv.release(d_jr); dv.release(s.start); dv.release(s.end); dv.release(s.reg); dv.release(s.ord);
     dv.release(s.cur); dv.release(d_pf0); dv.release(d_pfn); dv.release(xt.xdoc); dv.release(d_och); dv.release(d_oreq);
     dv.release(d_olen); dv.release(d_ooff);
+}
+
+// The body of the lb_batch_export_* calls: the batch and every request are checked before anything launches (a request's
+// document index, then refused(request): why its pointers are bad, or nullptr), then answer() fills one answer per
+// request under the batch's export lock.
+template <class Req, class Refused>
+lb_status export_call(const lb_batch* cb, const Req* reqs, size_t n_reqs, lb_exports** out, Refused refused,
+                      void (*answer)(lb_batch*, const Req*, size_t, lb_exports&)) {
+    lb_batch* b = const_cast<lb_batch*>(cb);
+    if (!b || !out || (!reqs && n_reqs)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
+    *out = nullptr;
+    if (!(b->flags & LB_FLAG_EXPORT)) { g_last_error = "batch was imported without LB_FLAG_EXPORT"; return LB_ERR_INVALID_ARG; }
+    for (size_t i = 0; i < n_reqs; i++) {
+        if (reqs[i].doc >= b->n_docs) { g_last_error = "document index out of range"; return LB_ERR_INVALID_ARG; }
+        if (const char* err = refused(reqs[i])) { g_last_error = err; return LB_ERR_INVALID_ARG; }
+    }
+    std::unique_ptr<lb_exports> e(new lb_exports());
+    std::lock_guard<std::mutex> g(b->export_mu);
+    try {
+        answer(b, reqs, n_reqs, *e);
+    } catch (lb_status s) {
+        return s;
+    }
+    *out = e.release();
+    return LB_OK;
 }
 
 }  // namespace
@@ -1825,66 +1850,21 @@ lb_status lb_doc_export_updates(const lb_batch* cb, size_t doc, const lb_id_span
 }
 
 lb_status lb_batch_export_updates(const lb_batch* cb, const lb_export_request* reqs, size_t n_reqs, lb_exports** out) {
-    lb_batch* b = const_cast<lb_batch*>(cb);
-    if (!b || !out || (!reqs && n_reqs)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
-    *out = nullptr;
-    if (!(b->flags & LB_FLAG_EXPORT)) { g_last_error = "batch was imported without LB_FLAG_EXPORT"; return LB_ERR_INVALID_ARG; }
-    for (size_t i = 0; i < n_reqs; i++) {
-        if (reqs[i].doc >= b->n_docs) { g_last_error = "document index out of range"; return LB_ERR_INVALID_ARG; }
-        if (!reqs[i].from && reqs[i].n_from) { g_last_error = "null from with n_from > 0"; return LB_ERR_INVALID_ARG; }
-    }
-    std::unique_ptr<lb_exports> e(new lb_exports());
-    std::lock_guard<std::mutex> g(b->export_mu);
-    try {
-        export_requests(b, reqs, n_reqs, *e);
-    } catch (lb_status s) {
-        return s;
-    }
-    *out = e.release();
-    return LB_OK;
+    return export_call(cb, reqs, n_reqs, out, [](const lb_export_request& r) -> const char* {
+        return !r.from && r.n_from ? "null from with n_from > 0" : nullptr;
+    }, export_requests);
 }
 
 lb_status lb_batch_export_updates_in_range(const lb_batch* cb, const lb_range_request* reqs, size_t n_reqs, lb_exports** out) {
-    lb_batch* b = const_cast<lb_batch*>(cb);
-    if (!b || !out || (!reqs && n_reqs)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
-    *out = nullptr;
-    if (!(b->flags & LB_FLAG_EXPORT)) { g_last_error = "batch was imported without LB_FLAG_EXPORT"; return LB_ERR_INVALID_ARG; }
-    for (size_t i = 0; i < n_reqs; i++) {
-        if (reqs[i].doc >= b->n_docs) { g_last_error = "document index out of range"; return LB_ERR_INVALID_ARG; }
-        if (!reqs[i].spans && reqs[i].n_spans) { g_last_error = "null spans with n_spans > 0"; return LB_ERR_INVALID_ARG; }
-    }
-    std::unique_ptr<lb_exports> e(new lb_exports());
-    std::lock_guard<std::mutex> g(b->export_mu);
-    try {
-        export_range_requests(b, reqs, n_reqs, *e);
-    } catch (lb_status s) {
-        return s;
-    }
-    *out = e.release();
-    return LB_OK;
+    return export_call(cb, reqs, n_reqs, out, [](const lb_range_request& r) -> const char* {
+        return !r.spans && r.n_spans ? "null spans with n_spans > 0" : nullptr;
+    }, export_range_requests);
 }
 
 lb_status lb_batch_export_json_updates(const lb_batch* cb, const lb_json_request* reqs, size_t n_reqs, lb_exports** out) {
-    lb_batch* b = const_cast<lb_batch*>(cb);
-    if (!b || !out || (!reqs && n_reqs)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
-    *out = nullptr;
-    if (!(b->flags & LB_FLAG_EXPORT)) { g_last_error = "batch was imported without LB_FLAG_EXPORT"; return LB_ERR_INVALID_ARG; }
-    for (size_t i = 0; i < n_reqs; i++) {
-        if (reqs[i].doc >= b->n_docs) { g_last_error = "document index out of range"; return LB_ERR_INVALID_ARG; }
-        if ((!reqs[i].start && reqs[i].n_start) || (!reqs[i].end && reqs[i].n_end)) {
-            g_last_error = "null version with a count > 0";
-            return LB_ERR_INVALID_ARG;
-        }
-    }
-    std::unique_ptr<lb_exports> e(new lb_exports());
-    std::lock_guard<std::mutex> g(b->export_mu);
-    try {
-        json_requests(b, reqs, n_reqs, *e);
-    } catch (lb_status s) {
-        return s;
-    }
-    *out = e.release();
-    return LB_OK;
+    return export_call(cb, reqs, n_reqs, out, [](const lb_json_request& r) -> const char* {
+        return (!r.start && r.n_start) || (!r.end && r.n_end) ? "null version with a count > 0" : nullptr;
+    }, json_requests);
 }
 
 lb_status lb_exports_get(const lb_exports* e, size_t i, const uint8_t** bytes, size_t* len) {

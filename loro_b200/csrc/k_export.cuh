@@ -799,22 +799,42 @@ __device__ inline void xentry_summary(const BatchTables& t, const DocInfo& di, X
     E.last = last;
     E.last_valid = true;
 }
-// Change::slice at the `from` version: what lies before `start` is dropped.  false = nothing left.
-__device__ inline bool xentry_cut(const BatchTables& t, const DocInfo& di, XEntry& E, i32 start) {
-    i32 c0 = t.ch_counter[E.src] + (i32)E.from;
-    if (start <= c0) return true;
-    if (start >= c0 + (i32)E.atoms) return false;
-    xentry_trim_front(t, E, (u32)(start - c0));
-    xentry_summary(t, di, E);
-    return true;
-}
-// Change::slice(start, end) clamped to the entry, which overlaps [start, end)
-__device__ inline void xentry_slice(const BatchTables& t, const DocInfo& di, XEntry& E, i32 start, i32 end) {
+// Change::slice(start, end) clamped to the entry, which overlaps [start, end).  The summary is left to xentry_summary.
+__device__ inline void xentry_slice(const BatchTables& t, XEntry& E, i32 start, i32 end) {
     const i32 c0 = t.ch_counter[E.src] + (i32)E.from;
     if (start > c0) xentry_trim_front(t, E, (u32)(start - c0));
     const i32 c1 = t.ch_counter[E.src] + (i32)E.from;
     if (end < c1 + (i32)E.atoms) xentry_trim_back(t, E, (u32)(end - c1));
-    xentry_summary(t, di, E);
+}
+
+// The import store of one peer, rebuilt from its segments in counter order through xstore_push (insert_change merges,
+// MAX_BLOCK_SIZE splits, RleVec op merges written to the rows' XF_HEAD flags).  Every change the store completes goes to
+// take(change), and at the end its open change, with its accumulated last op.  more() is asked before each change of
+// the peer and before that last one: once it is false, the walk stops.
+template <class More, class Take>
+__device__ inline void xstore_walk(const BatchTables& t, const DocInfo& di, const DocPeer& dp, More more, Take take) {
+    XStore s1;
+    s1.have_block = s1.open_valid = s1.open_starts_block = false; s1.blk_est = 0;
+    XEntry done;
+    bool done_blk = false;
+    for (u32 k = 0; k < dp.ch_count && more(); k++) {
+        u32 pos = (u32)di.ch0 + dp.ch_first + k;
+        u32 ch = t.ch_aorder[pos];
+        u32 nseg = t.ch_nseg[ch];
+        for (u32 q = 0; q < nseg; q++) {
+            u64 sg = q == 0 ? (u64)ch : t.n_changes + t.ch_seg0[ch] + q - 1;
+            XEntry E;
+            E.src = ch; E.from = t.sg_from[sg]; E.pos = pos; E.r0 = t.sg_r0[sg]; E.atoms = t.sg_atoms[sg];
+            E.est_ops = t.sg_est[sg]; E.nmops = t.sg_nmops[sg]; E.ndel = t.sg_ndel[sg]; E.nrows = t.sg_nrows[sg];
+            E.lh_ch = ch; E.lh_row = t.sg_last_head[sg]; E.last_valid = false; E.skip = t.sg_skip[sg]; E.tail = 0;
+            if (xstore_push(t, di, s1, E, done, done_blk)) take(done);
+        }
+    }
+    if (s1.open_valid && more()) {
+        s1.open.last = s1.back;
+        s1.open.last_valid = true;
+        take(s1.open);
+    }
 }
 
 // first final-change slot of a document: one slot per segment, and in an export of chosen spans one more per span of
@@ -853,11 +873,10 @@ __global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, const 
         const u32 sp0 = t.x_spans ? t.x_span0[di.peer0 + p] : 0u;
         const u32 nsp = t.x_spans ? t.x_span0[di.peer0 + p + 1] - sp0 : 1u;
         u32 j = 0;   // the first span not yet finished
-        XStore s1, s2;   // import store, export store
-        s1.have_block = s1.open_valid = s1.open_starts_block = false; s1.blk_est = 0;
-        s2 = s1;
-        // a change the import store completed: its pieces inside the spans go to the export store
-        auto take = [&](const XEntry& c) {
+        XStore s2;   // export store
+        s2.have_block = s2.open_valid = s2.open_starts_block = false; s2.blk_est = 0;
+        // each change of the import store: its pieces inside the spans go to the export store; the walk ends with the spans
+        xstore_walk(t, di, dp, [&] { return j < nsp; }, [&](const XEntry& c) {
             const i32 c0 = t.ch_counter[c.src] + (i32)c.from, c1 = c0 + (i32)c.atoms;
             while (j < nsp) {
                 XSpan s;
@@ -870,7 +889,10 @@ __global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, const 
                         s2.have_block = s2.open_valid = false;
                     }
                     XEntry piece = c;
-                    if (s.start > c0 || s.end < c1) xentry_slice(t, di, piece, s.start, s.end);
+                    if (s.start > c0 || s.end < c1) {
+                        xentry_slice(t, piece, s.start, s.end);
+                        xentry_summary(t, di, piece);
+                    }
                     XEntry d2;
                     bool d2_blk = false;
                     if (xstore_push(t, di, s2, piece, d2, d2_blk)) emit(d2, d2_blk);
@@ -878,27 +900,7 @@ __global__ void k_exp_store(const DocInfo* __restrict__ docs, u32 n_docs, const 
                 if (s.end > c1) break;
                 j++;
             }
-        };
-        XEntry done;
-        bool done_blk = false;
-        for (u32 k = 0; k < dp.ch_count && j < nsp; k++) {
-            u32 pos = (u32)di.ch0 + dp.ch_first + k;
-            u32 ch = t.ch_aorder[pos];
-            u32 nseg = t.ch_nseg[ch];
-            for (u32 q = 0; q < nseg; q++) {
-                u64 sg = q == 0 ? (u64)ch : t.n_changes + t.ch_seg0[ch] + q - 1;
-                XEntry E;
-                E.src = ch; E.from = t.sg_from[sg]; E.pos = pos; E.r0 = t.sg_r0[sg]; E.atoms = t.sg_atoms[sg];
-                E.est_ops = t.sg_est[sg]; E.nmops = t.sg_nmops[sg]; E.ndel = t.sg_ndel[sg]; E.nrows = t.sg_nrows[sg];
-                E.lh_ch = ch; E.lh_row = t.sg_last_head[sg]; E.last_valid = false; E.skip = t.sg_skip[sg]; E.tail = 0;
-                if (xstore_push(t, di, s1, E, done, done_blk)) take(done);
-            }
-        }
-        if (s1.open_valid && j < nsp) {
-            s1.open.last = s1.back;
-            s1.open.last_valid = true;
-            take(s1.open);
-        }
+        });
         if (s2.open_valid) emit(s2.open, s2.open_starts_block);
     }
     x.n_fc = (u32)(w - w0);

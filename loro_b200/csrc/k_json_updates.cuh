@@ -8,14 +8,13 @@
 //   list_op.rs:603-658 (Op::slice), outdated_encode_reordered.rs:318-352 (create / move / delete of a tree op).
 //
 // The JSON lists the document's STORED changes (iter_changes_peer_by_peer walks the change store): k_jx_store rebuilds
-// the import store exactly as k_exp_store's `s1` does (xstore_push: insert_change merges, MAX_BLOCK_SIZE splits, RleVec
-// op merges written to the rows' XF_HEAD flags) and lists each stored change once in the fc_* tables, per peer slot.
-// k_jx_order (a thread per request) then orders the stored changes that overlap [start, end) by lamport -- a P-way merge
-// of the per-peer lists, ties by ascending peer id (the reference leaves them in FxHashMap order) -- lists them and
+// the import store with k_exp_store's walk (xstore_walk) and lists each stored change once in the fc_* tables, per peer
+// slot.  k_jx_order (a thread per request) then orders the stored changes that overlap [start, end) by lamport -- a P-way
+// merge of the per-peer lists, ties by ascending peer id (the reference leaves them in FxHashMap order) -- lists them and
 // registers the peers in first-use order.  The text is printed a thread per output change: k_jx_changes counts each
-// change's bytes (cutting it to [start, end): xentry_cut in front, the end cut here), the host scans the sizes and places
-// every request, and k_jx_changes writes each change while k_jx_envelope writes each request's head and tail, one chunk
-// of requests at a time.
+// change's bytes (cutting it to [start, end) with the export's xentry_slice, whose end cut the op gather honours), the
+// host scans the sizes and places every request, and k_jx_changes writes each change while k_jx_envelope writes each
+// request's head and tail, one chunk of requests at a time.
 #pragma once
 #include "k_export.cuh"
 #include "k_resolve.cuh"
@@ -46,7 +45,7 @@ struct JxScratch {   // per request and document peer slot
     u32* cur;        // merge cursor: next stored change of the peer (index relative to the peer's first)
 };
 
-// thread per requested document: the import store (k_exp_store's s1 alone), its changes listed peer by peer in fc_*;
+// thread per requested document: the import store (xstore_walk), its changes listed peer by peer in slot order in fc_*;
 // pf0 / pfn[peer slot] = first stored change of the peer (relative to the document's first) and how many it has
 __global__ void k_jx_store(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t,
                            u32* __restrict__ pf0, u32* __restrict__ pfn) {
@@ -57,32 +56,13 @@ __global__ void k_jx_store(const DocInfo* __restrict__ docs, u32 n_docs, const _
     if (di.code != DOC_OK || (x.flags & 1)) return;
     const u64 w0 = di.ch0 + t.ch_seg0[di.ch0];
     u64 w = w0;
-    auto emit = [&](const XEntry& e) {
-        t.fc_src[w] = e.src; t.fc_pos[w] = e.pos; t.fc_r0[w] = e.r0; t.fc_from[w] = e.from; t.fc_atoms[w] = e.atoms;
-        t.fc_nrows[w] = e.nrows; t.fc_skip[w] = e.skip;
-        w++;
-    };
     for (u32 p = 0; p < di.P; p++) {
-        const DocPeer& dp = t.dpeer[di.peer0 + p];
         pf0[di.peer0 + p] = (u32)(w - w0);
-        XStore s1;
-        s1.have_block = s1.open_valid = s1.open_starts_block = false; s1.blk_est = 0;
-        XEntry done;
-        bool done_blk = false;
-        for (u32 k = 0; k < dp.ch_count; k++) {
-            u32 pos = (u32)di.ch0 + dp.ch_first + k;
-            u32 ch = t.ch_aorder[pos];
-            u32 nseg = t.ch_nseg[ch];
-            for (u32 q = 0; q < nseg; q++) {
-                u64 sg = q == 0 ? (u64)ch : t.n_changes + t.ch_seg0[ch] + q - 1;
-                XEntry E;
-                E.src = ch; E.from = t.sg_from[sg]; E.pos = pos; E.r0 = t.sg_r0[sg]; E.atoms = t.sg_atoms[sg];
-                E.est_ops = t.sg_est[sg]; E.nmops = t.sg_nmops[sg]; E.ndel = t.sg_ndel[sg]; E.nrows = t.sg_nrows[sg];
-                E.lh_ch = ch; E.lh_row = t.sg_last_head[sg]; E.last_valid = false; E.skip = t.sg_skip[sg]; E.tail = 0;
-                if (xstore_push(t, di, s1, E, done, done_blk)) emit(done);
-            }
-        }
-        if (s1.open_valid) emit(s1.open);
+        xstore_walk(t, di, t.dpeer[di.peer0 + p], [] { return true; }, [&](const XEntry& e) {
+            t.fc_src[w] = e.src; t.fc_pos[w] = e.pos; t.fc_r0[w] = e.r0; t.fc_from[w] = e.from; t.fc_atoms[w] = e.atoms;
+            t.fc_nrows[w] = e.nrows; t.fc_skip[w] = e.skip;
+            w++;
+        });
         pfn[di.peer0 + p] = (u32)(w - w0) - pf0[di.peer0 + p];
     }
     x.n_fc = (u32)(w - w0);
@@ -221,8 +201,8 @@ struct JxWriter {
         return la < lb ? -1 : (la > lb ? 1 : 0);
     }
 
-    // the stored change k as it lies in [start, end) of its peer: false when nothing of it does
-    __device__ bool entry(u32 p, u32 k, XEntry& E, u32& keep) {
+    // the stored change k cut to [start, end) of its peer (Change::slice at both ends): false when nothing of it lies there
+    __device__ bool entry(u32 p, u32 k, XEntry& E) {
         const u64 f = fc_base + pf0[di.peer0 + p] + k;
         E.src = t.fc_src[f]; E.from = t.fc_from[f]; E.pos = t.fc_pos[f]; E.r0 = t.fc_r0[f]; E.atoms = t.fc_atoms[f];
         E.nrows = t.fc_nrows[f]; E.skip = t.fc_skip[f]; E.tail = 0; E.last_valid = false;
@@ -230,26 +210,21 @@ struct JxWriter {
         if (st >= en) return false;   // from.diff_iter(to) holds nothing of the peer
         const i32 c0 = t.ch_counter[E.src] + (i32)E.from;
         if (c0 >= en || c0 + (i32)E.atoms <= st) return false;
-        if (st > c0 && !xentry_cut(t, di, E, st)) return false;
-        const i32 c1 = t.ch_counter[E.src] + (i32)E.from;
-        keep = (u32)(en - c1) < E.atoms ? (u32)(en - c1) : E.atoms;   // Change::slice(0, end - counter)
+        xentry_slice(t, E, st, en);
         return true;
     }
 
-    // the ops of E up to `keep` atoms: f(op, atoms kept, cursor at its first row, atoms of that row outside the op)
+    // the ops of E: f(op, cursor at its first row, atoms of that row outside the op)
     template <class F>
-    __device__ void ops(const XEntry& E, u32 keep, F f) {
+    __device__ void ops(const XEntry& E, F f) {
         XRows it(t, E.pos, E.r0);
         u32 left = E.nrows;
         bool first = true;
-        while (left && keep) {
+        while (left) {
             XRows at = it;
             const u32 skip = first ? E.skip : it.skip;
             first = false;
-            XOp op = xop_gather(t, di, it, left, skip);
-            const u32 take = op.atoms < keep ? op.atoms : keep;
-            f(op, take, at, skip);
-            keep -= take;
+            f(xop_gather(t, di, it, left, skip, E.tail), at, skip);
         }
     }
     // the items (List) or text (Text) of an insert, `take` atoms from the cursor on: f(cursor, payload of the row
@@ -269,12 +244,12 @@ struct JxWriter {
 
     // encode_change's register order (json_schema.rs:301-548): per op its container (normal ids), the containers among
     // its values, a delete's start id, a tree op's target and parent; then the change id; then the sorted deps
-    __device__ void register_change(const XEntry& E, u32 keep, u32 cp) {
-        ops(E, keep, [&](const XOp& op, u32 take, XRows at, u32 skip) {
+    __device__ void register_change(const XEntry& E, u32 cp) {
+        ops(E, [&](const XOp& op, XRows at, u32 skip) {
             const DocContainer& dc = t.dcont[di.cid0 + op.cidx];
             if (!dc.is_root) reg(dc.key_or_peer);
             if (op.xk == XK_LIST) {
-                payload(at, skip, XK_LIST, take, [&](XRows&, const u8* pp, u32 pn, u32 n, u32) {
+                payload(at, skip, XK_LIST, op.atoms, [&](XRows&, const u8* pp, u32 pn, u32 n, u32) {
                     Cur c(pp, pn);
                     for (u32 i = 0; i < n && !c.err; i++) { u8 k = c.get(); if (k == 9) reg(cp); skip_loro_value_content(c, k, nullptr); }
                 });
@@ -319,7 +294,7 @@ struct JxWriter {
         }
     }
 
-    __device__ void put_change(const XEntry& E, u32 keep) {
+    __device__ void put_change(const XEntry& E) {
         const u32 cp = t.ch_peer[E.src];
         const i32 c0 = t.ch_counter[E.src] + (i32)E.from;
         o.puts_("{\"id\":");
@@ -336,7 +311,7 @@ struct JxWriter {
         else o.puts_("null");
         o.puts_(",\"ops\":[");
         first = true;
-        ops(E, keep, [&](XOp op, u32 take, XRows at, u32 skip) {
+        ops(E, [&](const XOp& op, XRows at, u32 skip) {
             if (!first) o.put(',');
             first = false;
             o.puts_("{\"container\":\"");
@@ -349,7 +324,7 @@ struct JxWriter {
                     o.put_i64(op.prop);
                     o.puts_(text ? ",\"text\":\"" : ",\"value\":[");
                     u32 i = 0;
-                    payload(at, skip, op.xk, take, [&](XRows& r, const u8* pp, u32 pn, u32 n, u32 avail) {
+                    payload(at, skip, op.xk, op.atoms, [&](XRows& r, const u8* pp, u32 pn, u32 n, u32 avail) {
                         if (text) { o.put_escaped(pp, text_byte_index(pp, pn, avail, n)); return; }
                         Cur c(pp, pn);
                         const BlockInfo& blk = t.blocks[t.ch_block[r.ch]];
@@ -359,7 +334,6 @@ struct JxWriter {
                     break;
                 }
                 case XK_DEL: {
-                    xop_slice_back(t, op, at.row(), op.atoms - take);
                     o.puts_("\"delete\",\"pos\":");
                     o.put_i64(op.prop);
                     o.puts_(",\"len\":");
@@ -492,9 +466,8 @@ struct JxWriter {
             if (best == JX_NONE) break;
             const u32 k = s.cur[rq.slot0 + best]++;
             XEntry E;
-            u32 keep = 0;
-            entry(best, k, E, keep);
-            if (compress) register_change(E, keep, t.ch_peer[E.src]);
+            entry(best, k, E);
+            if (compress) register_change(E, t.ch_peer[E.src]);
             och[rq.ch0 + n++] = pf0[di.peer0 + best] + k;
         }
         rq.n_out = n;
@@ -503,10 +476,9 @@ struct JxWriter {
     __device__ void change_text(u32 rel, u32 rank) {
         const u32 p = t.ch_peer[t.fc_src[fc_base + rel]];
         XEntry E;
-        u32 keep = 0;
-        entry(p, rel - pf0[di.peer0 + p], E, keep);
+        entry(p, rel - pf0[di.peer0 + p], E);
         if (rank) o.put(',');
-        put_change(E, keep);
+        put_change(E);
     }
 };
 
