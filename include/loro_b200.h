@@ -28,6 +28,9 @@
  *   lb_import_batch_at       crates/loro-internal/src/loro.rs:1353-1433 LoroDoc::checkout(&frontiers) after the import,
  *   lb_docset_checkout       then get_deep_value() (the state at an earlier version: time travel)
  *   lb_docset_read           a stored document's get_deep_value / oplog_vv / oplog_frontiers / export, nothing imported
+ *   lb_doc_attribution       who wrote the state, for the whole document: crates/loro/src/lib.rs:2644
+ *                            LoroText::get_editor_at_unicode_pos, :1906 LoroList::get_id_at, :2117 LoroMap::get_last_editor,
+ *                            :3046 LoroTree::get_last_move_id
  *
  * Conventions (mirroring the reference): input buffers are borrowed for the duration of the call only;
  * outputs are owned by the batch handle until lb_batch_free; a bad blob never aborts the batch -- it yields a
@@ -86,6 +89,7 @@ typedef struct lb_options {
 #define LB_FLAG_KEEP_DEVICE 2u  /* keep intermediate device tables for lb_debug_* (tests) */
 #define LB_FLAG_EXPORT 4u       /* also re-export every document (phase 7) for lb_doc_export_updates */
 #define LB_FLAG_COMPACT 8u      /* lb_docset_import: afterwards keep each touched document as its own export (see below) */
+#define LB_FLAG_ATTRIBUTION 16u /* also compute each document's attribution (phase 6b) for lb_doc_attribution */
 
 typedef struct lb_id_span {
     uint64_t peer;
@@ -133,6 +137,7 @@ typedef struct lb_timings { /* device time per phase in milliseconds (CUDA event
     /* host wall time of the whole import call, and of its tail: from the moment the last kernel was enqueued (results
      * download, status tables) -- what a step costs beyond `total_device` */
     float host_call_ms, host_tail_ms;
+    float attribution;                 /* attribution phase (LB_FLAG_ATTRIBUTION; 0 without it) */
 } lb_timings;
 
 typedef struct lb_batch lb_batch;
@@ -151,6 +156,22 @@ size_t lb_doc_count(const lb_batch* b);
 lb_status lb_doc_status(const lb_batch* b, size_t doc, lb_import_status* out);
 lb_status lb_doc_json(const lb_batch* b, size_t doc, const char** utf8, size_t* len);
 lb_status lb_doc_vv(const lb_batch* b, size_t doc, const lb_id_span** spans, size_t* n); /* start=0,end=vv[peer] */
+/* Who wrote each part of the document's state, at the version the state was built at (the latest, or the checkout's),
+ * as one UTF-8 JSON object (INTEGRATION.md), canonical so that it compares byte for byte:
+ *   {"peers":["<id>",...],"containers":{"<cid>":<entry>,...}}
+ * `peers` are the peers of the oplog vv as decimal strings, ascending; entries name a peer by its index p there.  A
+ * container is listed by its ContainerID display (full peer id) when it has an entry: root containers first by (name
+ * bytes, type), then normal ones by (peer, counter).  Entries:
+ *   Text / List  [[p,counter,len],...]  the ids of the visible elements in document order, in maximal runs of one peer
+ *                with consecutive counters (Text counts unicode scalar values): get_editor_at_unicode_pos, get_id_at;
+ *   Map          {"<key>":[p,lamport,present],...}  the winning op of every key, a delete included (present = 0), keys
+ *                ascending: get_last_editor;
+ *   Tree         {"<counter>@<peer>":[p,counter,alive],...}  every node the tree state holds, deleted ones included
+ *                (alive = 0), by (peer, counter): [p, counter] is get_last_move_id (creation counts as a move).
+ * Needs LB_FLAG_ATTRIBUTION at import (accepted by every import entry point, checkouts included; independent of
+ * LB_FLAG_NO_JSON and LB_FLAG_EXPORT), otherwise LB_ERR_INVALID_ARG.  A document that failed to import (any code but
+ * LB_DOC_OK) gives an empty string.  The bytes are owned by the batch. */
+lb_status lb_doc_attribution(const lb_batch* b, size_t doc, const char** utf8, size_t* len);
 /* LoroDoc::oplog_frontiers() (crates/loro/src/lib.rs:881; version/frontiers.rs:233-246): the heads of the causal graph,
  * one span [counter, counter + 1) per head id. */
 lb_status lb_doc_frontiers(const lb_batch* b, size_t doc, const lb_id_span** spans, size_t* n);

@@ -11,6 +11,7 @@ LB_FLAG_NO_JSON = 1
 LB_FLAG_KEEP_DEVICE = 2
 LB_FLAG_EXPORT = 4
 LB_FLAG_COMPACT = 8
+LB_FLAG_ATTRIBUTION = 16
 
 DOC_CODES = {0: "Ok", 1: "DecodeError", 2: "DecodeChecksumMismatchError", 3: "IncompatibleFutureEncodingError",
              4: "DecodeDataCorruptionError", 5: "Unsupported", 6: "CapacityExceeded", 7: "FrontiersNotFound"}
@@ -79,7 +80,7 @@ class _Timings(ctypes.Structure):
                 ("decode_fast_blocks", ctypes.c_uint64), ("decode_lane_blocks", ctypes.c_uint64),
                 ("decode_unstaged_blocks", ctypes.c_uint64),
                 ("alloc_host_ms", ctypes.c_float), ("reserved1", ctypes.c_uint32), ("device_bytes", ctypes.c_uint64),
-                ("host_call_ms", ctypes.c_float), ("host_tail_ms", ctypes.c_float)]
+                ("host_call_ms", ctypes.c_float), ("host_tail_ms", ctypes.c_float), ("attribution", ctypes.c_float)]
 
 
 _libs = {}
@@ -106,6 +107,7 @@ def load_library(path=None):
     L.lb_doc_count.argtypes = [vp]
     L.lb_doc_status.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(_Status)]
     L.lb_doc_json.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_size_t)]
+    L.lb_doc_attribution.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_size_t)]
     L.lb_doc_export_updates.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(_IdSpan), ctypes.c_size_t,
                                         ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_size_t)]
     L.lb_batch_export_updates.argtypes = [vp, ctypes.POINTER(_ExportRequest), ctypes.c_size_t, ctypes.POINTER(vp)]
@@ -309,6 +311,32 @@ class Batch:
         _check(self._L, self._L.lb_doc_json(self._h, i, ctypes.byref(p), ctypes.byref(n)), "lb_doc_json")
         return ctypes.string_at(p, n.value)
 
+    def attribution_bytes(self, i):
+        """who wrote document i's state, as the engine's canonical JSON (lb_doc_attribution; needs
+        flags=LB_FLAG_ATTRIBUTION at import).  Empty for a document that failed to import."""
+        p = ctypes.c_char_p()
+        n = ctypes.c_size_t()
+        _check(self._L, self._L.lb_doc_attribution(self._h, i, ctypes.byref(p), ctypes.byref(n)), "lb_doc_attribution")
+        return ctypes.string_at(p, n.value)
+
+    def attribution(self, i):
+        """attribution_bytes(i) parsed, peer indices resolved to peer ids: {container id: entry}, where a Text / List
+        entry is [(peer, counter, len), ...] (the ids of its visible elements, in runs), a Map entry {key: (peer,
+        lamport, present)} (the winning write of every key, LoroMap::get_last_editor) and a Tree entry {node: (peer,
+        counter, alive)} (the node's last move, LoroTree::get_last_move_id).  None for a document that failed."""
+        raw = self.attribution_bytes(i)
+        if not raw:
+            return None
+        doc = json.loads(raw)
+        peers = [int(p) for p in doc["peers"]]
+        out = {}
+        for cid, entry in doc["containers"].items():
+            if isinstance(entry, list):
+                out[cid] = [(peers[p], c, n) for p, c, n in entry]
+            else:
+                out[cid] = {k: (peers[p], c, bool(f)) for k, (p, c, f) in entry.items()}
+        return out
+
     def fetch_json(self):
         """make sure the JSON of every document of the batch is in host memory (one download of the whole buffer)"""
         if self.n_docs:
@@ -383,6 +411,8 @@ class MultiBatch:
 
     def status(self, i): p, j = self._loc(i); return p.status(j)
     def json_bytes(self, i): p, j = self._loc(i); return p.json_bytes(j)
+    def attribution_bytes(self, i): p, j = self._loc(i); return p.attribution_bytes(j)
+    def attribution(self, i): p, j = self._loc(i); return p.attribution(j)
     def get_deep_value(self, i): p, j = self._loc(i); return p.get_deep_value(j)
     def oplog_vv(self, i): p, j = self._loc(i); return p.oplog_vv(j)
     def oplog_frontiers(self, i): p, j = self._loc(i); return p.oplog_frontiers(j)

@@ -31,6 +31,7 @@
 #include "k_state.cuh"
 #include "k_export.cuh"
 #include "k_json_updates.cuh"
+#include "k_attr.cuh"
 #include "host_stage.hpp"
 
 static thread_local std::string g_last_error;
@@ -318,7 +319,7 @@ struct Dev {  // owns every device allocation of a batch
 // Events on the batch stream, in pipeline order: EV_x is recorded when phase x has been enqueued (mark), and a phase's
 // device time is the interval from the event before it (timings_from_events).
 enum BatchEvent { EV_START, EV_H2D, EV_FRAME, EV_DECODE, EV_RESOLVE, EV_CLASSIFY, EV_INTEGRATE, EV_TREE, EV_MATERIALISE,
-                  EV_EXPORT, EV_D2H, EV_COUNT };
+                  EV_ATTRIBUTION, EV_EXPORT, EV_D2H, EV_COUNT };
 
 struct lb_batch {
     Dev dev;
@@ -342,6 +343,13 @@ struct lb_batch {
     DocInfo* d_docs = nullptr;
     u8* d_json = nullptr;
     u8* d_export = nullptr;      // phase 7 output: one FastUpdates blob per document
+    // LB_FLAG_ATTRIBUTION (k_attr.cuh): document d's text is [attr_off[d], attr_off[d + 1]) of d_attr; both come home on
+    // the first lb_doc_attribution
+    u8* d_attr = nullptr;
+    u64* d_attr_off = nullptr;
+    char* attr = nullptr;
+    std::vector<u64> attr_off;
+    bool attr_fetched = false;
     u64 export_total = 0;
     std::vector<XDoc> xdocs;
     std::unordered_map<size_t, std::vector<uint8_t>> from_exports;   // last lb_doc_export_updates(from) per document
@@ -798,6 +806,21 @@ void pipeline(lb_batch* b) {
             b->json_ok = ok;
         });
     }
+    // ------------------------------------------------------------ phase 6b: attribution (reads out_*, map_*, tn_*)
+    if (b->flags & LB_FLAG_ATTRIBUTION) {
+        u32* cord = dv.alloc<u32>(NC + 1);
+        u32* kord = dv.alloc<u32>(NK + 1);
+        u32* d_attr_len = dv.alloc<u32>(D + 1);
+        b->d_attr_off = dv.alloc<u64>(D + 1);
+        LB_BATCH_LAUNCH(b, k_attr, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t, cord, kord, d_attr_len,
+                        (const u64*)nullptr, (u8*)nullptr, 0);
+        run_scans(b, {ScanJob{(const u8*)d_attr_len, (u8*)b->d_attr_off, 4, 8, D}});
+        const u64 AT = d2h_one(b, b->d_attr_off + D);
+        b->d_attr = dv.alloc<u8>(AT + 16);
+        LB_BATCH_LAUNCH(b, k_attr, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t, cord, kord, d_attr_len,
+                        (const u64*)b->d_attr_off, b->d_attr, 1);
+    }
+    mark(b, EV_ATTRIBUTION);
     // ------------------------------------------------------------ phase 7: re-export (all_updates per document)
     if (b->flags & LB_FLAG_EXPORT) {
         trace_point(b, "before export");
@@ -945,7 +968,8 @@ void timings_from_events(lb_batch* b) {
     t.integrate = el(EV_CLASSIFY, EV_INTEGRATE);
     t.tree = el(EV_INTEGRATE, EV_TREE);
     t.materialise = el(EV_TREE, EV_MATERIALISE);
-    t.reexport = el(EV_MATERIALISE, EV_EXPORT);
+    t.attribution = el(EV_MATERIALISE, EV_ATTRIBUTION);
+    t.reexport = el(EV_ATTRIBUTION, EV_EXPORT);
     t.d2h = el(EV_EXPORT, EV_D2H);
     t.total_device = el(EV_H2D, EV_EXPORT);
 }
@@ -1806,6 +1830,32 @@ lb_status lb_doc_json(const lb_batch* cb, size_t doc, const char** utf8, size_t*
     return LB_OK;
 }
 
+lb_status lb_doc_attribution(const lb_batch* cb, size_t doc, const char** utf8, size_t* len) {
+    lb_batch* b = const_cast<lb_batch*>(cb);
+    if (!b || !utf8 || !len || doc >= b->n_docs) { g_last_error = "bad argument"; return LB_ERR_INVALID_ARG; }
+    if (!(b->flags & LB_FLAG_ATTRIBUTION)) { g_last_error = "batch was imported without LB_FLAG_ATTRIBUTION"; return LB_ERR_INVALID_ARG; }
+    if (!b->attr_fetched) {   // one download of the whole buffer
+        b->attr_off.assign(b->n_docs + 1, 0);
+        if (cudaMemcpy(b->attr_off.data(), b->d_attr_off, sizeof(u64) * (b->n_docs + 1), cudaMemcpyDeviceToHost) != cudaSuccess) {
+            g_last_error = "attribution d2h failed";
+            return LB_ERR_CUDA;
+        }
+        const u64 total = b->attr_off[b->n_docs];
+        b->attr = (char*)lbstage::host_cache().take(total + 1);
+        if (!b->attr) { g_last_error = "out of host memory"; return LB_ERR_OOM; }
+        if (total && !lbstage::download(b->d_attr, (u8*)b->attr, total, b->dev.stream)) {
+            g_last_error = "attribution d2h failed";
+            return LB_ERR_CUDA;
+        }
+        b->attr[total] = 0;
+        b->attr_fetched = true;
+    }
+    if (b->docs[doc].code != DOC_OK) { *utf8 = ""; *len = 0; return LB_OK; }
+    *utf8 = b->attr + b->attr_off[doc];
+    *len = b->attr_off[doc + 1] - b->attr_off[doc];
+    return LB_OK;
+}
+
 lb_status lb_doc_export_updates(const lb_batch* cb, size_t doc, const lb_id_span* from, size_t n_from,
                                 const uint8_t** bytes, size_t* len) {
     lb_batch* b = const_cast<lb_batch*>(cb);
@@ -1941,6 +1991,7 @@ void lb_batch_free(lb_batch* b) {
     }
     lbstage::host_cache().give(b->json);
     lbstage::host_cache().give(b->exported);
+    lbstage::host_cache().give(b->attr);
     delete b;
 }
 

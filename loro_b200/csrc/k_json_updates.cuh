@@ -37,6 +37,22 @@ struct JxReq {       // one request as the host lays it out
     u32 pre_len;     // bytes of the envelope in front of the changes (k_jx_order)
     u32 pad;
 };
+// ContainerType's name as ContainerID's Display prints it
+__device__ inline void put_ctype(Sink& o, u8 type) {
+    const char* names[6] = {"Map", "List", "Text", "Tree", "MovableList", "Counter"};
+    o.puts_(type < 6 ? names[type] : "Unknown");
+}
+// ContainerID's Display (loro-common/src/lib.rs:480-500) without the quotes; put_peer(p) prints the creator of a normal
+// container from its doc peer index (the JSON writer prints a register index or the id, k_attr.cuh the id)
+template <class PutPeer>
+__device__ __forceinline__ void put_cid_to(Sink& o, const BatchTables& t, const DocInfo& di, u32 cidx, PutPeer put_peer) {
+    const DocContainer& dc = t.dcont[di.cid0 + cidx];
+    if (dc.is_root) { o.puts_("cid:root-"); o.put_escaped(t.bytes + dc.name_off, dc.name_len); }
+    else { o.puts_("cid:"); o.put_i64(dc.counter); o.put('@'); put_peer(dc.key_or_peer); }
+    o.put(':');
+    put_ctype(o, dc.type);
+}
+
 struct JxScratch {   // per request and document peer slot
     i32* start;      // refined start_vv / end_vv (json_schema.rs:31-45: clamped to the oplog vv, 0 when absent)
     i32* end;
@@ -88,18 +104,8 @@ struct JxWriter {
     }
     __device__ void put_peer(u32 p) { if (compress) o.put_u64(s.reg[rq.slot0 + p]); else o.put_u64(t.dpeer[di.peer0 + p].id); }
     __device__ void put_id(u32 p, i64 ctr) { o.put('"'); o.put_i64(ctr); o.put('@'); put_peer(p); o.put('"'); }
-    __device__ void put_type(u8 type) {
-        const char* names[6] = {"Map", "List", "Text", "Tree", "MovableList", "Counter"};
-        o.puts_(type < 6 ? names[type] : "Unknown");
-    }
-    // ContainerID's Display (loro-common/src/lib.rs:480-500) without the quotes
-    __device__ void put_cid(u32 cidx) {
-        const DocContainer& dc = t.dcont[di.cid0 + cidx];
-        if (dc.is_root) { o.puts_("cid:root-"); o.put_escaped(t.bytes + dc.name_off, dc.name_len); }
-        else { o.puts_("cid:"); o.put_i64(dc.counter); o.put('@'); put_peer(dc.key_or_peer); }
-        o.put(':');
-        put_type(dc.type);
-    }
+    __device__ void put_type(u8 type) { put_ctype(o, type); }
+    __device__ void put_cid(u32 cidx) { put_cid_to(o, t, di, cidx, [&](u32 p) { put_peer(p); }); }
 
     // a LoroValue at c (kind byte + content), serde_json text (loro-common/src/value.rs:692-711): object keys ascending,
     // the later of two equal keys wins, a container is "🦜:" + its id, which is (peer, ctr) of the atom that created it.
