@@ -838,7 +838,7 @@ void pipeline(lb_batch* b) {
         t.ch_aval = dv.alloc<u32>(NCH + 1, true); t.ch_astr = dv.alloc<u32>(NCH + 1, true);
         t.ch_aval0 = dv.alloc<u64>(NCH + 2, true); t.ch_astr0 = dv.alloc<u64>(NCH + 2, true);
         // segment / final-change records: one slot per change + one per extra segment of a split change; the
-        // extras are counted by pass 0, so the arrays are sized with a bound first and checked after the scan
+        // extras are counted by k_exp_changes, so the arrays are sized with a bound first and checked after the scan
         u64 SEGCAP = NCH + NCH / 4 + 1024;
         if (getenv("LB_EXPORT_TIGHT_SEGCAP")) SEGCAP = NCH;   // testing hook: force the growth path
         // the u32 tables of the two groups (SG_TABLES, FC_TABLES) in allocation order; the *_skip and fc_tail tables
@@ -852,10 +852,10 @@ void pipeline(lb_batch* b) {
         trace_point(b, "export allocs");
         LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, t);
         if (NTR) LB_BATCH_LAUNCH(b, k_exp_posrank, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t);
-        if (NCH) LB_BATCH_LAUNCH(b, k_exp_arena, nblk(NCH, 64), 64, 0, NCH, t, b->d_docs);
+        if (NCH) LB_BATCH_LAUNCH(b, k_exp_arena, nblk(NCH * 32, XCH_TPB), XCH_TPB, 0, NCH, t, b->d_docs);
         run_scans(b, {ScanJob{(const u8*)t.ch_aval, (u8*)t.ch_aval0, 4, 8, NCH}, ScanJob{(const u8*)t.ch_astr, (u8*)t.ch_astr0, 4, 8, NCH}});
         trace_point(b, "posrank+arena");
-        if (NCH) LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, t, 0);
+        if (NCH) LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH * 32, XCH_TPB), XCH_TPB, 0, b->d_docs, NCH, t);
         trace_point(b, "changes pass 0");
         run_scans(b, {ScanJob{(const u8*)t.ch_novf, (u8*)t.ch_seg0, 4, 8, NCH}, ScanJob{(const u8*)t.ch_syn, (u8*)t.ch_syn0, 4, 8, NCH}});
         u64 NOVF = d2h_one(b, t.ch_seg0 + NCH);
@@ -863,7 +863,7 @@ void pipeline(lb_batch* b) {
         t.has_syn = NSYN ? 1 : 0;
         t.s_rec = dv.alloc<uint4>(NSYN); t.s_len = dv.alloc<u32>(NSYN); t.s_bytes = dv.alloc<u32>(NSYN);
         t.s_flag = dv.alloc<u8>(NSYN); t.s_voff = dv.alloc<u64>(NSYN); t.s_vlen = dv.alloc<u32>(NSYN); t.s_aux = dv.alloc<u32>(NSYN);
-        if (NCH + NOVF > SEGCAP) {   // unusually many split changes: grow the tables, keep what pass 0 wrote
+        if (NCH + NOVF > SEGCAP) {   // unusually many split changes: grow the tables, keep what k_exp_changes wrote
             u64 cap = NCH + NOVF;
             for (auto m : SG_TABLES) {
                 u32* nw = dv.alloc<u32>(cap);
@@ -877,7 +877,7 @@ void pipeline(lb_batch* b) {
         }
         b->n_segs = NCH + NOVF;
         b->fc_cap = std::max(SEGCAP, NCH + NOVF);
-        if (NOVF) LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, t, 1);
+        if (NOVF) LB_BATCH_LAUNCH(b, k_exp_split_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, t);
         LB_BATCH_LAUNCH(b, k_exp_store, nblk(D, 64), 64, 0, b->d_docs, D, t);
         u64 XT = 0;
         b->d_export = export_encode(b, t, &XT, false);
@@ -1089,8 +1089,8 @@ lb_exports::Answer doc_error(const DocInfo& di) {
 }
 
 // The start of an on-demand export pass over the documents h_req marks: a copy of the batch's tables with the request
-// mask (x_req) and a fresh XDoc table, and the marked documents' changes prepared for the stores (k_exp_init, both passes
-// of k_exp_changes).  The caller releases xt.x_req and xt.xdoc.
+// mask (x_req) and a fresh XDoc table, and the marked documents' changes prepared for the stores (k_exp_init,
+// k_exp_changes, k_exp_split_changes).  The caller releases xt.x_req and xt.xdoc.
 BatchTables export_pass(lb_batch* b, const std::vector<u8>& h_req) {
     Dev& dv = b->dev;
     const u32 D = (u32)b->n_docs;
@@ -1102,8 +1102,8 @@ BatchTables export_pass(lb_batch* b, const std::vector<u8>& h_req) {
     xt.xdoc = dv.alloc<XDoc>(D + 1, true);
     LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, xt);
     if (NCH) {
-        LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 0);
-        LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt, 1);
+        LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH * 32, XCH_TPB), XCH_TPB, 0, b->d_docs, NCH, xt);
+        LB_BATCH_LAUNCH(b, k_exp_split_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, xt);
     }
     return xt;
 }

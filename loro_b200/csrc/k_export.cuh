@@ -10,9 +10,10 @@
 //   DeltaRle, DeltaOfDelta; SURVEY Appendix B).
 //
 // What the imported document's change store looks like is re-derived from the decoded tables:
-//   A  (thread per change) ops of each decoded change go through the RleVec merge (block_encode.rs:651); a change
-//      whose size estimate exceeds one block is cut into segments (split_change_then_insert), List / Text inserts
-//      that do not fit a block are themselves cut (Op::slice) -- such a change is re-written as synthetic rows;
+//   A  (warp per change, 32 rows at a time) ops of each decoded change go through the RleVec merge
+//      (block_encode.rs:651); a change whose size estimate exceeds one block is cut into segments
+//      (split_change_then_insert, one lane), List / Text inserts that do not fit a block are themselves cut
+//      (Op::slice) -- such a change is re-written as synthetic rows (thread per change);
 //   B  (thread per document, per peer in id order) the segments enter the store in counter order
 //      (ChangeStore::insert_change, merge_interval 0 for imports), and what comes out is pushed, as it completes,
 //   C  into the fresh store export builds (export_blocks_from): same rules, freshly computed sizes.
@@ -333,7 +334,32 @@ __device__ inline void xop_slice_back(const BatchTables& t, XOp& o, u64 row, u32
 // ---------------------------------------------------------------------------------------------- X1: arenas
 // The importing document allocates arena space while it decodes (block_encode.rs:619-657): the position of a row's
 // payload is the sum over the rows decoded before it.  Changes are numbered in decode order, so: per-change sums
-// (thread per change), one scan over the changes, and k_exp_changes hands out the row positions.
+// (warp per change), one scan over the changes, and k_exp_changes hands out the row positions.
+//
+// Every decoded op allocates, applied or still pending (decode precedes the pending check: encoding.rs:232-270), so
+// the arena a row allocates from is taken from (container type, value kind), not from op_kind.
+enum { XA_NONE = 0, XA_VAL = 1, XA_STR = 2 };
+#define XCH_TPB 128   // CTA of the warp-per-change kernels (k_exp_arena, k_exp_changes)
+__device__ __forceinline__ u32 xr_arena(const BatchTables& t, const DocInfo& di, u64 row) {
+    u8 ctype = t.dcont[di.cid0 + t.op_cidx[row]].type;
+    u8 vt = t.op_vtype[row];
+    if (ctype == CT_TEXT && vt == VK_STR) return XA_STR;
+    if (ctype == CT_LIST && vt == VK_LORO_VALUE) return XA_VAL;
+    return XA_NONE;
+}
+__device__ __forceinline__ u32 warp_sum_u32(u32 v) {
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(LB_FULL, v, d);
+    return v;
+}
+__device__ __forceinline__ u32 warp_incl_scan_u32(u32 v, u32 lane) {
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        u32 x = __shfl_up_sync(LB_FULL, v, d);
+        if (lane >= (u32)d) v += x;
+    }
+    return v;
+}
 __global__ void k_exp_init(const DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t) {
     u32 d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_docs) return;
@@ -348,33 +374,35 @@ __global__ void k_exp_init(const DocInfo* __restrict__ docs, u32 n_docs, const _
     }
     t.xdoc[d] = x;
 }
+// warp per change: the lanes take 32 consecutive rows at a time (a change holds some hundreds of rows; a thread per
+// change put the lanes of a warp hundreds of rows apart, one sector per lane for every column it loads)
 __global__ void k_exp_arena(u64 n_changes, const __grid_constant__ BatchTables t, const DocInfo* __restrict__ docs) {
-    u64 ch = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (ch >= n_changes) return;
+    const u64 ch = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const u32 lane = threadIdx.x & 31;
+    if (ch >= n_changes) return;   // (whole warps)
     const BlockInfo& sb = t.blocks[t.ch_block[ch]];
     const DocInfo& di = docs[sb.doc];
     u32 vals = 0, strs = 0;
     if (di.code == DOC_OK) {
-        u64 r0 = t.ch_op0[ch];
-        u32 nr = t.ch_nops[ch];
-        for (u32 r = 0; r < nr; r++) {
-            u64 row = r0 + r;
-            // every decoded op allocates, applied or still pending (decode precedes the pending check:
-            // encoding.rs:232-270), so the op class is taken from (container type, value kind), not from op_kind
-            u8 ctype = t.dcont[di.cid0 + t.op_cidx[row]].type;
-            u8 vt = t.op_vtype[row];
-            bool ins = (ctype == CT_TEXT && vt == VK_STR) || (ctype == CT_LIST && vt == VK_LORO_VALUE);
-            if (!ins) continue;
-            if (ctype == CT_TEXT) {
+        const u64 r0 = t.ch_op0[ch];
+        const u32 nr = t.ch_nops[ch];
+        for (u32 r = lane; r < nr; r += 32) {
+            const u64 row = r0 + r;
+            const u32 a = xr_arena(t, di, row);
+            if (a == XA_STR) {
                 Cur c(t.bytes + t.op_val_off[row], t.op_val_len[row]);
                 u32 n = (u32)c.varint();
                 t.r_bytes[row] = n;
                 strs += n;
-            } else vals += t.op_len[row];
+            } else if (a == XA_VAL) vals += t.op_len[row];
         }
     }
-    t.ch_aval[ch] = vals;
-    t.ch_astr[ch] = strs;
+    vals = warp_sum_u32(vals);
+    strs = warp_sum_u32(strs);
+    if (lane == 0) {
+        t.ch_aval[ch] = vals;
+        t.ch_astr[ch] = strs;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------- A: per change
@@ -488,77 +516,158 @@ __device__ inline void segment_summaries(const BatchTables& t, const DocInfo& di
     }
 }
 
-// thread per change.  pass 0: per-row records, RleVec merge inside the change (XF_HEAD), segment count (XF_SEG marks
-// when no op has to be cut, a synthetic-row count otherwise).  pass 1 (split changes only): synthetic rows, summaries.
-__global__ void k_exp_changes(DocInfo* __restrict__ docs, u64 n_changes, const __grid_constant__ BatchTables t, int pass) {
+// XF_HEAD (the RleVec merge inside a change) from neighbouring rows.  The serial rule keeps `back`, the merged op
+// the previous row ended in, and row r merges when xop_mergable(back, row r).  For List / Text a pairwise test of
+// row r against row r - 1 decides the same thing: every merge of a run required ctr, prop and arena position to
+// continue and kind, container and string generation to be equal, so the run's end counter (ctr + atoms), end
+// position (prop + atoms), arena end (f1) and generation are those of its last row, and those are all the
+// left-hand side of the test reads.  Map and tree ops never merge.  Deletes are not pairwise: after a merge a
+// one-element ("bidi") span has a direction (xop_merge), so runs of delete rows are resolved serially inside the
+// warp, on shuffled registers, with `back` carried across the 32-row chunks.
+//
+// warp per change: per-row records, XF_HEAD, the summary of the change (estimate = per merged op: List
+// 4 x atoms, Text bytes, Del 8, Map 3, Tree 8, which for List / Text is the sum over its rows), segment count (XF_SEG
+// marks when no op has to be cut, a synthetic-row count otherwise; the rare split paths run on lane 0).
+__global__ void k_exp_changes(DocInfo* __restrict__ docs, u64 n_changes, const __grid_constant__ BatchTables t) {
+    const u64 ch = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const u32 lane = threadIdx.x & 31;
+    if (ch >= n_changes) return;   // (whole warps, as are the returns below)
+    if (t.x_req && !t.x_req[t.blocks[t.ch_block[ch]].doc]) return;
+    if (!t.ch_applied[ch]) { if (lane == 0) { t.ch_nseg[ch] = 0; t.ch_syn[ch] = 0; } return; }
+    const u32 doc = t.blocks[t.ch_block[ch]].doc;
+    const DocInfo& di = docs[doc];
+    const u64 r0 = t.ch_op0[ch];
+    const u32 nr = t.ch_nops[ch];
+    // arena positions of the rows (relative to the document): a warp scan per chunk plus what the chunks before used
+    u32 vals = (u32)(t.ch_aval0[ch] - t.ch_aval0[di.ch0]), strs = (u32)(t.ch_astr0[ch] - t.ch_astr0[di.ch0]);
+    // a change whose head the document already had entered the store as a slice (oplog.rs:181-196): rows before the
+    // cut are not part of it, the row under the cut loses its first atoms.  The counters of a change's rows increase,
+    // so the rows cut away are a prefix and r_first is final before the first kept row.
+    const u32 trim = t.ch_trim[ch];
+    const i32 cut = t.ch_counter[ch] + (i32)trim;
+    u32 r_first = 0, skip = 0;
+    u32 est_ops = 0, nm = 0, ndel = 0, last_head = 0;
+    bool bad = false;
+    // lane 0: row r - 1 (the last row of the previous chunk) as the fields the pairwise test reads
+    u32 c_xk = XK_NONE, c_cidx = 0, c_atoms = 0, c_f1 = 0, c_g = 0;
+    i32 c_ctr = 0, c_prop = 0;
+    bool c_del = false;   // the previous chunk's last row is a kept delete
+    XOp back;             // (the same in every lane) the merged delete the last delete row ended in
+    back.xk = XK_NONE;
+    for (u32 c0 = 0; c0 < nr; c0 += 32) {
+        const u32 r = c0 + lane;
+        const bool in = r < nr;
+        const u64 row = r0 + r;
+        const u32 len = in ? t.op_len[row] : 0;
+        const u32 ar = in ? xr_arena(t, di, row) : XA_NONE;
+        const u32 nv = ar == XA_VAL ? len : 0, ns = ar == XA_STR ? t.r_bytes[row] : 0;
+        const u32 iv = warp_incl_scan_u32(nv, lane), is = warp_incl_scan_u32(ns, lane);
+        const u32 astart = ar == XA_STR ? strs + is - ns : (ar == XA_VAL ? vals + iv - nv : 0);
+        vals += __shfl_sync(LB_FULL, iv, 31);
+        strs += __shfl_sync(LB_FULL, is, 31);
+        const i32 ctr = in ? t.op_counter[row] : 0;
+        const bool drop = in && trim && ctr + (i32)len <= cut;
+        const u32 dm = __ballot_sync(LB_FULL, drop);
+        if (dm) r_first = c0 + 32 - __clz(dm);
+        const bool kept = in && !drop;
+        XOp o;
+        o.xk = XK_NONE; o.cidx = 0; o.ctr = 0; o.atoms = 0; o.prop = 0; o.f0 = o.f1 = 0; o.f2 = 0; o.g = 0;
+        o.st0 = 0; o.nst = 1;
+        if (kept) {
+            o = xop_resolve(t, di, (u32)ch, row, astart);
+            t.x_rec[row] = xop_pack(o);
+            if (o.xk == XK_NONE) bad = true;
+            if (r == r_first && trim && ctr < cut) { skip = (u32)(cut - ctr); xop_slice_front(t, o, row, skip); }
+        } else if (in) {
+            t.x_rec[row] = mk4(0, 0, 0, 0);
+            t.r_flag[row] = 0;
+        }
+        // row r - 1 (lane 0 takes what it kept from the previous chunk; the rotation hands it this chunk's last row)
+        XOp p;
+        const int src = (lane + 31) & 31;
+        p.xk = (u8)__shfl_sync(LB_FULL, (u32)o.xk, src);
+        p.cidx = __shfl_sync(LB_FULL, o.cidx, src);
+        p.ctr = __shfl_sync(LB_FULL, o.ctr, src);
+        p.atoms = __shfl_sync(LB_FULL, o.atoms, src);
+        p.prop = __shfl_sync(LB_FULL, o.prop, src);
+        p.f1 = __shfl_sync(LB_FULL, o.f1, src);
+        p.g = __shfl_sync(LB_FULL, o.g, src);
+        p.f0 = 0; p.f2 = 0; p.st0 = 0; p.nst = 1;
+        if (lane == 0) {
+            const u32 xk = p.xk, cidx = p.cidx, atoms = p.atoms, f1 = p.f1, g = p.g;
+            const i32 pc = p.ctr, pp = p.prop;
+            p.xk = (u8)c_xk; p.cidx = c_cidx; p.ctr = c_ctr; p.atoms = c_atoms; p.prop = c_prop; p.f1 = c_f1; p.g = c_g;
+            c_xk = xk; c_cidx = cidx; c_ctr = pc; c_atoms = atoms; c_prop = pp; c_f1 = f1; c_g = g;
+        }
+        bool head = !(kept && o.xk != XK_DEL && r > r_first && xop_mergable(p, o));
+        // the delete rows, in row order
+        const u32 delm = __ballot_sync(LB_FULL, kept && o.xk == XK_DEL);
+        for (u32 m = delm; m; m &= m - 1) {
+            const int j = __ffs(m) - 1;
+            XOp d;
+            d.xk = XK_DEL;
+            d.cidx = __shfl_sync(LB_FULL, o.cidx, j);
+            d.ctr = __shfl_sync(LB_FULL, o.ctr, j);
+            d.atoms = __shfl_sync(LB_FULL, o.atoms, j);
+            d.prop = __shfl_sync(LB_FULL, o.prop, j);
+            d.f0 = __shfl_sync(LB_FULL, o.f0, j);
+            d.f1 = __shfl_sync(LB_FULL, o.f1, j);
+            d.f2 = __shfl_sync(LB_FULL, o.f2, j);
+            d.g = 0; d.st0 = 0; d.nst = 1;
+            const bool prev_del = j ? ((delm >> (j - 1)) & 1u) != 0 : c_del;
+            const bool merge = c0 + (u32)j > r_first && prev_del && xop_mergable(back, d);
+            if (merge) xop_merge(back, d);
+            else back = d;
+            if (lane == (u32)j) head = !merge;
+        }
+        c_del = (delm >> 31) & 1u;
+        if (kept) t.r_flag[row] = head ? XF_HEAD : 0;
+        const u32 hm = __ballot_sync(LB_FULL, kept && head);
+        nm += __popc(hm);
+        ndel += __popc(hm & delm);
+        if (hm) last_head = c0 + 31 - __clz(hm);
+        const bool ins = o.xk == XK_LIST || o.xk == XK_TEXT;
+        est_ops += warp_sum_u32(kept && (ins || head) ? xop_estimate(o) : 0);
+    }
+    bad = __any_sync(LB_FULL, bad);
+    skip = warp_sum_u32(skip);   // (one lane at most)
+    __syncwarp();                // the rows' flags are read by the split walk below
+    if (lane) return;
+    const u32 ndeps = t.ch_ndeps[ch] + (t.ch_dep_self[ch] ? 1u : 0u);
+    const u32 est0 = 4 + (ndeps > 1 ? (ndeps - 1) * 4 : 0);
+    u32 nseg = 1, nsyn = 0;
+    t.ch_syn[ch] = 0;   // (xop_from_row below must see the decoded rows)
+    if (trim && est0 + est_ops > LB_MAX_BLOCK_SIZE) {
+        bad = true;   // a trimmed change that also has to be split over several blocks: not covered
+        t.r_flag[r0 + (r_first < nr ? r_first : 0)] |= XF_SEG;
+    } else if (est0 + est_ops > LB_MAX_BLOCK_SIZE) {
+        XSplit sp = split_change(t, di, (u32)ch, r0, nr, est0, [&](u64 row, u32 a, u32, bool, bool seg) {
+            if (seg && a == 0) t.r_flag[row] |= XF_SEG;   // valid when nothing gets cut (else the synthetic rows carry it)
+        });
+        nseg = sp.nseg;
+        if (sp.sliced && nseg > 1) nsyn = sp.nsyn;   // (a lone "slice" that is the whole op changes nothing)
+    } else t.r_flag[r0 + (r_first < nr ? r_first : 0)] |= XF_SEG;
+    t.ch_nseg[ch] = nseg;
+    t.ch_novf[ch] = nseg - 1;
+    t.ch_syn[ch] = nsyn;
+    if (nseg == 1) {   // the common case: the change is its own (only) segment, summarised right here
+        t.sg_src[ch] = (u32)ch; t.sg_r0[ch] = r_first; t.sg_from[ch] = trim; t.sg_atoms[ch] = t.ch_len[ch] - trim; t.sg_est[ch] = est_ops;
+        t.sg_nmops[ch] = nm; t.sg_ndel[ch] = ndel; t.sg_nrows[ch] = nr - r_first; t.sg_last_head[ch] = last_head; t.sg_skip[ch] = skip;
+    }
+    if (bad) atomicOr(&t.xdoc[doc].flags, 1u);
+}
+
+// thread per change, the changes k_exp_changes found to span several segments: synthetic rows, summaries
+__global__ void k_exp_split_changes(DocInfo* __restrict__ docs, u64 n_changes, const __grid_constant__ BatchTables t) {
     u64 ch = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (ch >= n_changes) return;
     if (t.x_req && !t.x_req[t.blocks[t.ch_block[ch]].doc]) return;
-    if (!t.ch_applied[ch]) { if (!pass) { t.ch_nseg[ch] = 0; t.ch_syn[ch] = 0; } return; }
-    u32 doc = t.blocks[t.ch_block[ch]].doc;
-    const DocInfo& di = docs[doc];
+    if (!t.ch_applied[ch] || t.ch_nseg[ch] <= 1) return;
+    const DocInfo& di = docs[t.blocks[t.ch_block[ch]].doc];
     u64 r0 = t.ch_op0[ch];
     u32 nr = t.ch_nops[ch];
     u32 ndeps = t.ch_ndeps[ch] + (t.ch_dep_self[ch] ? 1u : 0u);
     u32 est0 = 4 + (ndeps > 1 ? (ndeps - 1) * 4 : 0);
-    if (pass == 0) {
-        // arena positions of the rows (relative to the document) + RleVec merge inside the change + total estimate
-        u32 vals = (u32)(t.ch_aval0[ch] - t.ch_aval0[di.ch0]), strs = (u32)(t.ch_astr0[ch] - t.ch_astr0[di.ch0]);
-        XOp back;
-        back.xk = XK_NONE;
-        u32 est_ops = 0, nm = 0, ndel = 0, last_head = 0;
-        bool bad = false;
-        // a change whose head the document already had entered the store as a slice (oplog.rs:181-196): rows before the
-        // cut are not part of it, the row under the cut loses its first atoms
-        const u32 trim = t.ch_trim[ch];
-        const i32 cut = t.ch_counter[ch] + (i32)trim;
-        u32 r_first = 0, skip = 0;
-        for (u32 r = 0; r < nr; r++) {
-            u64 row = r0 + r;
-            u32 astart = 0;
-            {   // every decoded insert allocated arena space, kept or not (same rule as k_exp_arena)
-                u8 ctype = t.dcont[di.cid0 + t.op_cidx[row]].type;
-                u8 vt = t.op_vtype[row];
-                if (ctype == CT_TEXT && vt == VK_STR) { astart = strs; strs += t.r_bytes[row]; }
-                else if (ctype == CT_LIST && vt == VK_LORO_VALUE) { astart = vals; vals += t.op_len[row]; }
-            }
-            if (trim && t.op_counter[row] + (i32)t.op_len[row] <= cut) {
-                t.x_rec[row] = mk4(0, 0, 0, 0);
-                t.r_flag[row] = 0;
-                r_first = r + 1;
-                continue;
-            }
-            XOp o = xop_resolve(t, di, (u32)ch, row, astart);
-            t.x_rec[row] = xop_pack(o);
-            if (o.xk == XK_NONE) bad = true;
-            if (r == r_first && trim && t.op_counter[row] < cut) { skip = (u32)(cut - t.op_counter[row]); xop_slice_front(t, o, row, skip); }
-            if (r > r_first && xop_mergable(back, o)) { est_ops -= xop_estimate(back); xop_merge(back, o); est_ops += xop_estimate(back); t.r_flag[row] = 0; }
-            else { back = o; est_ops += xop_estimate(o); t.r_flag[row] = XF_HEAD; nm++; ndel += o.xk == XK_DEL; last_head = r; }
-        }
-        u32 nseg = 1, nsyn = 0;
-        t.ch_syn[ch] = 0;   // (xop_from_row below must see the decoded rows)
-        if (trim && est0 + est_ops > LB_MAX_BLOCK_SIZE) {
-            bad = true;   // a trimmed change that also has to be split over several blocks: not covered
-            t.r_flag[r0 + (r_first < nr ? r_first : 0)] |= XF_SEG;
-        } else if (est0 + est_ops > LB_MAX_BLOCK_SIZE) {
-            XSplit sp = split_change(t, di, (u32)ch, r0, nr, est0, [&](u64 row, u32 a, u32, bool, bool seg) {
-                if (seg && a == 0) t.r_flag[row] |= XF_SEG;   // valid when nothing gets cut (else the synthetic rows carry it)
-            });
-            nseg = sp.nseg;
-            if (sp.sliced && nseg > 1) nsyn = sp.nsyn;   // (a lone "slice" that is the whole op changes nothing)
-        } else t.r_flag[r0 + (r_first < nr ? r_first : 0)] |= XF_SEG;
-        t.ch_nseg[ch] = nseg;
-        t.ch_novf[ch] = nseg - 1;
-        t.ch_syn[ch] = nsyn;
-        if (nseg == 1) {   // the common case: the change is its own (only) segment, summarised right here
-            t.sg_src[ch] = (u32)ch; t.sg_r0[ch] = r_first; t.sg_from[ch] = trim; t.sg_atoms[ch] = t.ch_len[ch] - trim; t.sg_est[ch] = est_ops;
-            t.sg_nmops[ch] = nm; t.sg_ndel[ch] = ndel; t.sg_nrows[ch] = nr - r_first; t.sg_last_head[ch] = last_head; t.sg_skip[ch] = skip;
-        }
-        if (bad) atomicOr(&t.xdoc[doc].flags, 1u);
-        return;
-    }
-    // pass 1 (split changes only)
-    if (t.ch_nseg[ch] <= 1) return;
     u32 nsyn = t.ch_syn[ch];
     if (nsyn) {
         // materialise the synthetic rows: a copy of every untouched row, one row per slice of a cut insert
