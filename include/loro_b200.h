@@ -68,10 +68,18 @@ typedef enum lb_doc_code {
     LB_DOC_ERR_CORRUPT = 4,         /* LoroError::DecodeDataCorruptionError                               */
     LB_DOC_ERR_UNSUPPORTED = 5,     /* well-formed, but outside this path: an intact FastSnapshot blob    */
                                     /* (mode 3, SURVEY 8f.1), or ops the engine does not merge yet        */
-                                    /* (rich-text styles, movable list, counter)                          */
+                                    /* (rich-text styles, movable list, counter), or nesting deeper than  */
+                                    /* LB_MAX_NESTING                                                     */
     LB_DOC_ERR_CAPACITY = 6,        /* internal capacity bound exceeded (engine bug or adversarial input) */
     LB_DOC_ERR_FRONTIERS = 7        /* LoroError::FrontiersNotFound: a checkout id is not in the document  */
 } lb_doc_code;
+
+/* Nesting the engine covers (the reference has no bound).  A document answers LB_DOC_ERR_UNSUPPORTED when one of its
+ * op values nests List / Map values more than LB_MAX_NESTING levels deep (the outermost List or Map counts; decided
+ * at decode, on every path), or when its state nests child containers more than LB_MAX_NESTING levels below a root
+ * container (decided while its state JSON is written, so not under LB_FLAG_NO_JSON).  The two bounds are
+ * independent: a value may nest LB_MAX_NESTING levels inside a container that is itself LB_MAX_NESTING levels deep. */
+#define LB_MAX_NESTING 64
 
 typedef struct lb_blob {
     const uint8_t* ptr; /* host pointer, borrowed */

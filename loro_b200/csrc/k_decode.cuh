@@ -39,8 +39,9 @@ __device__ inline void skip_loro_value_content(Cur& c, u8 kind, u32* n_child_con
         if (flat) { if (n_child_containers) *n_child_containers += kids; return; }
         c = save;          // nested content: start over on the general path
     }
-    // stack of remaining item counts; bit 31 marks a map level (items carry a key index)
-    u32 stack[24];
+    // stack of remaining item counts; bit 31 marks a map level (items carry a key index).  The decoder is the one walker
+    // that meets values deeper than LB_MAX_NESTING: it rejects them, so every later walker's stack of that size fits.
+    u32 stack[LB_MAX_NESTING];
     int sp = 0;
     bool have = true;  // a value of `kind` must be consumed now
     while (true) {
@@ -52,7 +53,8 @@ __device__ inline void skip_loro_value_content(Cur& c, u8 kind, u32* n_child_con
                 case 5: case 6: { u64 n = c.varint(); c.skip(n); break; }
                 case 7: case 8: {
                     u64 n = c.varint();
-                    if (n > (1u << 28) || sp >= 24) { c.err = 1; return; }
+                    if (n > (1u << 28)) { c.err = 1; return; }
+                    if (sp >= LB_MAX_NESTING) { c.err = CUR_ERR_DEEP; return; }
                     stack[sp++] = (u32)n | (kind == 8 ? 0x80000000u : 0);
                     if (kind == 8 && n_maps) (*n_maps)++;
                     break;
@@ -543,8 +545,10 @@ __device__ inline u32 decode_block_rows_cols(const u8* b, const BlockInfo& bi, c
             t.tr_parent_ctr[ti] = (i32)pcn;
             t.tr_pos[ti] = pk == TRP_DELETED ? 0xFFFFFFFFu : (u32)(bi.pos0 + pi);
             aux_idx = (u32)ti;
-        } else
+        } else {
             skip_value(v, vt, &n_maps);
+            if (v.err == CUR_ERR_DEEP) { err = LB_ERR(DOC_ERR_UNSUPPORTED); break; }
+        }
         t.op_val_off[row] = bi.off + (u64)(v0 - b);
         t.op_val_len[row] = (u32)(v.p - v0);
         if (vt == VK_DELETE_SEQ) aux_idx = (u32)(bi.del0 + ndel++);

@@ -26,8 +26,9 @@
 // arenas (arena.rs:237-263): values are adjacent when nothing else was allocated in between (decode order),
 // strings additionally need the append-only buffer not to have been reallocated (capacity doubles from 32;
 // restated from append-only-bytes 0.1.12, same model as the oracle, unpinned by reference tests).
-// Not yet covered (lb_doc_export_updates answers LB_ERR_UNSUPPORTED for the document): values containing nested
-// maps (block-local key indices inside the payload); Tree/MovableList/styles never reach this phase.  Pending changes stay out of the
+// Values containing nested maps carry block-local key indices: xvalue_copy re-registers their keys in the output
+// block.  Documents with MovableList, Counter or style ops are not covered (lb_doc_export_updates answers
+// LB_ERR_UNSUPPORTED for them).  Pending changes stay out of the
 // export but their payloads still count for the arena positions; a document built from several blobs sees them
 // in import_batch's order (the host lays them out that way).
 #pragma once
@@ -1233,9 +1234,11 @@ struct XReg {
 // LoroValues [p, p + n) copied into `s` with the key indices of nested maps translated from the source block's key
 // arena (doc-level key = key_map[src_key0 + idx]) to the output block's register (write_loro_value registers a map's
 // keys as it meets them: encoding/value.rs:1027-1036).
+// The stack holds LB_MAX_NESTING levels, as deep as the decoder admits a value: it never fills, so a value is always
+// copied whole.
 __device__ inline void xvalue_copy(XSink& s, const u8* p, u32 n, const BatchTables& t, u64 src_key0, XReg& keys) {
     Cur c(p, n);
-    u32 stack[24];
+    u32 stack[LB_MAX_NESTING];
     int sp = 0;
     while (!c.err) {
         while (sp > 0 && (stack[sp - 1] & 0x7fffffffu) == 0) sp--;
@@ -1257,7 +1260,7 @@ __device__ inline void xvalue_copy(XSink& s, const u8* p, u32 n, const BatchTabl
             case 7: case 8: {
                 u64 cnt = c.varint();
                 s.varint(cnt);
-                if (sp >= 24 || cnt > (1u << 28)) return;
+                if (sp >= LB_MAX_NESTING || cnt > (1u << 28)) return;
                 stack[sp++] = (u32)cnt | (kind == 8 ? 0x80000000u : 0u);
                 break;
             }

@@ -109,13 +109,14 @@ struct JxWriter {
 
     // a LoroValue at c (kind byte + content), serde_json text (loro-common/src/value.rs:692-711): object keys ascending,
     // the later of two equal keys wins, a container is "🦜:" + its id, which is (peer, ctr) of the atom that created it.
-    // Nested lists and maps go on an explicit stack (the decoder admits 24 levels): the stack a recursive walk needs
+    // Nested lists and maps go on an explicit stack of LB_MAX_NESTING levels, as deep as the decoder admits (so it never
+    // fills, and a value is never cut short): the stack a recursive walk needs
     // cannot be sized at compile time.  A map level prints its keys by selection, O(entries^2) per level, which is cheap
     // for the small nested values documents carry.  k_state.cuh prints the same byte format, but as part of its
     // container frame machine (a child container there is expanded, here it is an id), so the two walkers stay apart.
     struct VLevel { const u8* body; const u8* after; u32 n, left, last; bool map; };
     __device__ void value(Cur& c, const BlockInfo& blk, u32 peer, i32 ctr) {
-        VLevel st[24];
+        VLevel st[LB_MAX_NESTING];
         int sp = 0;
         while (true) {
             const u8 kind = c.get();
@@ -142,7 +143,7 @@ struct JxWriter {
                 }
                 case 7: case 8: {
                     const u32 n = (u32)c.varint();
-                    if (sp == 24) { c.err = 1; break; }
+                    if (sp == LB_MAX_NESTING) { c.err = 1; break; }
                     VLevel& l = st[sp++];
                     l.map = kind == 8; l.n = l.left = n; l.last = JX_NONE; l.body = c.p;
                     if (l.map) for (u32 i = 0; i < n && !c.err; i++) { (void)c.varint(); u8 k = c.get(); skip_loro_value_content(c, k, nullptr); }

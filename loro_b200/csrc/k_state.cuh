@@ -54,6 +54,8 @@ enum { FK_LIST = 1, FK_MAP = 2, FK_VLIST = 3, FK_VMAP = 4, FK_ROOT = 5, FK_TREE 
 struct Frame {
     u8 kind;
     u8 first;      // nothing emitted yet at this level
+    u8 cdepth;     // container levels down to this frame's (FK_ROOT 0, a root container 1; a value frame: its owner's)
+    u8 vdepth;     // value levels down to this frame (0 but for FK_V*)
     u32 a, b, c;   // FK_LIST: cidx, run, elem-in-run ; FK_MAP/FK_ROOT: cidx, last key/root (or NONE) ; FK_V*: remaining
                    // FK_TREE: cidx, slot whose children are being listed, next child index (id_peer: node whose meta
                    // map was just printed, or NONE)
@@ -61,7 +63,8 @@ struct Frame {
     u32 id_peer;   // doc peer idx + counter of the op atom that owns the values being printed
     i32 id_ctr;
 };
-#define MAX_FRAMES 24
+// every frame but the root's adds one container level or one value level, and each kind of level is bounded on its own
+#define MAX_FRAMES (2 * LB_MAX_NESTING + 2)
 
 // per warp: the document's first peers with their ids as decimal text (tree node ids are "<counter>@<peer>": two per node,
 // and formatting a 64-bit peer id costs twenty 64-bit divisions -- done once per peer instead of twice per node)
@@ -166,6 +169,8 @@ struct Emitter {
     }
     // open a container value: scalars-like (text) print directly, list/map push a frame
     __device__ void open_container(u32 cidx, u8 type) {
+        const u8 depth = st[sp - 1].cdepth + 1;
+        if (depth > LB_MAX_NESTING + 1) { err = LB_ERR(DOC_ERR_UNSUPPORTED); return; }
         if (cidx == 0xFFFFFFFFu) {  // never targeted by an op: empty value of its type
             switch (type) {
                 case CT_TEXT: out.puts_("\"\""); break;
@@ -177,6 +182,8 @@ struct Emitter {
         }
         Frame f;
         f.first = 1;
+        f.cdepth = depth;
+        f.vdepth = st[sp - 1].vdepth;
         f.a = cidx;
         f.b = 0;
         f.c = 0;
@@ -409,6 +416,9 @@ struct Emitter {
                 Frame f;
                 f.kind = kind == 7 ? FK_VLIST : FK_VMAP;
                 f.first = 1;
+                f.cdepth = st[sp - 1].cdepth;
+                f.vdepth = st[sp - 1].vdepth + 1;   // the decoder admits no value deeper than LB_MAX_NESTING
+                if (f.vdepth > LB_MAX_NESTING) { err = LB_ERR(DOC_ERR_UNSUPPORTED); return; }
                 f.a = (u32)n;
                 f.b = cur_blk;
                 f.c = 0xFFFFFFFFu;   // FK_VMAP: block-local index of the last key printed
@@ -543,6 +553,8 @@ struct Emitter {
         Frame rf;
         rf.kind = FK_ROOT;
         rf.first = 1;
+        rf.cdepth = 0;
+        rf.vdepth = 0;
         rf.a = 0;
         rf.b = 0xFFFFFFFFu;
         rf.c = 0;

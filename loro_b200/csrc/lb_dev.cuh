@@ -5,6 +5,7 @@
 #pragma once
 #include <stdint.h>
 #include <stddef.h>
+#include "../../include/loro_b200.h"   // LB_MAX_NESTING: the stacks of every LoroValue walker
 
 #ifdef LB_SIMT_EMU
 #include "simt_emu.h"
@@ -65,10 +66,11 @@ enum { OPK_SKIP = 0, OPK_SEQ_INS = 1, OPK_SEQ_DEL = 2, OPK_MAP_SET = 3, OPK_MAP_
 // Bytes are fetched eight at a time (one aligned 64-bit load per 8-byte window, validated by address so that code
 // moving `p` directly stays correct): the decoders are bound by the latency of their byte loads, not by bandwidth.
 // The batch byte buffer is padded, so the aligned window around any in-range byte is readable.
+#define CUR_ERR_DEEP 2u   // Cur::err of a well-formed value that nests deeper than LB_MAX_NESTING (skip_loro_value_content)
 struct Cur {
     const u8* p;
     const u8* end;
-    u32 err;
+    u32 err;          // 0, 1 (malformed or past the end) or CUR_ERR_DEEP
     u64 buf;
     const u8* bp;   // address of the window held in buf (8-byte aligned), nullptr = none
     __device__ __forceinline__ Cur(const u8* b, size_t n) : p(b), end(b + n), err(0), buf(0), bp(nullptr) {}

@@ -273,7 +273,9 @@ class OracleDoc:
             lib().lo_map_set_tagged(self._d, c, k, len(k), self._tagged(v))
             return
         n, kinds, ints, f64s, strs, slens = self._vals([v])
-        lib().lo_map_set(self._d, c, k, len(k), kinds[0], ints[0], f64s[0], strs[0] or b"", slens[0])
+        # the payload itself: reading strs[0] back returns the bytes cut at the first NUL, slens[0] does not
+        payload = v.encode() if isinstance(v, str) else v if isinstance(v, bytes) else b""
+        lib().lo_map_set(self._d, c, k, len(k), kinds[0], ints[0], f64s[0], payload, slens[0])
 
     def map_set_container(self, c, key, ctype):
         ctr = lib().lo_next_counter(self._d)

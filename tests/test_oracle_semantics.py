@@ -346,3 +346,18 @@ def test_string_arena_growth_model_against_golden_blocks(golden_dir):
                 assert ga != gb, (peer, cum)      # the reference left them apart: the model must put them in different buffers
                 seen.add(cum)
         assert seen == cuts, (peer, seen)
+
+
+def test_map_values_with_nul_bytes_read_back_unchanged():
+    """a Str or Binary Map value holding NUL bytes is stored whole (the wrapper passes the payload, not a C string)"""
+    d = OracleDoc(5)
+    m = d.get_map("m")
+    d.map_set(m, "s", "a\x00b\x00")
+    d.map_set(m, "b", b"\x00\xff\x00")
+    d.map_set(m, "z", b"\x00")
+    d.commit()
+    want = {"m": {"s": "a\x00b\x00", "b": [0, 255, 0], "z": [0]}}
+    assert d.get_deep_value() == want
+    e = OracleDoc(6)
+    e.import_(d.export_updates())
+    assert e.get_deep_value() == want
