@@ -4,20 +4,19 @@
 //   get_container_deep_value ; state/{list,map,richtext}_state.rs value extraction ;
 //   crates/loro-common/src/value.rs:692-711 (human-readable serde: I64 integer, Binary array, ...).
 // Object keys are emitted in ascending byte order (the reference's FxHashMap order is unspecified;
-// its own tests compare parsed JSON).  Round-1 shape: one thread per document, two passes over the same
-// emitter (count bytes, then write) with an explicit frame stack instead of recursion.
+// its own tests compare parsed JSON).  One warp per document, two launches of the same emitter (count bytes, then
+// write) with an explicit frame stack instead of recursion: lane 0 walks the document; the lanes share the elements of
+// a scalar-only List or the runs of a Text with 64 runs or more (32 consecutive pieces at a time, staged in shared
+// memory and stored as words) and the nodes of a Tree whose meta maps are empty.
 #pragma once
 #include "lb_tables.cuh"
 #include "k_frame.cuh"
 #include "k_tree.cuh"
 #include "lb_f64.cuh"
 
-struct Sink {
-    u8* dst;   // nullptr = counting pass
-    u64 n;
-    u32 flags; // bit0: value the emitter cannot print exactly (non-integral f64, nested map value)
-    bool wr;   // this lane writes (one warp per document: lane 0 owns the sequential parts)
-    __device__ __forceinline__ void put(u8 c) { if (dst && wr) dst[n] = c; n++; }
+// the text printers of a sink S, which supplies put(u8)
+template <class S> struct PutText {
+    __device__ __forceinline__ void put(u8 c) { static_cast<S*>(this)->put(c); }
     __device__ __forceinline__ void puts_(const char* s) { while (*s) put((u8)*s++); }
     __device__ void put_u64(u64 v) {
         char tmp[24];
@@ -48,6 +47,29 @@ struct Sink {
             }
         }
     }
+};
+
+struct Sink : PutText<Sink> {
+    u8* dst;   // nullptr = counting pass
+    u64 n;
+    u32 flags; // bit0: value the emitter cannot print exactly (non-integral f64, nested map value)
+    bool wr;   // this lane writes (one warp per document: lane 0 owns the sequential parts)
+    __device__ __forceinline__ void put(u8 c) { if (dst && wr) dst[n] = c; n++; }
+};
+
+// Containers with many runs are written 32 pieces at a time (a list element or a text run per lane): each lane prints
+// its piece into its slot, the warp packs the slots in lane order and stores the packed window with aligned words.
+// 32 bytes hold every integer, float, bool and null with its comma, and a short string with its escapes; a longer
+// piece is counted past its slot and written straight from its lane.
+#define JSON_SLOT 32
+struct JsonStage {
+    u8 slot[32][JSON_SLOT + 1];   // odd stride: the lanes' byte stores at the same slot position hit different banks
+    u32 packed[(32 * JSON_SLOT + 4) / 4];   // the window behind up to 3 bytes that put it on the global word grid
+};
+struct SlotSink : PutText<SlotSink> {
+    u8* dst;
+    u32 n;
+    __device__ __forceinline__ void put(u8 c) { if (n < JSON_SLOT) dst[n] = c; n++; }
 };
 
 enum { FK_LIST = 1, FK_MAP = 2, FK_VLIST = 3, FK_VMAP = 4, FK_ROOT = 5, FK_TREE = 6 };
@@ -85,7 +107,9 @@ struct Emitter {
     int lane;
     u32 cur_blk;   // block of the op whose value is being printed (nested map keys are block-local indices)
     TreeEmitSmem* tsm;
-    __device__ Emitter(const BatchTables& t_, const DocInfo& di_, Sink& o, int lane_, TreeEmitSmem* tsm_) : t(t_), di(di_), out(o), sp(0), err(0), lane(lane_), cur_blk(0), tsm(tsm_) {}
+    JsonStage* stg;
+    __device__ Emitter(const BatchTables& t_, const DocInfo& di_, Sink& o, int lane_, TreeEmitSmem* tsm_, JsonStage* stg_)
+        : t(t_), di(di_), out(o), sp(0), err(0), lane(lane_), cur_blk(0), tsm(tsm_), stg(stg_) {}
 
     __device__ int cmp_bytes(const u8* a, u32 al, const u8* b, u32 bl) {
         u32 n = al < bl ? al : bl;
@@ -129,35 +153,34 @@ struct Emitter {
         }
         return s;
     }
-    // text of a Text container: concatenation of the visible runs; with many runs the lanes split them
+    // text of a Text container: concatenation of the visible runs; with many runs, consecutive runs on consecutive lanes
     __device__ __noinline__ void emit_text(u32 cidx) {
         const DocContainer& dc = t.dcont[di.cid0 + cidx];
         out.put('"');
         if (dc.n_out >= 64) {
-            u32 chunk = (dc.n_out + 31) / 32;
-            u32 lo = (u32)lane * chunk, hi = lo + chunk < dc.n_out ? lo + chunk : dc.n_out;
-            if (lo > dc.n_out) lo = dc.n_out;
             Sink cnt;
             cnt.dst = nullptr; cnt.n = 0; cnt.flags = 0; cnt.wr = false;
-            for (u32 r = lo; r < hi; r++) {
-                u64 b0, b1;
-                const u8* s = text_run(dc, r, &b0, &b1);
-                cnt.put_escaped(s + b0, b1 - b0);
-            }
-            u32 mine = (u32)cnt.n;
-            u32 incl = (u32)warp_incl_scan((int)mine, lane);
-            u32 total = __shfl_sync(LB_FULL, incl, 31);
-            if (out.dst) {
-                Sink w;
-                w.dst = out.dst; w.n = out.n + (incl - mine); w.flags = 0; w.wr = true;
-                for (u32 r = lo; r < hi; r++) {
-                    u64 b0, b1;
-                    const u8* s = text_run(dc, r, &b0, &b1);
+            u64 pos = out.n;
+            for (u32 r0 = 0; r0 < dc.n_out; r0 += 32) {
+                const u32 r = r0 + (u32)lane;
+                u64 b0 = 0, b1 = 0;
+                const u8* s = r < dc.n_out ? text_run(dc, r, &b0, &b1) : nullptr;
+                if (out.dst) {
+                    SlotSink w;
+                    w.dst = stg->slot[lane]; w.n = 0;
                     w.put_escaped(s + b0, b1 - b0);
-                }
+                    const u32 incl = (u32)warp_incl_scan((int)w.n, lane), W = __shfl_sync(LB_FULL, incl, 31);
+                    if (store_window(out.dst + pos, w.n, incl - w.n, W)) {
+                        Sink d;
+                        d.dst = out.dst + pos + (incl - w.n); d.n = 0; d.flags = 0; d.wr = true;
+                        d.put_escaped(s + b0, b1 - b0);
+                    }
+                    pos += W;
+                } else cnt.put_escaped(s + b0, b1 - b0);
             }
             __syncwarp();
-            out.n += total;
+            if (out.dst) out.n = pos;
+            else out.n += (u32)warp_sum((int)cnt.n);
         } else {
             for (u32 r = 0; r < dc.n_out; r++) {
                 u64 b0, b1;
@@ -364,7 +387,7 @@ struct Emitter {
         (void)my;
     }
     // print a scalar LoroValue (kinds 0-6) at *pp into `o`; false (nothing consumed) for lists, maps, containers
-    __device__ bool emit_scalar(Sink& o, const u8** pp, const u8* end) {
+    template <class S> __device__ bool emit_scalar(S& o, const u8** pp, const u8* end) {
         Cur c(*pp, (size_t)(end - *pp));
         u8 kind = c.get();
         switch (kind) {
@@ -458,54 +481,103 @@ struct Emitter {
         return c.p;
     }
 
-    // ---- one warp per document: the runs of a scalar-only list are split over the lanes (sizes, scan, write)
+    // write pass of a container written 32 pieces at a time: this lane's piece of n bytes, printed into its slot as far
+    // as it fits, goes to dst + off; the window is the W bytes at dst.  True when the piece outgrew its slot: the lane
+    // then writes it itself.
+    __device__ __noinline__ bool store_window(u8* dst, u32 n, u32 off, u32 W) {
+        const bool big = n > JSON_SLOT;
+        const u8* s = stg->slot[lane];
+        if (__any_sync(LB_FULL, big)) {   // rare: every lane stores its own piece
+            if (!big) for (u32 i = 0; i < n; i++) dst[off + i] = s[i];
+            __syncwarp();
+            return big;
+        }
+        const u32 mis = (u32)((uintptr_t)dst & 3), e = mis + W;
+        u8* pk = (u8*)stg->packed;
+        for (u32 i = 0; i < n; i++) pk[mis + off + i] = s[i];
+        __syncwarp();
+        u8* d0 = dst - mis;   // word aligned: packed word w goes to word w of d0
+        for (u32 w = (u32)lane; 4 * w < e; w += 32) {
+            const u32 lo = 4 * w;
+            if (lo >= mis && lo + 4 <= e) ((u32*)d0)[w] = stg->packed[w];
+            else for (u32 b = lo < mis ? mis : lo; b < lo + 4 && b < e; b++) d0[b] = pk[b];
+        }
+        __syncwarp();
+        return false;
+    }
+
+    // ---- one warp per document: the elements of a scalar-only list, element k of each window of 32 on lane k % 32.
+    // The runs are taken 32 at a time (consecutive runs on consecutive lanes), a warp scan of their lengths gives each
+    // element its run; the count pass sums the printed lengths, the write pass prints every element once into its slot.
     __device__ __noinline__ bool coop_list(u32 cidx) {
         const DocContainer& dc = t.dcont[di.cid0 + cidx];
-        u32 n_out = dc.n_out;
+        const u32 n_out = dc.n_out;
         if (n_out < 64) return false;
-        u32 chunk = (n_out + 31) / 32;
-        u32 lo = (u32)lane * chunk, hi = lo + chunk < n_out ? lo + chunk : n_out;
-        if (lo > n_out) lo = n_out;
+        const u32 err0 = err;   // a lane-local decode error must not leave the lanes in different states
         Sink cnt;
         cnt.dst = nullptr; cnt.n = 0; cnt.flags = 0; cnt.wr = false;
-        bool complex_ = false;
-        u32 elems = 0;
-        u32 err0 = err;   // a lane-local decode error must not leave the lanes in different states
-        for (u32 r = lo; r < hi && !complex_; r++) {
-            u32 row = t.out_row[dc.out0 + r];
-            u32 off = t.out_off[dc.out0 + r], len = t.out_len[dc.out0 + r];
-            const u8* end;
-            const u8* p = list_elem_ptr(row, off, &end);
-            for (u32 e = 0; e < len; e++) {
-                if (!emit_scalar(cnt, &p, end)) { complex_ = true; break; }
-                elems++;
-            }
-        }
-        if (__any_sync(LB_FULL, complex_ || err != err0)) { err = err0; return false; }
-        u32 mine = (u32)cnt.n + elems - (lane == 0 ? 1u : 0u);   // a comma before every element but the first
-        u32 incl = (u32)warp_incl_scan((int)mine, lane);
-        u32 total = __shfl_sync(LB_FULL, incl, 31);
-        u32 flags_all = cnt.flags;
-        for (int d = 16; d > 0; d >>= 1) flags_all |= __shfl_xor_sync(LB_FULL, flags_all, d);
-        out.flags |= flags_all;
-        if (out.dst) {
-            Sink w;
-            w.dst = out.dst; w.n = out.n + (incl - mine); w.flags = 0; w.wr = true;
-            bool first = lane == 0;
-            for (u32 r = lo; r < hi; r++) {
-                u32 row = t.out_row[dc.out0 + r];
-                u32 off = t.out_off[dc.out0 + r], len = t.out_len[dc.out0 + r];
-                const u8* end;
-                const u8* p = list_elem_ptr(row, off, &end);
-                for (u32 e = 0; e < len; e++) {
-                    if (!first) w.put(',');
-                    first = false;
-                    emit_scalar(w, &p, end);
+        u64 pos = out.n;
+        for (u32 r0 = 0; r0 < n_out; r0 += 32) {
+            const u32 r = r0 + (u32)lane;
+            u32 row = 0, off = 0, len = 0;
+            if (r < n_out) { row = t.out_row[dc.out0 + r]; off = t.out_off[dc.out0 + r]; len = t.out_len[dc.out0 + r]; }
+            const u32 incl = (u32)warp_incl_scan((int)len, lane), T = __shfl_sync(LB_FULL, incl, 31);
+            const u8* carry = nullptr;   // where the element after the previous window starts
+            for (u32 k0 = 0; k0 < T; k0 += 32) {
+                const u32 k = k0 + (u32)lane;
+                u32 j = 0;   // runs of the batch that end at or before element k
+#pragma unroll
+                for (u32 s = 16; s; s >>= 1) if (__shfl_sync(LB_FULL, incl, j + s - 1) <= k) j += s;
+                const u32 jrow = __shfl_sync(LB_FULL, row, j), joff = __shfl_sync(LB_FULL, off, j);
+                const u32 jstart = __shfl_sync(LB_FULL, incl - len, j);
+                const u8* p = nullptr;
+                const u8* el = nullptr;
+                const u8* end = nullptr;
+                const bool comma = r0 + k != 0;   // a comma before every element but the first
+                bool ok = true;
+                SlotSink w;
+                w.dst = stg->slot[lane]; w.n = 0;
+                if (k < T) {
+                    end = t.bytes + t.op_val_off[jrow] + t.op_val_len[jrow];
+                    u32 from = k0;   // a run that goes on from the previous window goes on from that window's cursor
+                    if (jstart < k0) p = carry;
+                    else { p = list_elem_ptr(jrow, joff, &end); from = jstart; }
+                    Cur c(p, (size_t)(end - p));
+                    for (u32 i = from; i < k && !c.err; i++) {
+                        u8 kind = c.get();
+                        skip_loro_value_content(c, kind, nullptr);
+                    }
+                    el = p = c.p;
+                    if (out.dst) {
+                        if (comma) w.put(',');
+                        ok = emit_scalar(w, &p, end);
+                    } else {
+                        if (comma) cnt.put(',');
+                        ok = emit_scalar(cnt, &p, end);
+                    }
+                }
+                // a nested value: the sequential walk prints the container (over what earlier windows wrote, the same bytes)
+                if (__any_sync(LB_FULL, !ok || err != err0)) { err = err0; return false; }
+                carry = (const u8*)__shfl_sync(LB_FULL, (unsigned long long)p, 31);
+                if (out.dst) {
+                    const u32 n = k < T ? w.n : 0u;
+                    const u32 wincl = (u32)warp_incl_scan((int)n, lane), W = __shfl_sync(LB_FULL, wincl, 31);
+                    if (store_window(out.dst + pos, n, wincl - n, W)) {
+                        Sink d;
+                        d.dst = out.dst + pos + (wincl - n); d.n = 0; d.flags = 0; d.wr = true;
+                        if (comma) d.put(',');
+                        emit_scalar(d, &el, end);
+                    }
+                    pos += W;
                 }
             }
         }
+        u32 flags_all = cnt.flags;
+        for (int d = 16; d > 0; d >>= 1) flags_all |= __shfl_xor_sync(LB_FULL, flags_all, d);
+        out.flags |= flags_all;
         __syncwarp();
-        out.n += total;
+        if (out.dst) out.n = pos;
+        else out.n += (u32)warp_sum((int)cnt.n);
         return true;
     }
 
@@ -680,6 +752,7 @@ struct Emitter {
 // pass = 0: count bytes into docs[d].json_len ; pass = 1: write at docs[d].json_off
 __global__ void __launch_bounds__(128, 8) k_json(DocInfo* __restrict__ docs, u32 n_docs, const __grid_constant__ BatchTables t, u8* __restrict__ json, int pass) {
     __shared__ TreeEmitSmem tsm[4];   // 128 threads: one entry per warp
+    __shared__ JsonStage stg[4];
     u32 d = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // one warp per document
     int lane = threadIdx.x & 31;
     if (d >= n_docs) return;
@@ -690,7 +763,7 @@ __global__ void __launch_bounds__(128, 8) k_json(DocInfo* __restrict__ docs, u32
     s.n = 0;
     s.flags = 0;
     s.wr = lane == 0;
-    Emitter e(t, di, s, lane, &tsm[(threadIdx.x >> 5) & 3]);
+    Emitter e(t, di, s, lane, &tsm[(threadIdx.x >> 5) & 3], &stg[(threadIdx.x >> 5) & 3]);
     e.run();
     __syncwarp();
     if (!pass && lane == 0) {
