@@ -31,3 +31,25 @@ def check_batch_against_oracle(blobs, lib_path=None, expect_json=None):
         assert st.success == ost["success"], (i, st.success, ost["success"])
         assert st.pending == ost["pending"], (i, st.pending, ost["pending"])
     return batch
+
+
+def check_c5_documents_of_atoms(atoms, lib_path=None):
+    """One batch of config C5 tree documents, document k of atoms[k] atom ops (n_nodes creates + 3 peers x n_moves
+    moves, n_moves = 1,000 or a sixth of the atoms): JSON against the generator's own merge and the oracle, re-exported bytes against the oracle's.  The
+    largest document decides whether the tree apply keeps its parent links in shared memory (up to
+    TREE_S_NODES_MAX = 32,768 atoms, 16-bit links next to the 0xFFFD..0xFFFF sentinels) or, for the documents past
+    it, in global memory while the others of the launch keep theirs in shared memory."""
+    from loro_b200.workload import C5Batch
+    from .export_checks import check_export_against_oracle
+    blobs, want = [], []
+    for k, a in enumerate(atoms):
+        n_moves = min(1000, a // 6)
+        g = C5Batch(1, n_nodes=a - 3 * n_moves, n_moves=n_moves, first_doc=k, want_json=True)
+        assert g.atom_ops == a, (k, g.atom_ops, a)
+        blobs.append(g.blob(0))
+        want.append(g.expected_json(0))
+        g.close()
+    batch = check_batch_against_oracle(blobs, lib_path=lib_path, expect_json=want)
+    assert batch.counters()["atom_ops"] == sum(atoms)
+    check_export_against_oracle(blobs, lib_path=lib_path, reimport=False)
+    return batch

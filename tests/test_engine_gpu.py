@@ -322,6 +322,20 @@ def test_config_c5_full_size_documents():
     check_export_against_oracle(blobs[:4])
 
 
+
+def test_tree_links_in_shared_memory_at_their_limit():
+    """The largest tree document has exactly TREE_S_NODES_MAX = 32,768 atoms: shared-memory links at their limit
+    (the same documents as test_tree_emu.py)."""
+    from tests.engine_checks import check_c5_documents_of_atoms
+    check_c5_documents_of_atoms([32768, 760])
+
+
+def test_tree_links_in_global_memory_past_the_limit():
+    """32,769- and 36,000-atom documents take global-memory links beside a 32,768-atom and a small document that use
+    64 KB of shared memory per CTA in the same launch (the same documents as test_tree_emu.py)."""
+    from tests.engine_checks import check_c5_documents_of_atoms
+    check_c5_documents_of_atoms([32769, 760, 36000, 32768])
+
 def test_export_from_version_vector_and_c1_end_to_end():
     """lb_doc_export_updates(from): export(ExportMode::updates(vv)) on the CUDA path, byte-equal to the oracle; config C1
     (A exports updates(vv_B), B imports) driven by the engine."""

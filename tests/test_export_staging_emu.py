@@ -1,22 +1,16 @@
-"""Phase 7 (re-export) on the emulated kernels with staging slots smaller than the blocks need.
-
-The encoder writes each output block once, into a staging slot sized from the block's rows and store estimate, and
-the blobs are assembled from the slots.  A block that outgrows its slot is encoded again by the same code, into a
-retry slot of its exact size.  LB_EXPORT_STAGE_CAP caps every first slot's capacity (in bytes): 0 sends every block
-through the retry, a small cap only the larger blocks.  Either way the bytes must stay the oracle's."""
-import gzip
+"""Phase 7 (re-export) on the emulated kernels with staging slots smaller than the blocks need: the cases of
+tests/export_staging_checks.py, whose bytes must stay the oracle's whether a block fits its slot or goes through the
+retry.  The same cases run on the CUDA build in test_export_staging_gpu.py."""
 import os
-import re
 import subprocess
 
 import pytest
 
-from tests import workloads
-from tests.export_checks import check_export_against_oracle, check_export_from_versions
+from tests import export_staging_checks as sc
+from tests.export_staging_checks import stage_cap  # noqa: F401 -- the fixture
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 EMU = os.path.join(HERE, "emu", "libloro_b200_emu.so")
-TRACE = re.compile(r"\[trace\] export: (\d+) blocks, (\d+) outgrew their staging slot")
 
 
 @pytest.fixture(scope="session", autouse=True)
@@ -24,71 +18,23 @@ def build_emu():
     subprocess.check_call([os.path.join(HERE, "emu", "build_emu.sh")])
 
 
-@pytest.fixture
-def stage_cap(monkeypatch, capfd):
-    """Sets the slot cap; returns a function giving (blocks, blocks that outgrew their slot) over the exports so far."""
-    monkeypatch.setenv("LB_PHASE_TRACE", "1")
-
-    def setcap(cap):
-        monkeypatch.setenv("LB_EXPORT_STAGE_CAP", str(cap))
-
-    def counts():
-        err = capfd.readouterr().err
-        m = TRACE.findall(err)
-        assert m, "no export trace line"
-        return sum(int(a) for a, _ in m), sum(int(b) for _, b in m)
-    return setcap, counts
-
-
-def random_histories(seed):
-    return [workloads.make_doc_history(seed * 100 + i, n_sites=2 + i % 4, n_ops=200 + 40 * i, sync_prob=0.03 + 0.02 * (i % 3))[0]
-            for i in range(6)]
-
-
 @pytest.mark.parametrize("seed", [21, 22])
 def test_every_block_outgrows_its_slot_random_histories(stage_cap, seed):
-    setcap, counts = stage_cap
-    setcap(0)
-    check_export_against_oracle(random_histories(seed), lib_path=EMU)
-    blocks, ovf = counts()
-    assert blocks > 0 and ovf == blocks
+    sc.every_block_outgrows_random_histories(stage_cap, seed, lib_path=EMU)
 
 
 def test_some_blocks_outgrow_their_slot_random_histories(stage_cap):
-    setcap, counts = stage_cap
-    setcap(1000)
-    check_export_against_oracle(random_histories(23), lib_path=EMU)
-    blocks, ovf = counts()
-    assert 0 < ovf < blocks, (blocks, ovf)
+    sc.some_blocks_outgrow_random_histories(stage_cap, lib_path=EMU)
 
 
 def test_every_block_outgrows_its_slot_generator_documents(stage_cap):
-    from loro_b200.workload import C3Batch
-    setcap, counts = stage_cap
-    setcap(0)
-    check_export_against_oracle(C3Batch(4, n_ops=2500, threads=4).blobs(), lib_path=EMU)
-    blocks, ovf = counts()
-    assert blocks > 0 and ovf == blocks
+    sc.every_block_outgrows_generator_documents(stage_cap, lib_path=EMU)
 
 
 def test_every_block_outgrows_its_slot_split_changes_and_trace(stage_cap, golden_dir):
-    from loro_b200.workload import C3Batch
-    setcap, counts = stage_cap
-    setcap(0)
-    blobs = C3Batch(2, n_ops=10000, threads=2).blobs()
-    blobs.append(gzip.open(os.path.join(golden_dir, "automerge_trace_blob.bin.gz"), "rb").read())
-    check_export_against_oracle(blobs, lib_path=EMU, reimport=False)
-    blocks, ovf = counts()
-    assert blocks > 0 and ovf == blocks
+    sc.every_block_outgrows_split_changes_and_trace(stage_cap, golden_dir, lib_path=EMU)
 
 
 @pytest.mark.parametrize("cap", [0, 1000])
 def test_slot_overflow_export_from_version_vector(stage_cap, cap):
-    setcap, counts = stage_cap
-    setcap(cap)
-    check_export_from_versions(workloads.make_doc_history(7220, n_sites=3, n_ops=260)[0], lib_path=EMU, seed=1)
-    blocks, ovf = counts()
-    if cap == 0:
-        assert blocks > 0 and ovf == blocks
-    else:
-        assert 0 < ovf < blocks, (blocks, ovf)
+    sc.slot_overflow_export_from_version_vector(stage_cap, cap, lib_path=EMU)

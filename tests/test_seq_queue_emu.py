@@ -6,7 +6,6 @@ import subprocess
 
 import pytest
 
-from oracle import OracleDoc
 from tests import workloads
 from tests.engine_checks import check_batch_against_oracle
 from tests.export_checks import check_export_against_oracle
@@ -18,28 +17,6 @@ EMU = os.path.join(HERE, "emu", "libloro_b200_emu.so")
 @pytest.fixture(scope="session", autouse=True)
 def build_emu():
     subprocess.check_call([os.path.join(HERE, "emu", "build_emu.sh")])
-
-
-def _pending_only():
-    """A document whose one change depends on a change the blob does not carry: nothing of it is applied."""
-    a = OracleDoc(5)
-    a.text_insert(a.get_text("t"), 0, "abc")
-    a.commit()
-    vv = a.oplog_vv()
-    a.text_insert(a.get_text("t"), 3, "def")
-    return a.export_updates(vv)
-
-
-def _map_only():
-    a = OracleDoc(6)
-    m = a.get_map("map")
-    a.map_set(m, "k", 1)
-    a.map_set(m, "s", "v")
-    return a.export_updates()
-
-
-def _bad_checksum(blob):
-    return blob[:30] + bytes([blob[30] ^ 1]) + blob[31:]
 
 
 def _healthy():
@@ -54,7 +31,7 @@ def _healthy():
 
 def test_one_warp_many_documents():
     healthy = _healthy()
-    skipped = [_bad_checksum(healthy[0]), _pending_only(), _map_only(), OracleDoc(8).export_updates()]
+    skipped = workloads.skipped_kinds(healthy[0])
     blobs = []
     for i, h in enumerate(healthy):   # every skipped document sits right before a healthy one
         blobs.append(skipped[i % len(skipped)])

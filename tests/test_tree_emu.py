@@ -160,3 +160,17 @@ def test_tree_long_sibling_list_with_equal_positions():
                     workloads.merge(docs[i], docs[j])
     b = check_batch_against_oracle([docs[0].export_updates()], lib_path=EMU)
     assert len(b.get_deep_value(0)["t"][0]["children"]) == 60
+
+
+def test_tree_links_in_shared_memory_at_their_limit():
+    """The largest document has exactly TREE_S_NODES_MAX = 32,768 atoms: every document of the launch keeps its
+    16-bit parent links in shared memory, with links up to 32,767 next to the 0xFFFD..0xFFFF sentinels."""
+    from tests.engine_checks import check_c5_documents_of_atoms
+    check_c5_documents_of_atoms([32768, 760], lib_path=EMU)
+
+
+def test_tree_links_in_global_memory_past_the_limit():
+    """Documents of 32,769 and 36,000 atoms keep their parent links in global memory, while a 32,768-atom and a
+    small document of the same launch use 64 KB of shared memory per CTA."""
+    from tests.engine_checks import check_c5_documents_of_atoms
+    check_c5_documents_of_atoms([32769, 760, 36000, 32768], lib_path=EMU)

@@ -233,3 +233,31 @@ def import_batch_order(blobs):
     def n_changes(blob):
         return sum(len(bl["changes"]) for bl in oracle.decode_dump(blob)["blocks"])
     return sorted(blobs, key=lambda x: -n_changes(x))
+
+
+def pending_only_blob():
+    """A document whose one change depends on a change the blob does not carry: nothing of it is applied."""
+    a = OracleDoc(5)
+    a.text_insert(a.get_text("t"), 0, "abc")
+    a.commit()
+    vv = a.oplog_vv()
+    a.text_insert(a.get_text("t"), 3, "def")
+    return a.export_updates(vv)
+
+
+def map_only_blob():
+    a = OracleDoc(6)
+    m = a.get_map("map")
+    a.map_set(m, "k", 1)
+    a.map_set(m, "s", "v")
+    return a.export_updates()
+
+
+def bad_checksum(blob):
+    return blob[:30] + bytes([blob[30] ^ 1]) + blob[31:]
+
+
+def skipped_kinds(blob):
+    """documents the list integration kernel skips: `blob` with a bad checksum, a pending-only, a map-only and an empty
+    document"""
+    return [bad_checksum(blob), pending_only_blob(), map_only_blob(), OracleDoc(8).export_updates()]
