@@ -37,7 +37,7 @@ int main(int argc, char** argv) {
     if (argc < 2) { fprintf(stderr, "usage: %s update.bin [more updates of the same document ...]\n", argv[0]); return 2; }
     lb_options opt;
     memset(&opt, 0, sizeof(opt));
-    opt.flags = LB_FLAG_EXPORT;
+    opt.flags = LB_FLAG_EXPORT | LB_FLAG_CURSORS;
     /* 1. LoroDoc::import_batch into a fresh document: every blob carries the same doc_id */
     size_t n = (size_t)argc - 1;
     lb_blob* blobs = (lb_blob*)calloc(n, sizeof(lb_blob));
@@ -50,6 +50,18 @@ int main(int argc, char** argv) {
     lb_status rc = lb_import_batch(blobs, n, &opt, &b);
     if (rc != LB_OK) { fprintf(stderr, "lb_import_batch: %d (%s)\n", (int)rc, lb_last_error()); return 1; }
     print_doc(b, 0);
+    /* LoroDoc::get_cursor_pos: a cursor at the end of the root Text "text" (no id, Side::Right) lies at its length */
+    lb_cursor cur;
+    memset(&cur, 0, sizeof(cur));
+    cur.doc = 0;
+    cur.name = (const uint8_t*)"text";
+    cur.name_len = 4;
+    cur.is_root = 1;
+    cur.type = 2;   /* Text */
+    cur.side = 1;
+    lb_cursor_result res;
+    if (lb_batch_cursor_pos(b, &cur, 1, &res) != LB_OK) { fprintf(stderr, "lb_batch_cursor_pos: %s\n", lb_last_error()); return 1; }
+    printf("  cursor at the end of text: status %d, pos %llu\n", (int)res.status, (unsigned long long)res.pos);
     lb_batch_free(b);
     /* 2. the same updates one call at a time against a document that lives in device memory between the calls */
     lb_docset* set = NULL;

@@ -31,6 +31,8 @@
  *   lb_doc_attribution       who wrote the state, for the whole document: crates/loro/src/lib.rs:2644
  *                            LoroText::get_editor_at_unicode_pos, :1906 LoroList::get_id_at, :2117 LoroMap::get_last_editor,
  *                            :3046 LoroTree::get_last_move_id
+ *   lb_batch_cursor_pos      crates/loro-internal/src/loro.rs:1560-1737 LoroDoc::get_cursor_pos(&Cursor) (query_pos): where
+ *                            an anchored element of a Text / List lies now, for many cursors in one call
  *
  * Conventions (mirroring the reference): input buffers are borrowed for the duration of the call only;
  * outputs are owned by the batch handle until lb_batch_free; a bad blob never aborts the batch -- it yields a
@@ -98,6 +100,7 @@ typedef struct lb_options {
 #define LB_FLAG_EXPORT 4u       /* also re-export every document (phase 7) for lb_doc_export_updates */
 #define LB_FLAG_COMPACT 8u      /* lb_docset_import: afterwards keep each touched document as its own export (see below) */
 #define LB_FLAG_ATTRIBUTION 16u /* also compute each document's attribution (phase 6b) for lb_doc_attribution */
+#define LB_FLAG_CURSORS 32u     /* also keep each Text / List container's element order (after phase 5) for lb_batch_cursor_pos */
 
 typedef struct lb_id_span {
     uint64_t peer;
@@ -146,6 +149,7 @@ typedef struct lb_timings { /* device time per phase in milliseconds (CUDA event
      * download, status tables) -- what a step costs beyond `total_device` */
     float host_call_ms, host_tail_ms;
     float attribution;                 /* attribution phase (LB_FLAG_ATTRIBUTION; 0 without it) */
+    float cursors;                     /* import-time part of the cursor phase (LB_FLAG_CURSORS; 0 without it) */
 } lb_timings;
 
 typedef struct lb_batch lb_batch;
@@ -180,6 +184,64 @@ lb_status lb_doc_vv(const lb_batch* b, size_t doc, const lb_id_span** spans, siz
  * LB_FLAG_NO_JSON and LB_FLAG_EXPORT), otherwise LB_ERR_INVALID_ARG.  A document that failed to import (any code but
  * LB_DOC_OK) gives an empty string.  The bytes are owned by the batch. */
 lb_status lb_doc_attribution(const lb_batch* b, size_t doc, const char** utf8, size_t* len);
+/* ---- cursors ----------------------------------------------------------------------------------------------------------
+ * LoroDoc::get_cursor_pos(&Cursor) (crates/loro-internal/src/loro.rs:1560-1737 query_pos): a Cursor anchors a place of a
+ * Text or List to the element with id `id` (comments, highlights, selections, carets); the query says where that element
+ * lies now.  Request i is answered in out[i]:
+ *   a visible target            pos = its index (Text: unicode scalar values), side = the request's side, no update
+ *                               (state.rs:1403-1433);
+ *   a deleted target            pos = the visible elements before it in document order, side = Left (tracker.rs:588-619),
+ *                               and an update cursor, get_cursor(pos, Left) on the current state (handler.rs:2337-2390,
+ *                               :2912-2952): {no id, Left, 0} in an empty container, {no id, Right, len} when pos >= len,
+ *                               otherwise {id of the visible element at pos, Left, pos};
+ *   no id (has_id = 0)          pos = 0 for Left, the container's length otherwise; side = the request's side, no update;
+ *   LB_CURSOR_ID_NOT_FOUND      the target was never an element of this container (another container's, a delete op's,
+ *                               an id the document lacks), or a normal container the document does not have.  A root
+ *                               container always exists (loro.rs:889-896): one that no op touches is empty;
+ *   LB_CURSOR_CONTAINER_DELETED CannotFindRelativePosition::ContainerDeleted, kept for the mapping: the reference raises it
+ *                               only for a container has_container already refused, so it is never returned;
+ *   LB_ERR_INVALID_ARG          the document failed to import, or the container is not a Text or List (the reference
+ *                               reaches unreachable!() for Map, Tree, Counter and MovableList), or side is not -1/0/1;
+ *   LB_ERR_UNSUPPORTED          the document has code LB_DOC_ERR_UNSUPPORTED.
+ * Needs LB_FLAG_CURSORS at import; lb_import_batch, lb_import_batch_device, lb_docset_import and lb_docset_read accept it.
+ * lb_import_batch_at and lb_docset_checkout refuse it with LB_ERR_INVALID_ARG: on a checked-out document the reference
+ * answers a visible id from the state at the checkout's version but a deleted one from the latest oplog, a mix that would
+ * need both versions' orders.  The flag keeps, until lb_batch_free, one table of every span of every Text / List rope in
+ * document order and one by id; without it nothing is allocated or launched.  One call uploads the requests once,
+ * launches one kernel and downloads the answers once, whatever their number or documents.  The whole call fails with
+ * LB_ERR_INVALID_ARG, launching nothing, for a `doc` out of range, a null pointer with a count above 0 (reqs, out, a root
+ * name), or a batch imported without LB_FLAG_CURSORS; n = 0 does nothing.  Calls on one batch run one at a time. */
+#define LB_CURSOR_ID_NOT_FOUND 100       /* CannotFindRelativePosition::IdNotFound */
+#define LB_CURSOR_CONTAINER_DELETED 101  /* CannotFindRelativePosition::ContainerDeleted */
+typedef struct lb_cursor {
+    size_t doc;                 /* document index in the batch */
+    /* the container: root (name bytes, type) when is_root, else normal (peer, counter, type); type as the reference
+     * encodes ContainerType: 0 Map, 1 List, 2 Text, 3 Tree, 4 MovableList, 5 Counter */
+    const uint8_t* name;        /* root: name bytes, borrowed for the call */
+    size_t name_len;
+    uint64_t peer;              /* normal: the id of the op that created it */
+    int32_t counter;
+    uint8_t is_root;
+    uint8_t type;
+    uint8_t has_id;             /* Cursor.id is Some: the target id (id_peer, id_counter) */
+    int8_t side;                /* Side: -1 Left, 0 Middle, 1 Right */
+    uint64_t id_peer;
+    int32_t id_counter;
+} lb_cursor;
+typedef struct lb_cursor_result {
+    int32_t status;             /* LB_OK, LB_CURSOR_ID_NOT_FOUND, LB_CURSOR_CONTAINER_DELETED, LB_ERR_INVALID_ARG,
+                                   LB_ERR_UNSUPPORTED */
+    int8_t side;                /* AbsolutePosition.side */
+    uint8_t has_update;         /* PosQueryResult.update is Some: */
+    uint8_t update_has_id;      /*   its id (update_peer, update_counter) is Some */
+    int8_t update_side;
+    uint64_t pos;               /* AbsolutePosition.pos */
+    uint64_t update_peer;
+    int32_t update_counter;
+    uint32_t reserved;
+    uint64_t update_origin_pos;
+} lb_cursor_result;
+lb_status lb_batch_cursor_pos(const lb_batch* b, const lb_cursor* reqs, size_t n, lb_cursor_result* out);
 /* LoroDoc::oplog_frontiers() (crates/loro/src/lib.rs:881; version/frontiers.rs:233-246): the heads of the causal graph,
  * one span [counter, counter + 1) per head id. */
 lb_status lb_doc_frontiers(const lb_batch* b, size_t doc, const lb_id_span** spans, size_t* n);

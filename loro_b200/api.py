@@ -12,6 +12,10 @@ LB_FLAG_KEEP_DEVICE = 2
 LB_FLAG_EXPORT = 4
 LB_FLAG_COMPACT = 8
 LB_FLAG_ATTRIBUTION = 16
+LB_FLAG_CURSORS = 32
+LB_CURSOR_ID_NOT_FOUND = 100        # CannotFindRelativePosition::IdNotFound
+LB_CURSOR_CONTAINER_DELETED = 101   # CannotFindRelativePosition::ContainerDeleted
+CONTAINER_TYPES = {"Map": 0, "List": 1, "Text": 2, "Tree": 3, "MovableList": 4, "Counter": 5}
 
 DOC_CODES = {0: "Ok", 1: "DecodeError", 2: "DecodeChecksumMismatchError", 3: "IncompatibleFutureEncodingError",
              4: "DecodeDataCorruptionError", 5: "Unsupported", 6: "CapacityExceeded", 7: "FrontiersNotFound"}
@@ -61,6 +65,34 @@ class _JsonRequest(ctypes.Structure):
 LB_JSON_NO_PEER_COMPRESSION = 1
 
 
+class _Cursor(ctypes.Structure):
+    _fields_ = [("doc", ctypes.c_size_t), ("name", ctypes.c_char_p), ("name_len", ctypes.c_size_t),
+                ("peer", ctypes.c_uint64), ("counter", ctypes.c_int32), ("is_root", ctypes.c_uint8),
+                ("type", ctypes.c_uint8), ("has_id", ctypes.c_uint8), ("side", ctypes.c_int8),
+                ("id_peer", ctypes.c_uint64), ("id_counter", ctypes.c_int32)]
+
+
+class _CursorResult(ctypes.Structure):
+    _fields_ = [("status", ctypes.c_int32), ("side", ctypes.c_int8), ("has_update", ctypes.c_uint8),
+                ("update_has_id", ctypes.c_uint8), ("update_side", ctypes.c_int8), ("pos", ctypes.c_uint64),
+                ("update_peer", ctypes.c_uint64), ("update_counter", ctypes.c_int32), ("reserved", ctypes.c_uint32),
+                ("update_origin_pos", ctypes.c_uint64)]
+
+
+def parse_container_id(cid):
+    """ContainerID's display form ("cid:root-<name>:<Type>" or "cid:<counter>@<peer>:<Type>", as Batch.attribution
+    lists containers) -> (is_root, name bytes or None, peer, counter, type code)"""
+    if not cid.startswith("cid:") or ":" not in cid[4:]:
+        raise ValueError(f"not a container id: {cid!r}")
+    body, tname = cid[4:].rsplit(":", 1)
+    if tname not in CONTAINER_TYPES:
+        raise ValueError(f"unknown container type in {cid!r}")
+    if body.startswith("root-"):
+        return True, body[5:].encode(), 0, 0, CONTAINER_TYPES[tname]
+    counter, peer = body.split("@")
+    return False, None, int(peer), int(counter), CONTAINER_TYPES[tname]
+
+
 class _Status(ctypes.Structure):
     _fields_ = [("code", ctypes.c_int), ("n_success", ctypes.c_size_t), ("success", ctypes.POINTER(_IdSpan)),
                 ("n_pending", ctypes.c_size_t), ("pending", ctypes.POINTER(_IdSpan))]
@@ -80,7 +112,8 @@ class _Timings(ctypes.Structure):
                 ("decode_fast_blocks", ctypes.c_uint64), ("decode_lane_blocks", ctypes.c_uint64),
                 ("decode_unstaged_blocks", ctypes.c_uint64),
                 ("alloc_host_ms", ctypes.c_float), ("reserved1", ctypes.c_uint32), ("device_bytes", ctypes.c_uint64),
-                ("host_call_ms", ctypes.c_float), ("host_tail_ms", ctypes.c_float), ("attribution", ctypes.c_float)]
+                ("host_call_ms", ctypes.c_float), ("host_tail_ms", ctypes.c_float), ("attribution", ctypes.c_float),
+                ("cursors", ctypes.c_float)]
 
 
 _libs = {}
@@ -108,6 +141,7 @@ def load_library(path=None):
     L.lb_doc_status.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(_Status)]
     L.lb_doc_json.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_size_t)]
     L.lb_doc_attribution.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_size_t)]
+    L.lb_batch_cursor_pos.argtypes = [vp, ctypes.POINTER(_Cursor), ctypes.c_size_t, ctypes.POINTER(_CursorResult)]
     L.lb_doc_export_updates.argtypes = [vp, ctypes.c_size_t, ctypes.POINTER(_IdSpan), ctypes.c_size_t,
                                         ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_size_t)]
     L.lb_batch_export_updates.argtypes = [vp, ctypes.POINTER(_ExportRequest), ctypes.c_size_t, ctypes.POINTER(vp)]
@@ -337,6 +371,37 @@ class Batch:
                 out[cid] = {k: (peers[p], c, bool(f)) for k, (p, c, f) in entry.items()}
         return out
 
+    def cursor_pos(self, cursors):
+        """LoroDoc::get_cursor_pos for many cursors in one call (lb_batch_cursor_pos; needs flags=LB_FLAG_CURSORS at
+        import).  cursors: [(doc, container, id, side), ...] with container a ContainerID display string
+        ("cid:root-text:Text", "cid:3@7:List"), id (peer, counter) or None, side -1 / 0 / 1.  Returns one
+        (status, pos, side, update) per cursor: status 0 or LB_CURSOR_* or an lb_status; update None or
+        (id or None, side, origin_pos)."""
+        cursors = list(cursors)
+        n = len(cursors)
+        arr = (_Cursor * max(n, 1))()
+        keep = []
+        for k, (doc, cid, tid, side) in enumerate(cursors):
+            is_root, name, peer, counter, ctype = parse_container_id(cid)
+            c = arr[k]
+            c.doc, c.is_root, c.type, c.side = doc, is_root, ctype, side
+            if is_root:
+                keep.append(name)
+                c.name, c.name_len = name, len(name)
+            else:
+                c.peer, c.counter = peer, counter
+            if tid is not None:
+                c.has_id, c.id_peer, c.id_counter = 1, tid[0], tid[1]
+        res = (_CursorResult * max(n, 1))()
+        _check(self._L, self._L.lb_batch_cursor_pos(self._h, arr, n, res), "lb_batch_cursor_pos")
+        out = []
+        for r in res[:n]:
+            upd = None
+            if r.has_update:
+                upd = ((r.update_peer, r.update_counter) if r.update_has_id else None, r.update_side, r.update_origin_pos)
+            out.append((r.status, r.pos, r.side, upd))
+        return out
+
     def fetch_json(self):
         """make sure the JSON of every document of the batch is in host memory (one download of the whole buffer)"""
         if self.n_docs:
@@ -435,6 +500,10 @@ class MultiBatch:
     def export_updates_many(self, requests):
         """Batch.export_updates_many with every request sent to its sub-batch: one C call per sub-batch."""
         return self._many("export_updates_many", requests)
+
+    def cursor_pos(self, cursors):
+        """Batch.cursor_pos with every cursor sent to its sub-batch: one C call per sub-batch, answers in request order"""
+        return self._many("cursor_pos", cursors)
 
     def export_updates_in_range(self, i, spans): p, j = self._loc(i); return p.export_updates_in_range(j, spans)
     def export_updates_till(self, i, vv): p, j = self._loc(i); return p.export_updates_till(j, vv)

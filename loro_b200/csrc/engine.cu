@@ -32,6 +32,7 @@
 #include "k_export.cuh"
 #include "k_json_updates.cuh"
 #include "k_attr.cuh"
+#include "k_cursor.cuh"
 #include "host_stage.hpp"
 
 static thread_local std::string g_last_error;
@@ -318,7 +319,7 @@ struct Dev {  // owns every device allocation of a batch
 
 // Events on the batch stream, in pipeline order: EV_x is recorded when phase x has been enqueued (mark), and a phase's
 // device time is the interval from the event before it (timings_from_events).
-enum BatchEvent { EV_START, EV_H2D, EV_FRAME, EV_DECODE, EV_RESOLVE, EV_CLASSIFY, EV_INTEGRATE, EV_TREE, EV_MATERIALISE,
+enum BatchEvent { EV_START, EV_H2D, EV_FRAME, EV_DECODE, EV_RESOLVE, EV_CLASSIFY, EV_INTEGRATE, EV_CURSORS, EV_TREE, EV_MATERIALISE,
                   EV_ATTRIBUTION, EV_EXPORT, EV_D2H, EV_COUNT };
 
 struct lb_batch {
@@ -350,6 +351,8 @@ struct lb_batch {
     char* attr = nullptr;
     std::vector<u64> attr_off;
     bool attr_fetched = false;
+    // LB_FLAG_CURSORS (k_cursor.cuh): every Text / List rope in document order and by id, for lb_batch_cursor_pos
+    CursorTables cur{};
     u64 export_total = 0;
     std::vector<XDoc> xdocs;
     std::unordered_map<size_t, std::vector<uint8_t>> from_exports;   // last lb_doc_export_updates(from) per document
@@ -741,11 +744,26 @@ void pipeline(lb_batch* b) {
     const unsigned seq_ctas = seq_resident_ctas(b->device);
     if (nblk(D, LB_SEQ_WARPS) > seq_ctas) LB_BATCH_LAUNCH(b, k_seq_integrate<1>, seq_ctas, 32 * LB_SEQ_WARPS, 0, b->d_docs, D, sp, t);
     else LB_BATCH_LAUNCH(b, k_seq_integrate<0>, nblk(D, LB_SEQ_WARPS), 32 * LB_SEQ_WARPS, 0, b->d_docs, D, sp, t);
+    mark(b, EV_INTEGRATE);
+    // ------------------------------------------------------------ phase 5, cursors: the ropes' order, kept (k_cursor.cuh)
+    if (b->flags & LB_FLAG_CURSORS) {
+        if (NOUT >= 0xFFFFFFFFull) { g_last_error = "batch too large for LB_FLAG_CURSORS: spans must fit 32 bits"; throw lb_status(LB_ERR_INVALID_ARG); }
+        b->cur.ord = dv.alloc<uint4>(NOUT);
+        b->cur.idx = dv.alloc<uint2>(NOUT);
+        b->cur.n = dv.alloc<u32>(NC + 1, true);
+        u32* ent_cont = dv.alloc<u32>(NOUT);
+        u32* fill = dv.alloc<u32>(NC + 1, true);
+        // the atom -> leaf array is done with: it holds the span marks of the counting sort now
+        CK(cudaMemsetAsync(sp.atom_leaf, 0xFF, sizeof(u32) * NATOM, st));
+        LB_BATCH_LAUNCH(b, k_cursor_tables, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, sp, t, b->cur, sp.atom_leaf,
+                        ent_cont, fill);
+        dv.release(ent_cont); dv.release(fill);
+    }
     if (!(b->flags & LB_FLAG_KEEP_DEVICE)) {   // the tracker pools are the largest tables of the batch: free them early
         dv.release(sp.leaf); dv.release(sp.node); dv.release(sp.node_parent); dv.release(sp.atom_leaf); dv.release(sp.a_org);
         dv.release(sp.cvv); dv.release(sp.cont_epoch); dv.release(sp.next_doc); dv.release(t.atom_row); dv.release(t.op_rec);
     }
-    mark(b, EV_INTEGRATE);
+    mark(b, EV_CURSORS);
     // ------------------------------------------------------------ phase 5b: movable trees
     if (NTR) {
         u32* d_tree_slots = dv.alloc<u32>(D + 1);
@@ -966,7 +984,8 @@ void timings_from_events(lb_batch* b) {
     t.resolve = el(EV_DECODE, EV_RESOLVE);
     t.classify = el(EV_RESOLVE, EV_CLASSIFY);
     t.integrate = el(EV_CLASSIFY, EV_INTEGRATE);
-    t.tree = el(EV_INTEGRATE, EV_TREE);
+    t.cursors = el(EV_INTEGRATE, EV_CURSORS);
+    t.tree = el(EV_CURSORS, EV_TREE);
     t.materialise = el(EV_TREE, EV_MATERIALISE);
     t.attribution = el(EV_MATERIALISE, EV_ATTRIBUTION);
     t.reexport = el(EV_ATTRIBUTION, EV_EXPORT);
@@ -1715,6 +1734,7 @@ lb_status lb_import_batch(const lb_blob* blobs, size_t n_blobs, const lb_options
 
 lb_status lb_import_batch_at(const lb_blob* blobs, size_t n_blobs, const lb_version* at, size_t n_at, const lb_options* opt,
                              lb_batch** out) {
+    if (opt && (opt->flags & LB_FLAG_CURSORS)) { g_last_error = "cursors are not answered on checked-out documents"; return LB_ERR_INVALID_ARG; }
     return import_host(blobs, n_blobs, at, n_at, opt, nullptr, false, nullptr, 0, out);
 }
 
@@ -1743,6 +1763,7 @@ lb_status lb_docset_import(lb_docset* set, const lb_blob* blobs, size_t n_blobs,
 
 lb_status lb_docset_checkout(lb_docset* set, const lb_version* at, size_t n_at, const lb_options* opt, lb_batch** out) {
     if (!set) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
+    if (opt && (opt->flags & LB_FLAG_CURSORS)) { g_last_error = "cursors are not answered on checked-out documents"; return LB_ERR_INVALID_ARG; }
     std::lock_guard<std::mutex> g(set->mu);
     return import_host(nullptr, 0, at, n_at, opt, set, true, nullptr, 0, out);
 }
@@ -1853,6 +1874,63 @@ lb_status lb_doc_attribution(const lb_batch* cb, size_t doc, const char** utf8, 
     if (b->docs[doc].code != DOC_OK) { *utf8 = ""; *len = 0; return LB_OK; }
     *utf8 = b->attr + b->attr_off[doc];
     *len = b->attr_off[doc + 1] - b->attr_off[doc];
+    return LB_OK;
+}
+
+lb_status lb_batch_cursor_pos(const lb_batch* cb, const lb_cursor* reqs, size_t n, lb_cursor_result* out) {
+    lb_batch* b = const_cast<lb_batch*>(cb);
+    if (!b || ((!reqs || !out) && n)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
+    if (!(b->flags & LB_FLAG_CURSORS)) { g_last_error = "batch was imported without LB_FLAG_CURSORS"; return LB_ERR_INVALID_ARG; }
+    // the requests, then the root names they carry, packed for one upload
+    size_t name_bytes = 0;
+    for (size_t i = 0; i < n; i++) {
+        if (reqs[i].doc >= b->n_docs) { g_last_error = "document index out of range"; return LB_ERR_INVALID_ARG; }
+        if (reqs[i].is_root && !reqs[i].name && reqs[i].name_len) { g_last_error = "null root container name"; return LB_ERR_INVALID_ARG; }
+        if (reqs[i].is_root) name_bytes += reqs[i].name_len;
+    }
+    if (!n) return LB_OK;
+    const size_t req_bytes = sizeof(CurReq) * n;
+    std::vector<u8> host(req_bytes + name_bytes);
+    CurReq* hq = (CurReq*)host.data();
+    size_t noff = 0;
+    for (size_t i = 0; i < n; i++) {
+        const lb_cursor& c = reqs[i];
+        CurReq& q = hq[i];
+        memset(&q, 0, sizeof(q));
+        q.doc = c.doc;
+        q.is_root = c.is_root ? 1 : 0;
+        q.type = c.type;
+        q.has_id = c.has_id ? 1 : 0;
+        q.side = c.side;
+        q.tpeer = c.id_peer;
+        q.tctr = c.id_counter;
+        if (q.is_root) {
+            if (c.name_len >= 0xFFFFFFFFull) { g_last_error = "root container name too long"; return LB_ERR_INVALID_ARG; }
+            q.name_off = noff;
+            q.name_len = (u32)c.name_len;
+            if (c.name_len) memcpy(host.data() + req_bytes + noff, c.name, c.name_len);
+            noff += c.name_len;
+        } else {
+            q.cpeer = c.peer;
+            q.ccounter = c.counter;
+        }
+    }
+    std::lock_guard<std::mutex> g(b->export_mu);   // device work on demand runs one call at a time
+    try {
+        Dev& dv = b->dev;
+        cudaStream_t st = b->dev.stream;
+        u8* d_in = dv.alloc<u8>(host.size());
+        lb_cursor_result* d_out = dv.alloc<lb_cursor_result>(n);
+        CK(cudaMemcpyAsync(d_in, host.data(), host.size(), cudaMemcpyHostToDevice, st));
+        LB_BATCH_LAUNCH(b, k_cursor_query, nblk((u64)n * 32, 128), 128, 0, b->d_docs, b->tb, b->cur, (const CurReq*)d_in,
+                        (const u8*)(d_in + req_bytes), (u64)n, d_out);
+        CK(cudaMemcpyAsync(out, d_out, sizeof(lb_cursor_result) * n, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        dv.release(d_in);
+        dv.release(d_out);
+    } catch (lb_status s) {
+        return s;
+    }
     return LB_OK;
 }
 
