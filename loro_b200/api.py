@@ -576,12 +576,17 @@ def auto_split(blobs):
     return 1
 
 
-def _import_one(L, blobs, device, flags, doc_ids):
-    arr, keep = _blob_array(blobs, doc_ids)
+def _open_batch(L, entry, device, flags, *args, keep=None):
+    """Call the C entry point `entry(*args, options, &batch)` and wrap the batch it returns."""
     opt = _Options(device=device, flags=flags)
     h = ctypes.c_void_p()
-    _check(L, L.lb_import_batch(arr, len(blobs), ctypes.byref(opt), ctypes.byref(h)), "lb_import_batch")
-    return Batch(L, h.value)
+    _check(L, entry(*args, ctypes.byref(opt), ctypes.byref(h)), entry.__name__)
+    return Batch(L, h.value, keep=keep)
+
+
+def _import_one(L, blobs, device, flags, doc_ids):
+    arr, keep = _blob_array(blobs, doc_ids)
+    return _open_batch(L, L.lb_import_batch, device, flags, arr, len(blobs))
 
 
 def import_batch(blobs, device=0, flags=0, lib_path=None, doc_ids=None, split=None):
@@ -630,12 +635,7 @@ def import_batch(blobs, device=0, flags=0, lib_path=None, doc_ids=None, split=No
                     p.close()
             raise errs[0]
         return MultiBatch(parts)
-    n = len(blobs)
-    arr, keep = _blob_array(blobs, doc_ids)
-    opt = _Options(device=device, flags=flags)
-    h = ctypes.c_void_p()
-    _check(L, L.lb_import_batch(arr, n, ctypes.byref(opt), ctypes.byref(h)), "lb_import_batch")
-    return Batch(L, h.value)
+    return _import_one(L, blobs, device, flags, doc_ids)
 
 
 def import_batch_at(blobs, versions, doc_ids=None, device=0, flags=0, lib_path=None):
@@ -645,11 +645,7 @@ def import_batch_at(blobs, versions, doc_ids=None, device=0, flags=0, lib_path=N
     L = load_library(lib_path)
     arr, keep = _blob_array(blobs, doc_ids)
     ver, vkeep = _version_array(list(versions.items()))
-    opt = _Options(device=device, flags=flags)
-    h = ctypes.c_void_p()
-    _check(L, L.lb_import_batch_at(arr, len(blobs), ver, len(versions), ctypes.byref(opt), ctypes.byref(h)),
-           "lb_import_batch_at")
-    return Batch(L, h.value)
+    return _open_batch(L, L.lb_import_batch_at, device, flags, arr, len(blobs), ver, len(versions))
 
 
 def _till_spans(vv):
@@ -717,10 +713,7 @@ class DocSet:
         """blobs[i] is imported into document doc_ids[i]; several blobs for one id = import_batch on that document.
         Documents of the returned Batch are numbered in order of first appearance of their id."""
         arr, keep = _blob_array(blobs, doc_ids)
-        opt = _Options(device=self._device, flags=flags)
-        h = ctypes.c_void_p()
-        _check(self._L, self._L.lb_docset_import(self._h, arr, len(blobs), ctypes.byref(opt), ctypes.byref(h)), "lb_docset_import")
-        return Batch(self._L, h.value)
+        return _open_batch(self._L, self._L.lb_docset_import, self._device, flags, self._h, arr, len(blobs))
 
     def checkout(self, requests, flags=0):
         """The stored documents at earlier versions: `requests` = [(doc_id, [(peer, counter), ...]), ...].  Document i of
@@ -728,11 +721,7 @@ class DocSet:
         not modified."""
         requests = list(requests)
         ver, keep = _version_array(requests)
-        opt = _Options(device=self._device, flags=flags)
-        h = ctypes.c_void_p()
-        _check(self._L, self._L.lb_docset_checkout(self._h, ver, len(requests), ctypes.byref(opt), ctypes.byref(h)),
-               "lb_docset_checkout")
-        return Batch(self._L, h.value)
+        return _open_batch(self._L, self._L.lb_docset_checkout, self._device, flags, self._h, ver, len(requests))
 
     def read(self, doc_ids, flags=0):
         """The stored documents as they are, nothing imported (lb_docset_read): document i of the returned Batch is
@@ -740,11 +729,7 @@ class DocSet:
         export_updates / export_updates_many answer for it.  The set is not modified."""
         doc_ids = [int(d) for d in doc_ids]
         ids = (ctypes.c_uint64 * max(len(doc_ids), 1))(*doc_ids)
-        opt = _Options(device=self._device, flags=flags)
-        h = ctypes.c_void_p()
-        _check(self._L, self._L.lb_docset_read(self._h, ids, len(doc_ids), ctypes.byref(opt), ctypes.byref(h)),
-               "lb_docset_read")
-        return Batch(self._L, h.value)
+        return _open_batch(self._L, self._L.lb_docset_read, self._device, flags, self._h, ids, len(doc_ids))
 
     @property
     def n_docs(self):
@@ -788,11 +773,7 @@ def import_batch_device(d_bytes_ptr, offsets, lens, device=0, flags=0, lib_path=
     else:
         offs = (ctypes.c_uint64 * max(n, 1))(*[int(x) for x in offsets])
         ls = (ctypes.c_uint32 * max(n, 1))(*[int(x) for x in lens])
-    opt = _Options(device=device, flags=flags)
-    h = ctypes.c_void_p()
-    _check(L, L.lb_import_batch_device(ctypes.c_void_p(d_bytes_ptr), offs, ls, n, ctypes.byref(opt), ctypes.byref(h)),
-           "lb_import_batch_device")
-    return Batch(L, h.value, keep=keep)
+    return _open_batch(L, L.lb_import_batch_device, device, flags, ctypes.c_void_p(d_bytes_ptr), offs, ls, n, keep=keep)
 
 
 def device_trim(device=0, lib_path=None):

@@ -322,6 +322,30 @@ struct Dev {  // owns every device allocation of a batch
 enum BatchEvent { EV_START, EV_H2D, EV_FRAME, EV_DECODE, EV_RESOLVE, EV_CLASSIFY, EV_INTEGRATE, EV_CURSORS, EV_TREE, EV_MATERIALISE,
                   EV_ATTRIBUTION, EV_EXPORT, EV_D2H, EV_COUNT };
 
+// The sizes of the batch-wide tables, each read back from the device by the phase that scans it; the later phases, the
+// on-demand exports, the counters and the debug tables are sized by them.
+struct BatchSizes {
+    u64 blocks = 0;                                                            // frame
+    u64 peers = 0, keys = 0, cids = 0, changes = 0, deps = 0, rows = 0, dels = 0, pos = 0, pos_bytes = 0, tree_ops = 0;  // decode
+    u64 atoms = 0, map_slots = 0;                                              // resolve
+    u64 leaves = 0, nodes = 0, runs = 0, cvv = 0;                              // classify: the sequence trackers' pools
+};
+
+// A per-document result that comes home whole on the first accessor call: the device buffer, its bytes, and the host
+// copy (from lbstage::host_cache, zero-terminated) once fetched.
+struct HostResult {
+    u8* d = nullptr; u64 total = 0; char* host = nullptr; bool fetched = false;
+    lb_status fetch(cudaStream_t st, const char* failed) {
+        if (fetched) return LB_OK;
+        if (!host) host = (char*)lbstage::host_cache().take(total + 1);
+        if (!host) { g_last_error = "out of host memory"; return LB_ERR_OOM; }
+        if (total && !lbstage::download(d, (u8*)host, total, st)) { g_last_error = failed; return LB_ERR_CUDA; }
+        host[total] = 0;
+        fetched = true;
+        return LB_OK;
+    }
+};
+
 struct lb_batch {
     Dev dev;
     size_t n_docs = 0;
@@ -342,34 +366,25 @@ struct lb_batch {
     bool stored_only = false;                 // lb_docset_checkout / lb_docset_read: nothing was imported, the status spans
                                               // stay empty
     DocInfo* d_docs = nullptr;
-    u8* d_json = nullptr;
-    u8* d_export = nullptr;      // phase 7 output: one FastUpdates blob per document
-    // LB_FLAG_ATTRIBUTION (k_attr.cuh): document d's text is [attr_off[d], attr_off[d + 1]) of d_attr; both come home on
-    // the first lb_doc_attribution
-    u8* d_attr = nullptr;
+    BatchSizes n;
+    // per-document results; document d's part is placed by docs[d].json_off / json_len, by [attr_off[d],
+    // attr_off[d + 1]) (LB_FLAG_ATTRIBUTION, k_attr.cuh; the offsets come home with the text) and by xdocs[d].exp_off /
+    // exp_len (phase 7: one FastUpdates blob per document)
+    HostResult json, attr, exported;
     u64* d_attr_off = nullptr;
-    char* attr = nullptr;
     std::vector<u64> attr_off;
-    bool attr_fetched = false;
     // LB_FLAG_CURSORS (k_cursor.cuh): every Text / List rope in document order and by id, for lb_batch_cursor_pos
     CursorTables cur{};
-    u64 export_total = 0;
     std::vector<XDoc> xdocs;
     std::unordered_map<size_t, std::vector<uint8_t>> from_exports;   // last lb_doc_export_updates(from) per document
     std::mutex export_mu;                     // on-demand exports of one batch run one at a time
-    uint8_t* exported = nullptr;  // malloc'ed host copy (lbstage::download)
-    bool export_fetched = false;
-    u64 n_blocks = 0, n_changes = 0, n_rows = 0, n_peers_tot = 0, json_total = 0, n_deps = 0;
     u64 n_segs = 0, fc_cap = 0;   // phase 7: segments (changes + extra segments of split ones), fc_* table capacity
     // host results
     std::vector<DocInfo> docs;
     std::vector<DocPeer> dpeer;          // packed: document d owns [peer_base[d], peer_base[d] + P)
     std::vector<u64> peer_base;
-    char* json = nullptr;   // from lbstage::host_cache (never zero-filled): filled by lbstage::download
-    bool json_fetched = false;
     // host-buffer entry point: the JSON goes home on a second stream while the export phase still computes
     bool eager_json = false, json_ok = true;
-    int device = 0;
     cudaStream_t stream2 = nullptr;
     cudaEvent_t json_ev = nullptr;
     std::thread json_thread;
@@ -464,8 +479,6 @@ unsigned seq_resident_ctas(int device) {
 #endif
 }
 
-// LB_PHASE_TRACE=1: host wall clock between named points (each one synchronises the stream: diagnosis only)
-void trace_point(lb_batch* b, const char* name);
 void mark(lb_batch* b, BatchEvent e) {
     CK(cudaEventRecord(b->ev[e], b->dev.stream));
     b->ev_recorded[e] = true;
@@ -479,6 +492,7 @@ T d2h_one(lb_batch* b, const T* src) {
     return v;
 }
 
+// LB_PHASE_TRACE=1: host wall clock between named points (each one synchronises the stream: diagnosis only)
 void trace_point(lb_batch* b, const char* name) {
     if (!phase_trace()) return;
     static std::chrono::steady_clock::time_point last = std::chrono::steady_clock::now();
@@ -497,9 +511,25 @@ void run_scans(lb_batch* b, std::vector<ScanJob> jobs) {
         LB_BATCH_LAUNCH(b, k_excl_scan_multi, n, 1024, 0, sj);
     }
 }
-#define FIELD_JOB(base, type, in_field, out_field, count)                                              \
-    ScanJob{(const u8*)(base) + offsetof(type, in_field), (u8*)(base) + offsetof(type, out_field), \
-            sizeof(type), sizeof(type), (u64)(count)}
+// The jobs of run_scans: n u32 counts summed exclusively into u64 offsets, the total at index n.  The offsets are the
+// member `field` of the records `rec`, or a plain array; the counts a plain array, or the member `count` of the same
+// records.  The byte offsets and strides of the job follow from the member pointers.
+template <class T>
+ScanJob scan_job(const u32* counts, T* rec, u64 T::*field, u64 n) { return ScanJob{(const u8*)counts, (u8*)&(rec->*field), 4, sizeof(T), n}; }
+template <class T>
+ScanJob scan_job(T* rec, u32 T::*count, u64 T::*field, u64 n) { return ScanJob{(const u8*)&(rec->*count), (u8*)&(rec->*field), sizeof(T), sizeof(T), n}; }
+ScanJob scan_job(const u32* counts, u64* offsets, u64 n) { return ScanJob{(const u8*)counts, (u8*)offsets, 4, 8, n}; }
+
+// Phase 7's final-change tables (FC_TABLES and fc_block) with room for `cap` slots: reallocated, zeroed, when they hold
+// fewer.  What they held is not kept: each export pass fills them afresh.
+void grow_fc_tables(lb_batch* b, u64 cap) {
+    if (cap <= b->fc_cap) return;
+    Dev& dv = b->dev;
+    b->fc_cap = cap;
+    for (auto m : FC_TABLES) { dv.release(b->tb.*m); b->tb.*m = dv.alloc<u32>(cap, true); }
+    dv.release(b->tb.fc_block);
+    b->tb.fc_block = dv.alloc<u8>(cap);
+}
 
 // The encode end of phase 7, after the stores (k_exp_store) have cut every document's changes into output blocks;
 // shared by the batch's export and export_from.  Block list with scratch and staging slots, one encode into the slots,
@@ -514,9 +544,8 @@ u8* export_encode(lb_batch* b, const BatchTables& xt, u64* total, bool cuts) {
     u32* cnt = dv.alloc<u32>(3 * (u64)(D + 1));
     u32 *n_a = cnt, *n_b = cnt + (D + 1), *n_c = cnt + 2 * (D + 1);
     LB_BATCH_LAUNCH(b, k_exp_sizes, nblk(D), TPB, 0, b->d_docs, D, xt, n_a, n_b, n_c);
-    run_scans(b, {ScanJob{(const u8*)n_a, (u8*)xt.xdoc + offsetof(XDoc, ob0), 4, sizeof(XDoc), D},
-                  ScanJob{(const u8*)n_b, (u8*)xt.xdoc + offsetof(XDoc, scratch0), 4, sizeof(XDoc), D},
-                  ScanJob{(const u8*)n_c, (u8*)xt.xdoc + offsetof(XDoc, stage0), 4, sizeof(XDoc), D}});
+    run_scans(b, {scan_job(n_a, xt.xdoc, &XDoc::ob0, D), scan_job(n_b, xt.xdoc, &XDoc::scratch0, D),
+                  scan_job(n_c, xt.xdoc, &XDoc::stage0, D)});
     XDoc xtot = d2h_one(b, xt.xdoc + D);
     const u64 NOB = xtot.ob0, NSCR = xtot.scratch0, NSTG = xtot.stage0;
     XBlock* xb = dv.alloc<XBlock>(NOB + 1);
@@ -529,9 +558,8 @@ u8* export_encode(lb_batch* b, const BatchTables& xt, u64* total, bool cuts) {
     launch_exp_encode(b, NOB, xt, xb, xscratch, xstage, 0, cuts);
     LB_BATCH_LAUNCH(b, k_exp_layout, nblk(D), TPB, 0, b->d_docs, D, xt, xb, n_a, n_b, n_c);
     trace_point(b, "encode");
-    run_scans(b, {ScanJob{(const u8*)n_a, (u8*)xt.xdoc + offsetof(XDoc, exp_off), 4, sizeof(XDoc), D},
-                  ScanJob{(const u8*)n_b, (u8*)xt.xdoc + offsetof(XDoc, ovf0), 4, sizeof(XDoc), D},
-                  ScanJob{(const u8*)n_c, (u8*)xt.xdoc + offsetof(XDoc, restage0), 4, sizeof(XDoc), D}});
+    run_scans(b, {scan_job(n_a, xt.xdoc, &XDoc::exp_off, D), scan_job(n_b, xt.xdoc, &XDoc::ovf0, D),
+                  scan_job(n_c, xt.xdoc, &XDoc::restage0, D)});
     xtot = d2h_one(b, xt.xdoc + D);
     const u64 XT = xtot.exp_off, NOVF = xtot.ovf0, NRST = xtot.restage0;
     if (phase_trace())
@@ -552,78 +580,68 @@ u8* export_encode(lb_batch* b, const BatchTables& xt, u64* total, bool cuts) {
     return out;
 }
 
-void pipeline(lb_batch* b) {
-    Dev& dv = b->dev;
-    cudaStream_t st = dv.stream;
-    u32 D = (u32)b->n_docs;
-    lb_timings& tm = b->timings;
-    if (D == 0) {
-        b->docs.resize(1);
-        return;
-    }
-    BatchTables& t = b->tb;
-    // ------------------------------------------------------------ phase 1: frame
-    u32 Q = (u32)b->n_blobs;
+// The device tables of the import pipeline that one phase makes and a later one reads, besides BatchTables.
+struct PhaseLinks {
+    u32* doc_blob0 = nullptr;                                                  // frame -> resolve
+    uint2* ck_range = nullptr; u64* ck_peer = nullptr; i32* ck_ctr = nullptr;  // checkout requests: frame -> resolve
+    unsigned long long* acc = nullptr;                                         // state hash and counts: materialise -> results
+};
+
+const u32 SEQ_LEAF_W = 32;   // slots per leaf of the sequence trackers = lanes per warp (k_seq.cuh)
+
+// phase 1: the blobs' blocks, and each document's block range
+void phase_frame(lb_batch* b, PhaseLinks& ln) {
+    Dev& dv = b->dev; cudaStream_t st = dv.stream; BatchTables& t = b->tb; const u32 D = (u32)b->n_docs, Q = (u32)b->n_blobs;
     b->d_docs = dv.alloc<DocInfo>(D + 1, true);
     u32* d_blob_code = dv.alloc<u32>(Q + 1, true);
     u32* d_blob_nblocks = dv.alloc<u32>(Q + 1, true);
     u64* d_blob_block0 = dv.alloc<u64>(Q + 2, true);
     u32* d_blob_doc = dv.alloc<u32>(Q + 1);
-    u32* d_doc_blob0 = dv.alloc<u32>(D + 2);
+    ln.doc_blob0 = dv.alloc<u32>(D + 2);
     CK(cudaMemcpyAsync(d_blob_doc, b->blob_doc.data(), sizeof(u32) * Q, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_doc_blob0, b->doc_blob0.data(), sizeof(u32) * (D + 1), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(ln.doc_blob0, b->doc_blob0.data(), sizeof(u32) * (D + 1), cudaMemcpyHostToDevice, st));
     LB_BATCH_LAUNCH(b, k_frame_count, nblk((u64)Q * 32, 128), 128, 0, t.bytes, b->d_offs, b->d_lens, Q, d_blob_code, d_blob_nblocks);
-    run_scans(b, {ScanJob{(const u8*)d_blob_nblocks, (u8*)d_blob_block0, 4, 8, Q}});
+    run_scans(b, {scan_job(d_blob_nblocks, d_blob_block0, Q)});
     u32* d_doc_nprior = nullptr;
     if (!b->doc_nprior.empty()) {
         d_doc_nprior = dv.alloc<u32>(D + 1);
         CK(cudaMemcpyAsync(d_doc_nprior, b->doc_nprior.data(), sizeof(u32) * D, cudaMemcpyHostToDevice, st));
     }
-    uint2* d_ck_range = nullptr;
-    u64* d_ck_peer = nullptr;
-    i32* d_ck_ctr = nullptr;
     if (!b->ck_range.empty()) {   // the host vectors live as long as the batch: no synchronise needed
         const size_t NF = b->ck_peer.size();
-        d_ck_range = dv.alloc<uint2>(D);
-        d_ck_peer = dv.alloc<u64>(NF);
-        d_ck_ctr = dv.alloc<i32>(NF);
-        CK(cudaMemcpyAsync(d_ck_range, b->ck_range.data(), sizeof(u32) * 2 * D, cudaMemcpyHostToDevice, st));
+        ln.ck_range = dv.alloc<uint2>(D);
+        ln.ck_peer = dv.alloc<u64>(NF);
+        ln.ck_ctr = dv.alloc<i32>(NF);
+        CK(cudaMemcpyAsync(ln.ck_range, b->ck_range.data(), sizeof(u32) * 2 * D, cudaMemcpyHostToDevice, st));
         if (NF) {
-            CK(cudaMemcpyAsync(d_ck_peer, b->ck_peer.data(), sizeof(u64) * NF, cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(d_ck_ctr, b->ck_ctr.data(), sizeof(i32) * NF, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(ln.ck_peer, b->ck_peer.data(), sizeof(u64) * NF, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(ln.ck_ctr, b->ck_ctr.data(), sizeof(i32) * NF, cudaMemcpyHostToDevice, st));
         }
     }
-    LB_BATCH_LAUNCH(b, k_frame_docs, nblk(D), TPB, 0, D, d_doc_blob0, d_blob_code, d_blob_block0, d_doc_nprior, b->d_docs);
-    u64 B = d2h_one(b, d_blob_block0 + Q);
-    b->n_blocks = B;
-    t.blocks = dv.alloc<BlockInfo>(B + 1, true);
-    LB_BATCH_LAUNCH(b, k_frame_fill, nblk(Q), TPB, 0, t.bytes, b->d_offs, b->d_lens, Q, d_blob_doc, d_blob_code, d_blob_block0, d_doc_blob0, t.blocks);
+    LB_BATCH_LAUNCH(b, k_frame_docs, nblk(D), TPB, 0, D, ln.doc_blob0, d_blob_code, d_blob_block0, d_doc_nprior, b->d_docs);
+    b->n.blocks = d2h_one(b, d_blob_block0 + Q);
+    t.blocks = dv.alloc<BlockInfo>(b->n.blocks + 1, true);
+    LB_BATCH_LAUNCH(b, k_frame_fill, nblk(Q), TPB, 0, t.bytes, b->d_offs, b->d_lens, Q, d_blob_doc, d_blob_code, d_blob_block0, ln.doc_blob0, t.blocks);
     mark(b, EV_FRAME);
-    // ------------------------------------------------------------ phase 2: decode
+}
+
+// phase 2: the blocks' column sizes, scanned into the batch-wide tables, then the columns decoded into them
+void phase_decode(lb_batch* b) {
+    Dev& dv = b->dev; BatchTables& t = b->tb;
     BlockInfo* blk = t.blocks;
-    if (B) {
-        LB_BATCH_LAUNCH(b, k_block_count, nblk(B, 64), 64, 0, t.bytes, blk, B);
-    }
-    run_scans(b, {FIELD_JOB(blk, BlockInfo, n_peers, peer0, B), FIELD_JOB(blk, BlockInfo, n_keys, key0, B),
-                  FIELD_JOB(blk, BlockInfo, n_cids, cid0, B), FIELD_JOB(blk, BlockInfo, n_changes, ch0, B),
-                  FIELD_JOB(blk, BlockInfo, n_deps, dep0, B), FIELD_JOB(blk, BlockInfo, n_ops, op0, B),
-                  FIELD_JOB(blk, BlockInfo, n_dels, del0, B), FIELD_JOB(blk, BlockInfo, n_pos, pos0, B),
-                  FIELD_JOB(blk, BlockInfo, pos_bytes, posb0, B), FIELD_JOB(blk, BlockInfo, n_tree, tr0, B)});
+    const u64 B = b->n.blocks;
+    if (B) LB_BATCH_LAUNCH(b, k_block_count, nblk(B, 64), 64, 0, t.bytes, blk, B);
+    run_scans(b, {scan_job(blk, &BlockInfo::n_peers, &BlockInfo::peer0, B), scan_job(blk, &BlockInfo::n_keys, &BlockInfo::key0, B),
+                  scan_job(blk, &BlockInfo::n_cids, &BlockInfo::cid0, B), scan_job(blk, &BlockInfo::n_changes, &BlockInfo::ch0, B),
+                  scan_job(blk, &BlockInfo::n_deps, &BlockInfo::dep0, B), scan_job(blk, &BlockInfo::n_ops, &BlockInfo::op0, B),
+                  scan_job(blk, &BlockInfo::n_dels, &BlockInfo::del0, B), scan_job(blk, &BlockInfo::n_pos, &BlockInfo::pos0, B),
+                  scan_job(blk, &BlockInfo::pos_bytes, &BlockInfo::posb0, B), scan_job(blk, &BlockInfo::n_tree, &BlockInfo::tr0, B)});
     BlockInfo tot = d2h_one(b, blk + B);
     u64 NP = tot.peer0, NK = tot.key0, NC = tot.cid0, NCH = tot.ch0, ND = tot.dep0, NR = tot.op0, NDEL = tot.del0;
     u64 NPOS = tot.pos0, NPOSB = tot.posb0, NTR = tot.tr0;
-    if (NTR >= 0xFFFFFFFFull || NPOS >= 0xFFFFFFFFull) {
-        g_last_error = "batch too large: tree ops / positions must fit 32 bits";
-        throw lb_status(LB_ERR_INVALID_ARG);
-    }
-    if (NR >= 0xFFFFFFFFull || NCH >= 0xFFFFFFFFull) {
-        g_last_error = "batch too large: op rows / changes must fit 32 bits";
-        throw lb_status(LB_ERR_INVALID_ARG);
-    }
-    b->n_changes = NCH;
-    b->n_rows = NR;
-    b->n_peers_tot = NP;
-    b->n_deps = ND;
+    if (NTR >= 0xFFFFFFFFull || NPOS >= 0xFFFFFFFFull) { g_last_error = "batch too large: tree ops / positions must fit 32 bits"; throw lb_status(LB_ERR_INVALID_ARG); }
+    if (NR >= 0xFFFFFFFFull || NCH >= 0xFFFFFFFFull) { g_last_error = "batch too large: op rows / changes must fit 32 bits"; throw lb_status(LB_ERR_INVALID_ARG); }
+    b->n = BatchSizes{B, NP, NK, NC, NCH, ND, NR, NDEL, NPOS, NPOSB, NTR};
     t.peer_id = dv.alloc<u64>(NP);
     t.key_off = dv.alloc<u64>(NK); t.key_len = dv.alloc<u32>(NK);
     t.cid_root = dv.alloc<u8>(NC); t.cid_type = dv.alloc<u8>(NC); t.cid_peer_idx = dv.alloc<u32>(NC); t.cid_koc = dv.alloc<i32>(NC);
@@ -658,94 +676,95 @@ void pipeline(lb_batch* b) {
     }
     mark(b, EV_DECODE);
     // SURVEY 8d algorithmic bytes of decode: blob bytes read + SoA written
-    tm.decode_bytes_written = NR * 13 + NCH * (4 + 4 + 8 + 4) + ND * 12;
-    // ------------------------------------------------------------ phase 3: resolve
+    b->timings.decode_bytes_written = NR * 13 + NCH * (4 + 4 + 8 + 4) + ND * 12;
+}
+
+// phase 3: each document's peers, containers and keys, causal order, version vectors and frontiers (and, for a
+// checkout, where each peer's history ends), then its atom and map-slot bases
+void phase_resolve(lb_batch* b, const PhaseLinks& ln) {
+    Dev& dv = b->dev; BatchTables& t = b->tb; BatchSizes& n = b->n; const u32 D = (u32)b->n_docs;
+    const u64 NP = n.peers, NC = n.cids, NK = n.keys, NCH = n.changes;
     t.dpeer = dv.alloc<DocPeer>(NP, true); t.peer_map = dv.alloc<u32>(NP);
     t.dcont = dv.alloc<DocContainer>(NC + 1, true); t.cid_map = dv.alloc<u32>(NC);
     t.dkey_off = dv.alloc<u64>(NK); t.dkey_len = dv.alloc<u32>(NK); t.key_map = dv.alloc<u32>(NK);
-    t.blk_order = dv.alloc<u32>(B);
-    t.ch_order = dv.alloc<u32>(NCH);
-    t.ch_aorder = dv.alloc<u32>(NCH);
-    t.ch_peer = dv.alloc<u16>(NCH);
-    t.ch_applied = dv.alloc<u8>(NCH, true);
-    t.ch_lamport = dv.alloc<u32>(NCH, true);
-    t.ch_walk = dv.alloc<u32>(NCH);
-    t.ch_pos = dv.alloc<u32>(NCH, true);
-    t.ch_trim = dv.alloc<u32>(NCH, true);
+    t.blk_order = dv.alloc<u32>(n.blocks);
+    t.ch_order = dv.alloc<u32>(NCH); t.ch_aorder = dv.alloc<u32>(NCH); t.ch_peer = dv.alloc<u16>(NCH);
+    t.ch_applied = dv.alloc<u8>(NCH, true); t.ch_lamport = dv.alloc<u32>(NCH, true); t.ch_walk = dv.alloc<u32>(NCH);
+    t.ch_pos = dv.alloc<u32>(NCH, true); t.ch_trim = dv.alloc<u32>(NCH, true);
     // status of multi-blob documents (import_batch groups, lb_docset_import): per-copy epochs, per-blob pending hulls
     i32* d_pend_scratch = nullptr;
-    if (Q > D) {
+    if (b->n_blobs > D) {
         t.ch_epoch = dv.alloc<u32>(NCH);
         t.ch_maxend = dv.alloc<i32>(NCH);
         t.head_lamport = dv.alloc<u32>(NP);
-        d_pend_scratch = dv.alloc<i32>(2 * (u64)Q + 2);
+        d_pend_scratch = dv.alloc<i32>(2 * (u64)b->n_blobs + 2);
     }
-    LB_BATCH_LAUNCH(b, k_doc_tables, nblk(D, 64), 64, 0, t.bytes, b->d_docs, D, blk, t);
+    LB_BATCH_LAUNCH(b, k_doc_tables, nblk(D, 64), 64, 0, t.bytes, b->d_docs, D, t.blocks, t);
     u32* d_vv_cells = dv.alloc<u32>(D + 1);
     LB_BATCH_LAUNCH(b, k_doc_vv_cells, nblk(D), TPB, 0, b->d_docs, D, d_vv_cells);
-    run_scans(b, {ScanJob{(const u8*)d_vv_cells, (u8*)b->d_docs + offsetof(DocInfo, vv0), 4, sizeof(DocInfo), D}});
+    run_scans(b, {scan_job(d_vv_cells, b->d_docs, &DocInfo::vv0, D)});
     u64 VV = d2h_one(b, &b->d_docs[D].vv0);
     t.ch_vv = dv.alloc<i32>(VV);
     u32* d_cursor = dv.alloc<u32>(NP);
-    LB_BATCH_LAUNCH(b, k_doc_causal, nblk(D, 64), 64, 0, b->d_docs, D, blk, t, d_cursor, d_doc_blob0, d_pend_scratch);
+    LB_BATCH_LAUNCH(b, k_doc_causal, nblk(D, 64), 64, 0, b->d_docs, D, t.blocks, t, d_cursor, ln.doc_blob0, d_pend_scratch);
     LB_BATCH_LAUNCH(b, k_doc_frontiers, nblk(D, 64), 64, 0, b->d_docs, D, t);
-    if (d_ck_range) {
+    if (ln.ck_range) {
         t.ck_end = dv.alloc<i32>(NP + 1);
-        LB_BATCH_LAUNCH(b, k_doc_checkout, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t, d_ck_range, d_ck_peer, d_ck_ctr);
+        LB_BATCH_LAUNCH(b, k_doc_checkout, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t, ln.ck_range, ln.ck_peer, ln.ck_ctr);
     }
     u32* d_atoms = dv.alloc<u32>(D + 1);
     u32* d_mapslots = dv.alloc<u32>(D + 1);
     LB_BATCH_LAUNCH(b, k_doc_atoms_mapslots, nblk(D), TPB, 0, b->d_docs, D, d_atoms, d_mapslots);
-    run_scans(b, {ScanJob{(const u8*)d_atoms, (u8*)b->d_docs + offsetof(DocInfo, atom0), 4, sizeof(DocInfo), D},
-                  ScanJob{(const u8*)d_mapslots, (u8*)b->d_docs + offsetof(DocInfo, mapslot0), 4, sizeof(DocInfo), D}});
+    run_scans(b, {scan_job(d_atoms, b->d_docs, &DocInfo::atom0, D), scan_job(d_mapslots, b->d_docs, &DocInfo::mapslot0, D)});
     DocInfo dtot = d2h_one(b, &b->d_docs[D]);
-    u64 NATOM = dtot.atom0, NSLOT = dtot.mapslot0;
+    n.atoms = dtot.atom0;
+    n.map_slots = dtot.mapslot0;
     mark(b, EV_RESOLVE);
-    // ------------------------------------------------------------ phase 4: classify + map LWW
+}
+
+// phase 4: classify + map LWW, then the capacities of the sequence trackers' pools
+void phase_classify(lb_batch* b) {
+    Dev& dv = b->dev; BatchTables& t = b->tb; BatchSizes& n = b->n; const u32 D = (u32)b->n_docs;
+    const u64 NR = n.rows, NTR = n.tree_ops, NC = n.cids;
     t.tr_rec = dv.alloc<uint4>(NTR); t.tr_key = dv.alloc<u64>(NTR); t.tr_ids = dv.alloc<uint4>(NTR);
     t.op_kind = dv.alloc<u8>(NR); t.op_cidx = dv.alloc<u32>(NR); t.op_lamport = dv.alloc<u32>(NR);
-    t.atom_row = dv.alloc<u32>(NATOM);
+    t.atom_row = dv.alloc<u32>(n.atoms);
     t.op_rec = dv.alloc<uint4>(NR); t.op_aux = dv.alloc<u32>(NR);
-    t.map_best = dv.alloc<unsigned long long>(NSLOT, true);
-    t.map_row = dv.alloc<u32>(NSLOT);
+    t.map_best = dv.alloc<unsigned long long>(n.map_slots, true);
+    t.map_row = dv.alloc<u32>(n.map_slots);
     if (NR) {
         LB_BATCH_LAUNCH(b, k_op_classify, nblk(NR, 256), 256, 0, b->d_docs, NR, t);
         LB_BATCH_LAUNCH(b, k_map_winner, nblk(NR, 256), 256, 0, b->d_docs, NR, t);
     }
     // capacities -> pools
-    u32* cap_leaf = dv.alloc<u32>(NC + 1, true);
-    u32* cap_node = dv.alloc<u32>(NC + 1, true);
-    u32* cap_out = dv.alloc<u32>(NC + 1, true);
-    u32* cap_cvv = dv.alloc<u32>(NC + 1, true);
+    u32* cap_leaf = dv.alloc<u32>(NC + 1, true); u32* cap_node = dv.alloc<u32>(NC + 1, true);
+    u32* cap_out = dv.alloc<u32>(NC + 1, true); u32* cap_cvv = dv.alloc<u32>(NC + 1, true);
     u32* span_cap = dv.alloc<u32>(D + 1, true);
-    const u32 leaf_w = 32;   // slots per leaf = lanes per warp (k_seq.cuh)
-    LB_BATCH_LAUNCH(b, k_container_caps, nblk(D), TPB, 0, b->d_docs, D, t.dcont, cap_leaf, cap_node, cap_out, cap_cvv, span_cap, leaf_w);
-    run_scans(b, {ScanJob{(const u8*)cap_leaf, (u8*)t.dcont + offsetof(DocContainer, leaf0), 4, sizeof(DocContainer), NC},
-                  ScanJob{(const u8*)cap_node, (u8*)t.dcont + offsetof(DocContainer, node0), 4, sizeof(DocContainer), NC},
-                  ScanJob{(const u8*)cap_out, (u8*)t.dcont + offsetof(DocContainer, out0), 4, sizeof(DocContainer), NC},
-                  ScanJob{(const u8*)cap_cvv, (u8*)t.dcont + offsetof(DocContainer, cvv0), 4, sizeof(DocContainer), NC},
-                  ScanJob{(const u8*)span_cap, (u8*)b->d_docs + offsetof(DocInfo, span0), 4, sizeof(DocInfo), D}});
+    LB_BATCH_LAUNCH(b, k_container_caps, nblk(D), TPB, 0, b->d_docs, D, t.dcont, cap_leaf, cap_node, cap_out, cap_cvv, span_cap, SEQ_LEAF_W);
+    run_scans(b, {scan_job(cap_leaf, t.dcont, &DocContainer::leaf0, NC), scan_job(cap_node, t.dcont, &DocContainer::node0, NC),
+                  scan_job(cap_out, t.dcont, &DocContainer::out0, NC), scan_job(cap_cvv, t.dcont, &DocContainer::cvv0, NC),
+                  scan_job(span_cap, b->d_docs, &DocInfo::span0, D)});
     DocContainer ctot = d2h_one(b, t.dcont + NC);
-    u64 NLEAF = ctot.leaf0, NNODE = ctot.node0, NOUT = ctot.out0, NCVV = ctot.cvv0;
+    n.leaves = ctot.leaf0; n.nodes = ctot.node0; n.runs = ctot.out0; n.cvv = ctot.cvv0;
     mark(b, EV_CLASSIFY);
-    // ------------------------------------------------------------ phase 5: sequence integration
+}
+
+// phase 5: sequence integration; with LB_FLAG_CURSORS the ropes' order is kept for lb_batch_cursor_pos (k_cursor.cuh)
+void phase_integrate(lb_batch* b) {
+    Dev& dv = b->dev; cudaStream_t st = dv.stream; BatchTables& t = b->tb; const BatchSizes& n = b->n; const u32 D = (u32)b->n_docs;
+    const u64 NATOM = n.atoms, NOUT = n.runs, NC = n.cids;
     SeqPools sp;
     memset(&sp, 0, sizeof(sp));
-    sp.leaf = dv.alloc<uint4>(NLEAF * leaf_w);
-    sp.node = dv.alloc<uint2>(NNODE * leaf_w);
-    sp.node_parent = dv.alloc<u32>(NNODE);
-    sp.atom_leaf = dv.alloc<u32>(NATOM);
+    sp.leaf = dv.alloc<uint4>(n.leaves * SEQ_LEAF_W); sp.node = dv.alloc<uint2>(n.nodes * SEQ_LEAF_W);
+    sp.node_parent = dv.alloc<u32>(n.nodes); sp.atom_leaf = dv.alloc<u32>(NATOM);
     CK(cudaMemsetAsync(sp.atom_leaf, 0xFF, sizeof(u32) * NATOM, st));   // LEAF_NONE everywhere
-    sp.a_org = dv.alloc<uint4>(NATOM);
-    sp.cvv = dv.alloc<i32>(NCVV, true);
-    sp.cont_epoch = dv.alloc<u32>(NC + 1);
-    sp.next_doc = dv.alloc<u32>(1, true);
+    sp.a_org = dv.alloc<uint4>(NATOM); sp.cvv = dv.alloc<i32>(n.cvv, true);
+    sp.cont_epoch = dv.alloc<u32>(NC + 1); sp.next_doc = dv.alloc<u32>(1, true);
     t.out_row = dv.alloc<u32>(NOUT); t.out_off = dv.alloc<u32>(NOUT); t.out_len = dv.alloc<u32>(NOUT);
-    const unsigned seq_ctas = seq_resident_ctas(b->device);
+    const unsigned seq_ctas = seq_resident_ctas(b->dev.device);
     if (nblk(D, LB_SEQ_WARPS) > seq_ctas) LB_BATCH_LAUNCH(b, k_seq_integrate<1>, seq_ctas, 32 * LB_SEQ_WARPS, 0, b->d_docs, D, sp, t);
     else LB_BATCH_LAUNCH(b, k_seq_integrate<0>, nblk(D, LB_SEQ_WARPS), 32 * LB_SEQ_WARPS, 0, b->d_docs, D, sp, t);
     mark(b, EV_INTEGRATE);
-    // ------------------------------------------------------------ phase 5, cursors: the ropes' order, kept (k_cursor.cuh)
     if (b->flags & LB_FLAG_CURSORS) {
         if (NOUT >= 0xFFFFFFFFull) { g_last_error = "batch too large for LB_FLAG_CURSORS: spans must fit 32 bits"; throw lb_status(LB_ERR_INVALID_ARG); }
         b->cur.ord = dv.alloc<uint4>(NOUT);
@@ -764,18 +783,22 @@ void pipeline(lb_batch* b) {
         dv.release(sp.cvv); dv.release(sp.cont_epoch); dv.release(sp.next_doc); dv.release(t.atom_row); dv.release(t.op_rec);
     }
     mark(b, EV_CURSORS);
-    // ------------------------------------------------------------ phase 5b: movable trees
+}
+
+// phase 5b: movable trees
+void phase_tree(lb_batch* b) {
+    Dev& dv = b->dev; BatchTables& t = b->tb; const u32 D = (u32)b->n_docs;
+    const u64 NTR = b->n.tree_ops;
     if (NTR) {
         u32* d_tree_slots = dv.alloc<u32>(D + 1);
         u32* d_max_tree_atoms = dv.alloc<u32>(1, true);
         LB_BATCH_LAUNCH(b, k_doc_tree_slots, nblk(D), TPB, 0, b->d_docs, D, d_tree_slots, d_max_tree_atoms);
-        run_scans(b, {ScanJob{(const u8*)d_tree_slots, (u8*)b->d_docs + offsetof(DocInfo, tree0), 4, sizeof(DocInfo), D}});
+        run_scans(b, {scan_job(d_tree_slots, b->d_docs, &DocInfo::tree0, D)});
         u64 NTS = d2h_one(b, &b->d_docs[D].tree0);
         const u32 max_atoms = d2h_one(b, d_max_tree_atoms);
         t.ts_key = dv.alloc<u64>(NTR); t.ts_val = dv.alloc<u32>(NTR); t.ts_rec = dv.alloc<uint4>(NTR);
         t.tn_parent = dv.alloc<u32>(NTS); t.tn_move = dv.alloc<u32>(NTS); t.tn_base = dv.alloc<u32>(NTS);
-        t.tn_cnt = dv.alloc<u32>(NTS); t.tn_sib = dv.alloc<u32>(NTS); t.ns_key = dv.alloc<u64>(NTS);
-        t.tn_child = dv.alloc<u32>(NTS);
+        t.tn_cnt = dv.alloc<u32>(NTS); t.tn_sib = dv.alloc<u32>(NTS); t.ns_key = dv.alloc<u64>(NTS); t.tn_child = dv.alloc<u32>(NTS);
         t.tn_root = dv.alloc<u32>(NTS); t.tn_aopen = dv.alloc<u32>(NTS); t.tn_aclose = dv.alloc<u32>(NTS);
         // 16-bit parent links of one document in shared memory, sized for the largest tree document of the batch:
         // the number of resident documents (one sequential chain each) is what the apply kernel's speed depends on
@@ -796,51 +819,62 @@ void pipeline(lb_batch* b) {
         LB_BATCH_LAUNCH(b, k_tree_layout, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t);
     }
     mark(b, EV_TREE);
-    tm.tree_ops = NTR;
-    // ------------------------------------------------------------ phase 6: JSON
-    unsigned long long* d_acc = dv.alloc<unsigned long long>(4, true);
+    b->timings.tree_ops = NTR;
+}
+
+// phase 6: every document's JSON and state hash.  The host-buffer entry point sends the JSON home from here, on a
+// second stream, while the later phases compute.
+void phase_materialise(lb_batch* b, PhaseLinks& ln) {
+    Dev& dv = b->dev; BatchTables& t = b->tb; const u32 D = (u32)b->n_docs;
+    ln.acc = dv.alloc<unsigned long long>(4, true);
     if (!(b->flags & LB_FLAG_NO_JSON)) {
         LB_BATCH_LAUNCH(b, k_json, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t, (u8*)nullptr, 0);
         u32* d_json_padded = dv.alloc<u32>(D + 1);
         LB_BATCH_LAUNCH(b, k_json_padlen, nblk(D), TPB, 0, b->d_docs, D, d_json_padded);
-        run_scans(b, {ScanJob{(const u8*)d_json_padded, (u8*)b->d_docs + offsetof(DocInfo, json_off), 4, sizeof(DocInfo), D}});
-        u64 JT = d2h_one(b, &b->d_docs[D].json_off);
-        b->json_total = JT;
-        b->d_json = dv.alloc<u8>(JT + 16, true);
-        LB_BATCH_LAUNCH(b, k_json, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t, b->d_json, 1);
+        run_scans(b, {scan_job(d_json_padded, b->d_docs, &DocInfo::json_off, D)});
+        b->json.total = d2h_one(b, &b->d_docs[D].json_off);
+        b->json.d = dv.alloc<u8>(b->json.total + 16, true);
+        LB_BATCH_LAUNCH(b, k_json, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t, b->json.d, 1);
     }
-    LB_BATCH_LAUNCH(b, k_doc_hash, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, (const u8*)b->d_json, d_acc);
+    LB_BATCH_LAUNCH(b, k_doc_hash, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, (const u8*)b->json.d, ln.acc);
     mark(b, EV_MATERIALISE);
-    if (b->eager_json && b->json_total && !(b->flags & LB_FLAG_NO_JSON)) {
+    if (b->eager_json && b->json.total && !(b->flags & LB_FLAG_NO_JSON)) {
         CK(cudaStreamCreate(&b->stream2));
         CK(cudaEventCreate(&b->json_ev));
-        CK(cudaEventRecord(b->json_ev, st));
-        b->json = (char*)lbstage::host_cache().take(b->json_total + 1);
-        if (!b->json) { g_last_error = "out of host memory"; throw lb_status(LB_ERR_OOM); }
+        CK(cudaEventRecord(b->json_ev, dv.stream));
+        b->json.host = (char*)lbstage::host_cache().take(b->json.total + 1);   // taken here: no memory fails the import
+        if (!b->json.host) { g_last_error = "out of host memory"; throw lb_status(LB_ERR_OOM); }
         b->json_thread = std::thread([b] {
-            bool ok = cudaSetDevice(b->device) == cudaSuccess && cudaStreamWaitEvent(b->stream2, b->json_ev, 0) == cudaSuccess &&
-                      lbstage::download(b->d_json, (u8*)b->json, b->json_total, b->stream2);
-            b->json[b->json_total] = 0;
-            b->json_ok = ok;
+            b->json_ok = cudaSetDevice(b->dev.device) == cudaSuccess && cudaStreamWaitEvent(b->stream2, b->json_ev, 0) == cudaSuccess &&
+                         b->json.fetch(b->stream2, "json d2h failed") == LB_OK;
         });
     }
-    // ------------------------------------------------------------ phase 6b: attribution (reads out_*, map_*, tn_*)
+}
+
+// phase 6b: attribution (reads out_*, map_*, tn_*)
+void phase_attribution(lb_batch* b) {
     if (b->flags & LB_FLAG_ATTRIBUTION) {
-        u32* cord = dv.alloc<u32>(NC + 1);
-        u32* kord = dv.alloc<u32>(NK + 1);
+        Dev& dv = b->dev; const u32 D = (u32)b->n_docs;
+        u32* cord = dv.alloc<u32>(b->n.cids + 1);
+        u32* kord = dv.alloc<u32>(b->n.keys + 1);
         u32* d_attr_len = dv.alloc<u32>(D + 1);
         b->d_attr_off = dv.alloc<u64>(D + 1);
-        LB_BATCH_LAUNCH(b, k_attr, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t, cord, kord, d_attr_len,
+        LB_BATCH_LAUNCH(b, k_attr, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, b->tb, cord, kord, d_attr_len,
                         (const u64*)nullptr, (u8*)nullptr, 0);
-        run_scans(b, {ScanJob{(const u8*)d_attr_len, (u8*)b->d_attr_off, 4, 8, D}});
-        const u64 AT = d2h_one(b, b->d_attr_off + D);
-        b->d_attr = dv.alloc<u8>(AT + 16);
-        LB_BATCH_LAUNCH(b, k_attr, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t, cord, kord, d_attr_len,
-                        (const u64*)b->d_attr_off, b->d_attr, 1);
+        run_scans(b, {scan_job(d_attr_len, b->d_attr_off, D)});
+        b->attr.total = d2h_one(b, b->d_attr_off + D);
+        b->attr.d = dv.alloc<u8>(b->attr.total + 16);
+        LB_BATCH_LAUNCH(b, k_attr, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, b->tb, cord, kord, d_attr_len,
+                        (const u64*)b->d_attr_off, b->attr.d, 1);
     }
     mark(b, EV_ATTRIBUTION);
-    // ------------------------------------------------------------ phase 7: re-export (all_updates per document)
+}
+
+// phase 7: re-export (all_updates per document)
+void phase_export(lb_batch* b) {
     if (b->flags & LB_FLAG_EXPORT) {
+        Dev& dv = b->dev; cudaStream_t st = dv.stream; BatchTables& t = b->tb; const u32 D = (u32)b->n_docs;
+        const u64 NCH = b->n.changes, NR = b->n.rows, NTR = b->n.tree_ops, NPOS = b->n.pos;
         trace_point(b, "before export");
         if (NTR) {
             t.pos_rank = dv.alloc<u32>(NPOS); t.pos_rep = dv.alloc<u32>(NPOS);
@@ -849,8 +883,7 @@ void pipeline(lb_batch* b) {
         t.x_rec = dv.alloc<uint4>(NR); t.r_bytes = dv.alloc<u32>(NR); t.r_flag = dv.alloc<u8>(NR);
         t.ch_nseg = dv.alloc<u32>(NCH + 1, true); t.ch_novf = dv.alloc<u32>(NCH + 1, true);
         t.ch_seg0 = dv.alloc<u64>(NCH + 2, true);
-        t.n_changes = NCH;
-        t.n_rows = NR;
+        t.n_changes = NCH; t.n_rows = NR;
         t.ch_syn = dv.alloc<u32>(NCH + 1, true); t.ch_syn0 = dv.alloc<u64>(NCH + 2, true);
         t.xdoc = dv.alloc<XDoc>(D + 1, true);
         t.ch_aval = dv.alloc<u32>(NCH + 1, true); t.ch_astr = dv.alloc<u32>(NCH + 1, true);
@@ -866,49 +899,47 @@ void pipeline(lb_batch* b) {
             if (m == &BatchTables::fc_skip) t.fc_block = dv.alloc<u8>(SEGCAP);
             t.*m = dv.alloc<u32>(SEGCAP, m == &BatchTables::fc_skip || m == &BatchTables::fc_tail);
         }
-        t.x_req = nullptr; t.x_span0 = nullptr; t.x_spans = nullptr;
+        b->fc_cap = SEGCAP;
         trace_point(b, "export allocs");
         LB_BATCH_LAUNCH(b, k_exp_init, nblk(D), TPB, 0, b->d_docs, D, t);
         if (NTR) LB_BATCH_LAUNCH(b, k_exp_posrank, nblk((u64)D * 32, 128), 128, 0, b->d_docs, D, t);
         if (NCH) LB_BATCH_LAUNCH(b, k_exp_arena, nblk(NCH * 32, XCH_TPB), XCH_TPB, 0, NCH, t, b->d_docs);
-        run_scans(b, {ScanJob{(const u8*)t.ch_aval, (u8*)t.ch_aval0, 4, 8, NCH}, ScanJob{(const u8*)t.ch_astr, (u8*)t.ch_astr0, 4, 8, NCH}});
+        run_scans(b, {scan_job(t.ch_aval, t.ch_aval0, NCH), scan_job(t.ch_astr, t.ch_astr0, NCH)});
         trace_point(b, "posrank+arena");
         if (NCH) LB_BATCH_LAUNCH(b, k_exp_changes, nblk(NCH * 32, XCH_TPB), XCH_TPB, 0, b->d_docs, NCH, t);
         trace_point(b, "changes pass 0");
-        run_scans(b, {ScanJob{(const u8*)t.ch_novf, (u8*)t.ch_seg0, 4, 8, NCH}, ScanJob{(const u8*)t.ch_syn, (u8*)t.ch_syn0, 4, 8, NCH}});
+        run_scans(b, {scan_job(t.ch_novf, t.ch_seg0, NCH), scan_job(t.ch_syn, t.ch_syn0, NCH)});
         u64 NOVF = d2h_one(b, t.ch_seg0 + NCH);
         u64 NSYN = d2h_one(b, t.ch_syn0 + NCH);
         t.has_syn = NSYN ? 1 : 0;
         t.s_rec = dv.alloc<uint4>(NSYN); t.s_len = dv.alloc<u32>(NSYN); t.s_bytes = dv.alloc<u32>(NSYN);
         t.s_flag = dv.alloc<u8>(NSYN); t.s_voff = dv.alloc<u64>(NSYN); t.s_vlen = dv.alloc<u32>(NSYN); t.s_aux = dv.alloc<u32>(NSYN);
         if (NCH + NOVF > SEGCAP) {   // unusually many split changes: grow the tables, keep what k_exp_changes wrote
-            u64 cap = NCH + NOVF;
             for (auto m : SG_TABLES) {
-                u32* nw = dv.alloc<u32>(cap);
+                u32* nw = dv.alloc<u32>(NCH + NOVF);
                 CK(cudaMemcpyAsync(nw, t.*m, sizeof(u32) * NCH, cudaMemcpyDeviceToDevice, st));
                 dv.release(t.*m);
                 t.*m = nw;
             }
-            for (auto m : FC_TABLES) { dv.release(t.*m); t.*m = dv.alloc<u32>(cap, true); }
-            dv.release(t.fc_block);
-            t.fc_block = dv.alloc<u8>(cap);
         }
+        grow_fc_tables(b, NCH + NOVF);
         b->n_segs = NCH + NOVF;
-        b->fc_cap = std::max(SEGCAP, NCH + NOVF);
         if (NOVF) LB_BATCH_LAUNCH(b, k_exp_split_changes, nblk(NCH, 64), 64, 0, b->d_docs, NCH, t);
         LB_BATCH_LAUNCH(b, k_exp_store, nblk(D, 64), 64, 0, b->d_docs, D, t);
-        u64 XT = 0;
-        b->d_export = export_encode(b, t, &XT, false);
-        b->export_total = XT;
-        tm.export_bytes = XT;
+        b->exported.d = export_encode(b, t, &b->exported.total, false);
+        b->timings.export_bytes = b->exported.total;
     }
     mark(b, EV_EXPORT);
-    // ------------------------------------------------------------ results to host
+}
+
+// the documents' records, the counters and the documents' peer entries to the host
+void results_to_host(lb_batch* b, const PhaseLinks& ln) {
+    Dev& dv = b->dev; cudaStream_t st = dv.stream; const BatchTables& t = b->tb; const u32 D = (u32)b->n_docs;
     b->t_tail = std::chrono::steady_clock::now();
     b->docs.resize(D + 1);
     CK(cudaMemcpyAsync(b->docs.data(), b->d_docs, sizeof(DocInfo) * (D + 1), cudaMemcpyDeviceToHost, st));
     unsigned long long acc[4];
-    CK(cudaMemcpyAsync(acc, d_acc, sizeof(acc), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(acc, ln.acc, sizeof(acc), cudaMemcpyDeviceToHost, st));
     unsigned long long dws[4] = {0, 0, 0, 0};
     CK(cudaMemcpyAsync(dws, t.dw_stats, sizeof(dws), cudaMemcpyDeviceToHost, st));
     if (t.xdoc) {
@@ -918,33 +949,44 @@ void pipeline(lb_batch* b) {
     CK(cudaStreamSynchronize(st));
     // the peer table is sized by the blocks' peer registers (a few entries per BLOCK: hundreds of MB for 10^6 blocks) but a
     // document uses only its first P entries: those are packed on the device and only they travel
-    {
-        b->peer_base.assign(D + 1, 0);
-        for (u32 d = 0; d < D; d++) b->peer_base[d + 1] = b->peer_base[d] + b->docs[d].P;
-        const u64 total = b->peer_base[D];
-        b->dpeer.resize(total);
-        if (total) {
-            u64* d_pbase = dv.alloc<u64>(D + 1);
-            DocPeer* d_packed = dv.alloc<DocPeer>(total);
-            CK(cudaMemcpyAsync(d_pbase, b->peer_base.data(), sizeof(u64) * (D + 1), cudaMemcpyHostToDevice, st));
-            LB_BATCH_LAUNCH(b, k_pack_peers, nblk(D), TPB, 0, b->d_docs, D, t.dpeer, d_pbase, d_packed);
-            CK(cudaMemcpyAsync(b->dpeer.data(), d_packed, sizeof(DocPeer) * total, cudaMemcpyDeviceToHost, st));
-        }
+    b->peer_base.assign(D + 1, 0);
+    for (u32 d = 0; d < D; d++) b->peer_base[d + 1] = b->peer_base[d] + b->docs[d].P;
+    const u64 total = b->peer_base[D];
+    b->dpeer.resize(total);
+    if (total) {
+        u64* d_pbase = dv.alloc<u64>(D + 1);
+        DocPeer* d_packed = dv.alloc<DocPeer>(total);
+        CK(cudaMemcpyAsync(d_pbase, b->peer_base.data(), sizeof(u64) * (D + 1), cudaMemcpyHostToDevice, st));
+        LB_BATCH_LAUNCH(b, k_pack_peers, nblk(D), TPB, 0, b->d_docs, D, t.dpeer, d_pbase, d_packed);
+        CK(cudaMemcpyAsync(b->dpeer.data(), d_packed, sizeof(DocPeer) * total, cudaMemcpyDeviceToHost, st));
     }
     mark(b, EV_D2H);   // the result copies are queued
     CK(cudaStreamSynchronize(st));
     lb_counters& c = b->counters;
-    c.docs = D;
-    c.docs_ok = acc[3];
-    c.blocks = B;
-    c.changes = NCH;
-    c.op_rows = NR;
-    c.atom_ops = acc[1];
-    c.pending_changes = acc[2];
-    c.state_hash = acc[0];
+    c.docs = D; c.docs_ok = acc[3]; c.atom_ops = acc[1]; c.pending_changes = acc[2]; c.state_hash = acc[0];
+    c.blocks = b->n.blocks; c.changes = b->n.changes; c.op_rows = b->n.rows;
+    lb_timings& tm = b->timings;
     tm.decode_fast_blocks = dws[0]; tm.decode_lane_blocks = dws[1]; tm.decode_unstaged_blocks = dws[2];
     c.json_bytes = 0;
     for (u32 d = 0; d < D; d++) c.json_bytes += b->docs[d].json_len;
+}
+
+void pipeline(lb_batch* b) {
+    if (b->n_docs == 0) {
+        b->docs.resize(1);
+        return;
+    }
+    PhaseLinks ln;
+    phase_frame(b, ln);
+    phase_decode(b);
+    phase_resolve(b, ln);
+    phase_classify(b);
+    phase_integrate(b);
+    phase_tree(b);
+    phase_materialise(b, ln);
+    phase_attribution(b);
+    phase_export(b);
+    results_to_host(b, ln);
 }
 
 // ImportStatus / vv / frontiers spans of every document, flat: [off[d], off[d + 1]) of one array per kind (a vector per
@@ -1070,9 +1112,9 @@ lb_status import_with_new_batch(const lb_options* opt, lb_batch** out, Fill fill
     if (s != LB_OK) return s;
     lb_batch* b = new lb_batch();
     b->flags = opt ? opt->flags : 0;
-    b->device = b->dev.device = opt ? opt->device : 0;
+    b->dev.device = opt ? opt->device : 0;
     try {
-        b->dev.stream = stream_take(b->device);
+        b->dev.stream = stream_take(b->dev.device);
         if (!b->dev.stream) { g_last_error = "cudaStreamCreate failed"; throw lb_status(LB_ERR_CUDA); }
         for (cudaEvent_t& e : b->ev) CK(cudaEventCreate(&e));
         b->ev_created = true;
@@ -1113,7 +1155,7 @@ lb_exports::Answer doc_error(const DocInfo& di) {
 BatchTables export_pass(lb_batch* b, const std::vector<u8>& h_req) {
     Dev& dv = b->dev;
     const u32 D = (u32)b->n_docs;
-    const u64 NCH = b->n_changes;
+    const u64 NCH = b->n.changes;
     BatchTables xt = b->tb;
     u8* d_req = dv.alloc<u8>(D);
     CK(cudaMemcpyAsync(d_req, h_req.data(), D, cudaMemcpyHostToDevice, dv.stream));
@@ -1142,13 +1184,7 @@ std::unique_ptr<uint8_t[]> export_round(lb_batch* b, const std::vector<u32>& h_s
     Dev& dv = b->dev;
     cudaStream_t st = dv.stream;
     const u32 D = (u32)b->n_docs;
-    // a document's final changes get one slot per segment and one per span (xfc0): grow the tables when a round needs more
-    if (b->n_segs + h_spans.size() > b->fc_cap) {
-        b->fc_cap = b->n_segs + h_spans.size();
-        for (auto m : FC_TABLES) { dv.release(b->tb.*m); b->tb.*m = dv.alloc<u32>(b->fc_cap, true); }
-        dv.release(b->tb.fc_block);
-        b->tb.fc_block = dv.alloc<u8>(b->fc_cap);
-    }
+    grow_fc_tables(b, b->n_segs + h_spans.size());   // a document's final changes get one slot per segment and one per span (xfc0)
     u32* d_span0 = dv.alloc<u32>(h_span0.size());
     XSpan* d_spans = dv.alloc<XSpan>(std::max<size_t>(h_spans.size(), 1));
     CK(cudaMemcpyAsync(d_span0, h_span0.data(), sizeof(u32) * h_span0.size(), cudaMemcpyHostToDevice, st));
@@ -1218,7 +1254,7 @@ void export_span_sets(lb_batch* b, size_t n, DocOf doc_of, KeyOf key_of, lb_expo
         for (size_t i : all_updates) {
             const XDoc& x = b->xdocs[doc_of(i)];
             if ((x.flags & 1) || x.exp_len == 0) { e.answers[i] = lb_exports::Answer{LB_ERR_UNSUPPORTED, ERR_NOT_COVERED, nullptr, 0}; continue; }
-            CK(cudaMemcpyAsync(w, b->d_export + x.exp_off, x.exp_len, cudaMemcpyDeviceToHost, b->dev.stream));
+            CK(cudaMemcpyAsync(w, b->exported.d + x.exp_off, x.exp_len, cudaMemcpyDeviceToHost, b->dev.stream));
             e.answers[i].bytes = w;
             e.answers[i].len = x.exp_len;
             w += x.exp_len;
@@ -1229,7 +1265,7 @@ void export_span_sets(lb_batch* b, size_t n, DocOf doc_of, KeyOf key_of, lb_expo
     for (const auto& kv : of_doc) rounds = std::max(rounds, kv.second.size());
     std::vector<XDoc> xd;
     for (size_t r = 0; r < rounds; r++) {
-        std::vector<const i32*> slot_key(b->n_peers_tot, nullptr);   // peer slot -> its part of the round's key
+        std::vector<const i32*> slot_key(b->n.peers, nullptr);   // peer slot -> its part of the round's key
         std::vector<u8> h_req(b->n_docs, 0);
         bool cuts = false;
         for (const auto& kv : of_doc) {
@@ -1244,14 +1280,14 @@ void export_span_sets(lb_batch* b, size_t n, DocOf doc_of, KeyOf key_of, lb_expo
             }
             h_req[v.doc] = 1;
         }
-        std::vector<u32> h_span0(b->n_peers_tot + 1, 0);
+        std::vector<u32> h_span0(b->n.peers + 1, 0);
         std::vector<XSpan> h_spans;
-        for (size_t slot = 0; slot < b->n_peers_tot; slot++) {
+        for (size_t slot = 0; slot < b->n.peers; slot++) {
             h_span0[slot] = (u32)h_spans.size();
             if (const i32* k = slot_key[slot])
                 for (i32 q = 0; q < k[0]; q++) h_spans.push_back(XSpan{k[1 + 3 * q], k[2 + 3 * q], (u32)k[3 + 3 * q], 0});
         }
-        h_span0[b->n_peers_tot] = (u32)h_spans.size();
+        h_span0[b->n.peers] = (u32)h_spans.size();
         e.bufs.push_back(export_round(b, h_span0, h_spans, cuts, h_req, xd));
         const uint8_t* blobs = e.bufs.back().get();
         for (size_t i = 0; i < n; i++) {
@@ -1374,8 +1410,8 @@ void json_requests(lb_batch* b, const lb_json_request* reqs, size_t n, lb_export
     const u64 NR = jr.size(), S = std::max<size_t>(h_start.size(), 1);
     JxReq* d_jr = dv.alloc<JxReq>(NR);
     JxScratch s{dv.alloc<i32>(S), dv.alloc<i32>(S), dv.alloc<u32>(S), dv.alloc<u32>(S), dv.alloc<u32>(S)};
-    u32* d_pf0 = dv.alloc<u32>(b->n_peers_tot + 1);
-    u32* d_pfn = dv.alloc<u32>(b->n_peers_tot + 1);
+    u32* d_pf0 = dv.alloc<u32>(b->n.peers + 1);
+    u32* d_pfn = dv.alloc<u32>(b->n.peers + 1);
     CK(cudaMemcpyAsync(s.start, h_start.data(), sizeof(i32) * h_start.size(), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(s.end, h_end.data(), sizeof(i32) * h_end.size(), cudaMemcpyHostToDevice, st));
     BatchTables xt = export_pass(b, h_req);
@@ -1531,7 +1567,7 @@ void docset_store(lb_docset* set, lb_batch* b, const std::vector<u64>& offs, con
             nd_.blobs.push_back(DocsetBlob{buf, w, len});
             w += ((u64)len + 15) & ~(u64)15;
         };
-        if (pk.exported) push(b->d_export + b->xdocs[pk.doc].exp_off, b->xdocs[pk.doc].exp_len);
+        if (pk.exported) push(b->exported.d + b->xdocs[pk.doc].exp_off, b->xdocs[pk.doc].exp_len);
         else for (u32 q = b->doc_blob0[pk.doc]; q < b->doc_blob0[pk.doc + 1]; q++) push(b->tb.bytes + offs[q], lens[q]);
         fresh.push_back({b->doc_ids[pk.doc], std::move(nd_)});
     }
@@ -1547,22 +1583,28 @@ void docset_store(lb_docset* set, lb_batch* b, const std::vector<u64>& offs, con
     }
 }
 
+// The host-buffer entry points (they share import_host).
+enum class HostEntry { IMPORT, IMPORT_AT, DOCSET_IMPORT, DOCSET_CHECKOUT, DOCSET_READ };
+
 extern "C" {
 
 // Host-buffer import, shared by lb_import_batch (fresh documents), lb_docset_import (documents with an earlier state:
 // their stored blobs come first, already in device memory, and count as `n_prior` for the import status) and the
-// checkout entry points: `at` names the documents built at an earlier version (k_checkout.cuh).  With `set_checkout` the
-// documents are the requests themselves, one per entry of `at`, each made of its document's stored blobs only; with
-// `read_ids` (lb_docset_read) they are the listed ids, each made of its stored blobs, at the latest version and exported.
-// In both the docset is read, never written.
-static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_version* at, size_t n_at, const lb_options* opt,
-                             lb_docset* set, bool set_checkout, const uint64_t* read_ids, size_t n_read, lb_batch** out) {
+// checkout entry points: `at` names the documents built at an earlier version (k_checkout.cuh).  For DOCSET_CHECKOUT the
+// documents are the requests themselves, one per entry of `at`, each made of its document's stored blobs only; for
+// DOCSET_READ they are the listed `read_ids`, each made of its stored blobs, at the latest version and exported.  In both
+// the docset is read, never written.
+// The flags each entry point takes are decided here: a checked-out document answers no cursor and is not exported, a
+// read writes nothing back, and a docset import or read is always exported (the re-export is what a stored document
+// keeps, and what a read answers from).  The cursor flag is refused before a null argument, the other flags after it.
+static lb_status import_host(HostEntry entry, lb_docset* set, const lb_blob* blobs, size_t n_blobs, const lb_version* at,
+                             size_t n_at, const uint64_t* read_ids, size_t n_read, const lb_options* opt, lb_batch** out) {
+    const bool checkout = entry == HostEntry::IMPORT_AT || entry == HostEntry::DOCSET_CHECKOUT;
+    lb_options o2 = opt ? *opt : lb_options{};
+    if (checkout && (o2.flags & LB_FLAG_CURSORS)) { g_last_error = "cursors are not answered on checked-out documents"; return LB_ERR_INVALID_ARG; }
     if (!out || (!blobs && n_blobs) || (!at && n_at) || (!read_ids && n_read)) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
     *out = nullptr;
-    lb_options o2;
-    memset(&o2, 0, sizeof(o2));
-    if (opt) o2 = *opt;
-    if (at || set_checkout) {
+    if (checkout) {
         if (o2.flags & (LB_FLAG_EXPORT | LB_FLAG_COMPACT)) {
             g_last_error = "a checked-out document is not exported (LB_FLAG_EXPORT / LB_FLAG_COMPACT)";
             return LB_ERR_INVALID_ARG;
@@ -1570,66 +1612,60 @@ static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_vers
         for (size_t i = 0; i < n_at; i++)
             if (!at[i].frontiers && at[i].n_frontiers) { g_last_error = "null frontiers"; return LB_ERR_INVALID_ARG; }
     }
-    if (read_ids && (o2.flags & LB_FLAG_COMPACT)) { g_last_error = "LB_FLAG_COMPACT on a read: the docset is not written"; return LB_ERR_INVALID_ARG; }
+    if (entry == HostEntry::DOCSET_READ && (o2.flags & LB_FLAG_COMPACT)) { g_last_error = "LB_FLAG_COMPACT on a read: the docset is not written"; return LB_ERR_INVALID_ARG; }
     if (set) o2.device = set->device;
-    if (set && !set_checkout) o2.flags |= LB_FLAG_EXPORT;   // the re-export is what a stored document keeps (or is read for)
+    if (entry == HostEntry::DOCSET_IMPORT || entry == HostEntry::DOCSET_READ) o2.flags |= LB_FLAG_EXPORT;
     return import_with_new_batch(&o2, out, [&](lb_batch* b) {
         if (n_blobs >= 0x7FFFFFFFull) { g_last_error = "too many blobs"; throw lb_status(LB_ERR_INVALID_ARG); }
         b->eager_json = true;   // host buffers in, host results expected
         // blobs with the same doc_id form one document (LoroDoc::import_batch); documents are numbered in order of
         // first appearance and their blobs laid out consecutively, in the order given
         std::vector<u32> order(n_blobs);
-        std::vector<u32> host_count;
+        std::vector<u32> count;   // new blobs per document
         std::unordered_map<u64, u32> doc_of;
-        {
-            std::vector<u32> doc_idx(n_blobs);
-            std::vector<u32>& count = host_count;
-            for (size_t i = 0; i < n_blobs; i++) {
-                auto it = doc_of.find(blobs[i].doc_id);
-                if (it == doc_of.end()) {
-                    it = doc_of.emplace(blobs[i].doc_id, (u32)count.size()).first;
-                    count.push_back(0);
-                    b->doc_ids.push_back(blobs[i].doc_id);
-                }
-                doc_idx[i] = it->second;
-                count[it->second]++;
-            }
-            size_t nd = count.size();
-            std::vector<u32> first(nd + 1, 0);
-            for (size_t d = 0; d < nd; d++) first[d + 1] = first[d] + count[d];
-            std::vector<u32> cursor(first.begin(), first.end() - 1);
-            for (size_t i = 0; i < n_blobs; i++) order[cursor[doc_idx[i]]++] = (u32)i;
-            // import_batch imports its blobs sorted by (mode, number of changes descending), stably
-            // (loro.rs:1194-1202): the order decides where payloads land in the document's arenas, which the
-            // re-export merge rules look at
-            for (size_t d = 0; d < nd; d++) {
-                u32 q0 = first[d], q1 = first[d + 1];
-                if (q1 - q0 < 2) continue;
-                std::vector<std::pair<std::pair<u32, i64>, u32>> keyed;
-                for (u32 q = q0; q < q1; q++) {
-                    const lb_blob& bl = blobs[order[q]];
-                    keyed.push_back({{blob_mode(bl.ptr, bl.len), -(i64)blob_change_count(bl.ptr, bl.len)}, order[q]});
-                }
-                std::stable_sort(keyed.begin(), keyed.end(), [](const auto& x, const auto& y) { return x.first < y.first; });
-                for (u32 q = q0; q < q1; q++) order[q] = keyed[q - q0].second;
-            }
-            if (set_checkout)   // one document per request, in request order (no new blobs)
-                for (size_t i = 0; i < n_at; i++) { b->doc_ids.push_back(at[i].doc_id); count.push_back(0); nd++; }
-            for (size_t i = 0; i < n_read; i++) {   // one document per listed id, in list order (no new blobs)
-                if (!doc_of.emplace(read_ids[i], (u32)nd).second) { g_last_error = "doc_id listed twice"; throw lb_status(LB_ERR_INVALID_ARG); }
-                b->doc_ids.push_back(read_ids[i]);
+        std::vector<u32> doc_idx(n_blobs);
+        for (size_t i = 0; i < n_blobs; i++) {
+            auto it = doc_of.find(blobs[i].doc_id);
+            if (it == doc_of.end()) {
+                it = doc_of.emplace(blobs[i].doc_id, (u32)count.size()).first;
                 count.push_back(0);
-                nd++;
+                b->doc_ids.push_back(blobs[i].doc_id);
             }
-            b->stored_only = set_checkout || read_ids;
-            b->n_docs = nd;
+            doc_idx[i] = it->second;
+            count[it->second]++;
         }
-        const size_t nd = b->n_docs;
-        if (at) {
+        size_t nd = count.size();
+        std::vector<u32> first(nd + 1, 0);
+        for (size_t d = 0; d < nd; d++) first[d + 1] = first[d] + count[d];
+        std::vector<u32> cursor(first.begin(), first.end() - 1);
+        for (size_t i = 0; i < n_blobs; i++) order[cursor[doc_idx[i]]++] = (u32)i;
+        // import_batch imports its blobs sorted by (mode, number of changes descending), stably
+        // (loro.rs:1194-1202): the order decides where payloads land in the document's arenas, which the
+        // re-export merge rules look at
+        for (size_t d = 0; d < nd; d++) {
+            u32 q0 = first[d], q1 = first[d + 1];
+            if (q1 - q0 < 2) continue;
+            std::vector<std::pair<std::pair<u32, i64>, u32>> keyed;
+            for (u32 q = q0; q < q1; q++) {
+                const lb_blob& bl = blobs[order[q]];
+                keyed.push_back({{blob_mode(bl.ptr, bl.len), -(i64)blob_change_count(bl.ptr, bl.len)}, order[q]});
+            }
+            std::stable_sort(keyed.begin(), keyed.end(), [](const auto& x, const auto& y) { return x.first < y.first; });
+            for (u32 q = q0; q < q1; q++) order[q] = keyed[q - q0].second;
+        }
+        if (entry == HostEntry::DOCSET_CHECKOUT)   // one document per request, in request order (no new blobs)
+            for (size_t i = 0; i < n_at; i++) { b->doc_ids.push_back(at[i].doc_id); count.push_back(0); nd++; }
+        for (size_t i = 0; i < n_read; i++) {   // one document per listed id, in list order (no new blobs)
+            if (!doc_of.emplace(read_ids[i], (u32)nd).second) { g_last_error = "doc_id listed twice"; throw lb_status(LB_ERR_INVALID_ARG); }
+            b->doc_ids.push_back(read_ids[i]); count.push_back(0); nd++;
+        }
+        b->stored_only = entry == HostEntry::DOCSET_CHECKOUT || entry == HostEntry::DOCSET_READ;
+        b->n_docs = nd;
+        if (checkout) {
             b->ck_range.assign(2 * nd, CK_LATEST);
             for (size_t i = 0; i < n_at; i++) {
                 u32 d = (u32)i;
-                if (!set_checkout) {
+                if (entry == HostEntry::IMPORT_AT) {
                     auto it = doc_of.find(at[i].doc_id);
                     if (it == doc_of.end()) { g_last_error = "checkout of a doc_id no blob carries"; throw lb_status(LB_ERR_INVALID_ARG); }
                     d = it->second;
@@ -1676,31 +1712,28 @@ static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_vers
         size_t q = 0, hq = 0;
         for (size_t d = 0; d < nd; d++) {
             b->doc_blob0[d] = (u32)q;
+            auto place = [&](u64& w, u64 len) {   // blob q of document d at byte w of the batch buffer
+                offs[q] = w;
+                lens[q] = (u32)len;
+                b->blob_doc[q++] = (u32)d;
+                w += (len + 15) & ~(u64)15;
+                b->counters.blob_bytes += len;
+            };
             if (prior[d])
                 for (const DocsetBlob& sb : prior[d]->blobs) {
-                    offs[q] = ptotal;
-                    lens[q] = sb.len;
-                    b->blob_doc[q] = (u32)d;
                     segs.push_back(CopySeg{sb.buf->d + sb.off, nullptr, sb.len});
                     seg_offs.push_back(ptotal);
-                    ptotal += ((u64)sb.len + 15) & ~(u64)15;
-                    b->counters.blob_bytes += sb.len;
-                    q++;
+                    place(ptotal, sb.len);
                 }
-            for (u32 k = 0; k < host_count[d]; k++, hq++) {
+            for (u32 k = 0; k < count[d]; k++, hq++) {
                 const lb_blob& bl = blobs[order[hq]];
                 if (bl.len > 0xFFFFFFF0ull || (!bl.ptr && bl.len)) {
                     g_last_error = "blob too large or null";
                     throw lb_status(LB_ERR_INVALID_ARG);
                 }
-                offs[q] = total;
-                lens[q] = (u32)bl.len;
-                b->blob_doc[q] = (u32)d;
                 views.push_back(lbstage::BlobView{bl.ptr, bl.len});
                 view_offs.push_back(total);
-                total += (bl.len + 15) & ~(u64)15;
-                b->counters.blob_bytes += bl.len;
-                q++;
+                place(total, bl.len);
             }
         }
         b->doc_blob0[nd] = (u32)q;
@@ -1729,13 +1762,12 @@ static lb_status import_host(const lb_blob* blobs, size_t n_blobs, const lb_vers
 }
 
 lb_status lb_import_batch(const lb_blob* blobs, size_t n_blobs, const lb_options* opt, lb_batch** out) {
-    return import_host(blobs, n_blobs, nullptr, 0, opt, nullptr, false, nullptr, 0, out);
+    return import_host(HostEntry::IMPORT, nullptr, blobs, n_blobs, nullptr, 0, nullptr, 0, opt, out);
 }
 
 lb_status lb_import_batch_at(const lb_blob* blobs, size_t n_blobs, const lb_version* at, size_t n_at, const lb_options* opt,
                              lb_batch** out) {
-    if (opt && (opt->flags & LB_FLAG_CURSORS)) { g_last_error = "cursors are not answered on checked-out documents"; return LB_ERR_INVALID_ARG; }
-    return import_host(blobs, n_blobs, at, n_at, opt, nullptr, false, nullptr, 0, out);
+    return import_host(HostEntry::IMPORT_AT, nullptr, blobs, n_blobs, at, n_at, nullptr, 0, opt, out);
 }
 
 lb_status lb_docset_new(const lb_options* opt, lb_docset** out) {
@@ -1758,20 +1790,19 @@ uint64_t lb_docset_stored_bytes(const lb_docset* set) { return set ? set->stored
 lb_status lb_docset_import(lb_docset* set, const lb_blob* blobs, size_t n_blobs, const lb_options* opt, lb_batch** out) {
     if (!set) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
     std::lock_guard<std::mutex> g(set->mu);
-    return import_host(blobs, n_blobs, nullptr, 0, opt, set, false, nullptr, 0, out);
+    return import_host(HostEntry::DOCSET_IMPORT, set, blobs, n_blobs, nullptr, 0, nullptr, 0, opt, out);
 }
 
 lb_status lb_docset_checkout(lb_docset* set, const lb_version* at, size_t n_at, const lb_options* opt, lb_batch** out) {
     if (!set) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
-    if (opt && (opt->flags & LB_FLAG_CURSORS)) { g_last_error = "cursors are not answered on checked-out documents"; return LB_ERR_INVALID_ARG; }
     std::lock_guard<std::mutex> g(set->mu);
-    return import_host(nullptr, 0, at, n_at, opt, set, true, nullptr, 0, out);
+    return import_host(HostEntry::DOCSET_CHECKOUT, set, nullptr, 0, at, n_at, nullptr, 0, opt, out);
 }
 
 lb_status lb_docset_read(lb_docset* set, const uint64_t* doc_ids, size_t n, const lb_options* opt, lb_batch** out) {
     if (!set) { g_last_error = "null argument"; return LB_ERR_INVALID_ARG; }
     std::lock_guard<std::mutex> g(set->mu);
-    return import_host(nullptr, 0, nullptr, 0, opt, set, false, doc_ids, n, out);
+    return import_host(HostEntry::DOCSET_READ, set, nullptr, 0, nullptr, 0, doc_ids, n, opt, out);
 }
 
 lb_status lb_import_batch_device(const uint8_t* d_bytes, const uint64_t* offsets, const uint32_t* blob_lens,
@@ -1811,19 +1842,15 @@ lb_status lb_doc_status(const lb_batch* b, size_t doc, lb_import_status* out) {
     return LB_OK;
 }
 
-lb_status lb_doc_vv(const lb_batch* b, size_t doc, const lb_id_span** spans, size_t* n) {
+// document doc's spans of kind k (b->spans: 2 the vv, 3 the frontiers)
+static lb_status doc_spans(const lb_batch* b, int k, size_t doc, const lb_id_span** spans, size_t* n) {
     if (!b || !spans || !n || doc >= b->n_docs) { g_last_error = "bad argument"; return LB_ERR_INVALID_ARG; }
-    *spans = b->spans[2].data() + b->span_off[2][doc];
-    *n = b->span_off[2][doc + 1] - b->span_off[2][doc];
+    *spans = b->spans[k].data() + b->span_off[k][doc];
+    *n = b->span_off[k][doc + 1] - b->span_off[k][doc];
     return LB_OK;
 }
-
-lb_status lb_doc_frontiers(const lb_batch* b, size_t doc, const lb_id_span** spans, size_t* n) {
-    if (!b || !spans || !n || doc >= b->n_docs) { g_last_error = "bad argument"; return LB_ERR_INVALID_ARG; }
-    *spans = b->spans[3].data() + b->span_off[3][doc];
-    *n = b->span_off[3][doc + 1] - b->span_off[3][doc];
-    return LB_OK;
-}
+lb_status lb_doc_vv(const lb_batch* b, size_t doc, const lb_id_span** spans, size_t* n) { return doc_spans(b, 2, doc, spans, n); }
+lb_status lb_doc_frontiers(const lb_batch* b, size_t doc, const lb_id_span** spans, size_t* n) { return doc_spans(b, 3, doc, spans, n); }
 
 lb_status lb_doc_json(const lb_batch* cb, size_t doc, const char** utf8, size_t* len) {
     lb_batch* b = const_cast<lb_batch*>(cb);
@@ -1832,21 +1859,11 @@ lb_status lb_doc_json(const lb_batch* cb, size_t doc, const char** utf8, size_t*
     if (b->json_thread.joinable()) {
         b->json_thread.join();
         if (!b->json_ok) { g_last_error = "json d2h failed"; return LB_ERR_CUDA; }
-        b->json_fetched = true;
     }
-    if (!b->json_fetched) {
-        b->json = (char*)lbstage::host_cache().take(b->json_total + 1);
-        if (!b->json) { g_last_error = "out of host memory"; return LB_ERR_OOM; }
-        if (b->json_total && !lbstage::download(b->d_json, (u8*)b->json, b->json_total, b->dev.stream)) {
-            g_last_error = "json d2h failed";
-            return LB_ERR_CUDA;
-        }
-        b->json[b->json_total] = 0;
-        b->json_fetched = true;
-    }
+    if (lb_status s = b->json.fetch(b->dev.stream, "json d2h failed")) return s;
     const DocInfo& di = b->docs[doc];
     if (di.code != DOC_OK) { *utf8 = ""; *len = 0; return LB_OK; }
-    *utf8 = b->json + di.json_off;
+    *utf8 = b->json.host + di.json_off;
     *len = di.json_len;
     return LB_OK;
 }
@@ -1855,24 +1872,16 @@ lb_status lb_doc_attribution(const lb_batch* cb, size_t doc, const char** utf8, 
     lb_batch* b = const_cast<lb_batch*>(cb);
     if (!b || !utf8 || !len || doc >= b->n_docs) { g_last_error = "bad argument"; return LB_ERR_INVALID_ARG; }
     if (!(b->flags & LB_FLAG_ATTRIBUTION)) { g_last_error = "batch was imported without LB_FLAG_ATTRIBUTION"; return LB_ERR_INVALID_ARG; }
-    if (!b->attr_fetched) {   // one download of the whole buffer
+    if (!b->attr.fetched) {   // the offsets, then the text: one download of each
         b->attr_off.assign(b->n_docs + 1, 0);
         if (cudaMemcpy(b->attr_off.data(), b->d_attr_off, sizeof(u64) * (b->n_docs + 1), cudaMemcpyDeviceToHost) != cudaSuccess) {
             g_last_error = "attribution d2h failed";
             return LB_ERR_CUDA;
         }
-        const u64 total = b->attr_off[b->n_docs];
-        b->attr = (char*)lbstage::host_cache().take(total + 1);
-        if (!b->attr) { g_last_error = "out of host memory"; return LB_ERR_OOM; }
-        if (total && !lbstage::download(b->d_attr, (u8*)b->attr, total, b->dev.stream)) {
-            g_last_error = "attribution d2h failed";
-            return LB_ERR_CUDA;
-        }
-        b->attr[total] = 0;
-        b->attr_fetched = true;
     }
+    if (lb_status s = b->attr.fetch(b->dev.stream, "attribution d2h failed")) return s;
     if (b->docs[doc].code != DOC_OK) { *utf8 = ""; *len = 0; return LB_OK; }
-    *utf8 = b->attr + b->attr_off[doc];
+    *utf8 = b->attr.host + b->attr_off[doc];
     *len = b->attr_off[doc + 1] - b->attr_off[doc];
     return LB_OK;
 }
@@ -1963,16 +1972,8 @@ lb_status lb_doc_export_updates(const lb_batch* cb, size_t doc, const lb_id_span
     }
     const XDoc& x = b->xdocs[doc];
     if ((x.flags & 1) || x.exp_len == 0) { g_last_error = ERR_NOT_COVERED; return LB_ERR_UNSUPPORTED; }
-    if (!b->export_fetched) {
-        b->exported = (uint8_t*)lbstage::host_cache().take(b->export_total + 1);
-        if (!b->exported) { g_last_error = "out of host memory"; return LB_ERR_OOM; }
-        if (b->export_total && !lbstage::download(b->d_export, b->exported, b->export_total, b->dev.stream)) {
-            g_last_error = "export d2h failed";
-            return LB_ERR_CUDA;
-        }
-        b->export_fetched = true;
-    }
-    *bytes = b->exported + x.exp_off;
+    if (lb_status s = b->exported.fetch(b->dev.stream, "export d2h failed")) return s;
+    *bytes = (const uint8_t*)b->exported.host + x.exp_off;
     *len = x.exp_len;
     return LB_OK;
 }
@@ -2028,19 +2029,19 @@ lb_status lb_debug_table(const lb_batch* b, const char* name, void* dst, size_t 
     size_t n = 0, es = 0;
     const BatchTables& t = b->tb;
 #define TAB(str, ptr, cnt) if (nm == str) { src = ptr; n = cnt; es = sizeof(*ptr); }
-    TAB("op_cid", t.op_cid, b->n_rows) TAB("op_prop", t.op_prop, b->n_rows) TAB("op_vtype", t.op_vtype, b->n_rows)
-    TAB("op_len", t.op_len, b->n_rows) TAB("op_counter", t.op_counter, b->n_rows)
-    TAB("ch_counter", t.ch_counter, b->n_changes) TAB("ch_len", t.ch_len, b->n_changes)
-    TAB("ch_lamport", t.ch_lamport_wire, b->n_changes) TAB("ch_ts", t.ch_ts, b->n_changes)
-    TAB("dep_peer", t.dep_peer_idx, b->n_deps) TAB("dep_counter", t.dep_counter, b->n_deps)
+    TAB("op_cid", t.op_cid, b->n.rows) TAB("op_prop", t.op_prop, b->n.rows) TAB("op_vtype", t.op_vtype, b->n.rows)
+    TAB("op_len", t.op_len, b->n.rows) TAB("op_counter", t.op_counter, b->n.rows)
+    TAB("ch_counter", t.ch_counter, b->n.changes) TAB("ch_len", t.ch_len, b->n.changes)
+    TAB("ch_lamport", t.ch_lamport_wire, b->n.changes) TAB("ch_ts", t.ch_ts, b->n.changes)
+    TAB("dep_peer", t.dep_peer_idx, b->n.deps) TAB("dep_counter", t.dep_counter, b->n.deps)
 #undef TAB
     if (nm == "blk_doc" || nm == "blk_nchanges") {   // fields of the block descriptors
-        *n_elems = b->n_blocks;
+        *n_elems = b->n.blocks;
         *elem_size = 4;
         if (dst) {
-            if (dst_bytes < b->n_blocks * 4) { g_last_error = "buffer too small"; return LB_ERR_INVALID_ARG; }
-            std::vector<BlockInfo> hb(b->n_blocks);
-            if (b->n_blocks && cudaMemcpy(hb.data(), b->tb.blocks, sizeof(BlockInfo) * b->n_blocks, cudaMemcpyDeviceToHost) != cudaSuccess) return LB_ERR_CUDA;
+            if (dst_bytes < b->n.blocks * 4) { g_last_error = "buffer too small"; return LB_ERR_INVALID_ARG; }
+            std::vector<BlockInfo> hb(b->n.blocks);
+            if (b->n.blocks && cudaMemcpy(hb.data(), b->tb.blocks, sizeof(BlockInfo) * b->n.blocks, cudaMemcpyDeviceToHost) != cudaSuccess) return LB_ERR_CUDA;
             for (size_t i = 0; i < hb.size(); i++) ((u32*)dst)[i] = nm == "blk_doc" ? hb[i].doc : hb[i].n_changes;
         }
         return LB_OK;
@@ -2065,11 +2066,9 @@ void lb_batch_free(lb_batch* b) {
     if (b->ev_created) {   // the stream exists whenever the events do (init_batch)
         cudaStreamSynchronize(b->dev.stream);
         for (cudaEvent_t e : b->ev) cudaEventDestroy(e);
-        stream_give(b->device, b->dev.stream);
+        stream_give(b->dev.device, b->dev.stream);
     }
-    lbstage::host_cache().give(b->json);
-    lbstage::host_cache().give(b->exported);
-    lbstage::host_cache().give(b->attr);
+    for (HostResult* r : {&b->json, &b->attr, &b->exported}) lbstage::host_cache().give(r->host);
     delete b;
 }
 
