@@ -1,7 +1,7 @@
 """Value-edge and nesting documents, and the comparisons every one of them goes through: state JSON, vv, frontiers and
 status; the re-export (all updates, from versions, in range); JSON updates under both peer-compression settings;
-attribution; the state at a mid-history checkout; a docset that imports the document in two halves.  Shared by
-test_values_emu.py and test_values_gpu.py.
+attribution; the state at a mid-history checkout; cursors; a docset that imports the document in two halves.  Shared
+by test_values_emu.py and test_values_gpu.py, and by the width cases of width_checks.py.
 
 Each case is one document of two commits by two peers; the first commit is its "middle" (checkout frontiers, the end of
 the docset's first half)."""
@@ -15,6 +15,7 @@ from . import json_updates_checks as jc
 from . import range_export_checks as rc
 from .attribution_checks import attribution_at
 from .checkout_checks import json_at, oracle_doc
+from .cursor_checks import cursor_pos_ref, sample_cursors, seq_containers
 from .engine_checks import check_batch_against_oracle
 from .export_checks import check_export_against_oracle, check_export_from_versions
 
@@ -23,8 +24,9 @@ UNSUPPORTED = 5
 
 
 class Case:
-    def __init__(self, name, blob, mid_frontiers, half1, half2):
+    def __init__(self, name, blob, mid_frontiers, half1, half2, cursors=()):
         self.name, self.blob, self.mid, self.half1, self.half2 = name, blob, mid_frontiers, half1, half2
+        self.cursors = list(cursors)   # [(container, id | None, side)] asked besides the sampled ones
 
 
 def two_commits(name, first, second, peers=(0x1234, 0xFEDCBA9876543210)):
@@ -301,7 +303,29 @@ def check_cases(cases, lib_path=None):
     for k, (c, r) in enumerate(zip(cases, refs)):
         assert at.status(k).code == 0, (c.name, at.status(k))
         assert at.json_bytes(k) == json_at(r, c.mid), c.name
+    answers = check_cursors(cases, refs, lib_path)
     check_docset_halves(cases, lib_path)
+    return answers
+
+
+def check_cursors(cases, refs, lib_path=None, k=80):
+    """k cursors sampled over every Text / List container of each case, and the case's own cursors, against the
+    reference field by field; returns each case's [(cursor, answer)]"""
+    batch = loro_b200.import_batch([c.blob for c in cases], flags=api.LB_FLAG_CURSORS, lib_path=lib_path)
+    rnd = random.Random(9)
+    reqs, want = [], []
+    for i, (c, r) in enumerate(zip(cases, refs)):
+        cids = sorted(seq_containers(r))
+        cs = (sample_cursors(rnd, cids, r.oplog_vv(), k) if cids else []) + c.cursors
+        reqs += [(i,) + x for x in cs]
+        want += cursor_pos_ref(r, cs)
+    got = batch.cursor_pos(reqs)
+    bad = [(cases[q[0]].name, q, g, w) for q, g, w in zip(reqs, got, want) if g != w]
+    assert not bad, (len(bad), bad[:6])
+    out = [[] for _ in cases]
+    for q, g in zip(reqs, got):
+        out[q[0]].append((q[1:], g))
+    return out
 
 
 def check_docset_halves(cases, lib_path=None):
